@@ -1,19 +1,20 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's headline metric on B200: giga-FMA-instructions/s (and TFLOP/s) of the
+"""bench.py -- BASELINE.json's headline metric on H100: giga-FMA-instructions/s (and TFLOP/s) of the
 FlashAttention forward at N=4096, D=128, bf16 in / fp32 out.
 
 One "step" = one pass of the hot path over one batch of synthetic input: H independent single-head
 (N=4096, D=128) problems per GPU, one kernel launch (the reference is single-head; independent heads
-are the only thing that scales, SURVEY.md section 8(e)).  Work model is the reference's:
+are the only thing that scales).  Work model is the reference's:
 (2D+5)*N^2 FMA-instructions per head forward (README.md:108-124; SquareAttentionTest.swift:742-756);
 TFLOP/s counts the two GEMMs only, 4*N^2*D per head.
 
     python bench.py --gpus 1 --steps 50 --warmup 5            # our arm
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 1   # the reference's CPU path (oracle port)
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
+    python bench.py --gpus 1 --steps 20 --warmup 3 --dump-outputs DIR   # + what the last timed step computed, as .npy
 
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.  Inputs
-for one step (Q,K,V = 192 MiB at H=64) exceed the 126 MB L2 and two buffer sets alternate between steps.
+for one step (Q,K,V = 192 MiB at H=64) exceed the 50 MB L2 and two buffer sets alternate between steps.
 `e2e` goes through the C ABI's host-buffer entry point (mfa_attention_run_host: pinned host Q,K,V -> device,
 kernel, O and L -> host) inside the timed region; the host buffers come from mfa_host_alloc (page-locked, on the
 GPU's NUMA node) and every rank pins itself to its GPU's socket first.
@@ -22,8 +23,8 @@ Further legs on the same JSON line (none of them replaces `value`):
   sustained  the same step looped for >= 2 s: the power-capped regime, fraction against bf16_tflops_sustained
   config5    BASELINE.json configs[4] as written: 64 x 32 = 2048 independent (N=4096, D=128) problems block-partitioned
              over the ranks; data starts on rank 0 (NCCL send/recv scatter), O and L end on rank 0 (gather); kernel
-             time and the scatter / gather times are reported separately (SURVEY.md section 8(d)/(e))
-  single_head one problem per call (split-KV across the SMs, merged inside the kernel)
+             time and the scatter / gather times are reported separately
+  single_head one problem per call (32 CTAs of 128 query rows: latency, not throughput)
 """
 import argparse
 import json
@@ -41,10 +42,11 @@ FMA_PER_HEAD = (2 * D_HEAD + 5) * N_SEQ * N_SEQ          # reference's forward w
 FLOP_PER_HEAD = 4 * N_SEQ * N_SEQ * D_HEAD               # two GEMMs
 METRIC = "giga-FMA-instr/sec forward attn N=4096 D=128 bf16"
 UNIT = "GINSTRS"
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu capture
-# (profiles/), for the default H; None until a capture exists.
-NCU_TRAFFIC_BYTES_PER_LAUNCH = 298728960  # profiles/r2_fwd_ncu_summary.csv: 201.77 MB read + 96.96 MB written
-NCU_TRAFFIC_SOURCE = "profiles/r2_fwd_ncu_summary.csv (ncu --set full, one 64-head launch of this kernel; not re-measured in this run)"
+# DRAM traffic per launch of the forward kernel: not measured on H100 (no profiler capture exists for these kernels)
+NCU_TRAFFIC_BYTES_PER_LAUNCH = None
+NCU_TRAFFIC_SOURCE = "not measured"
+# NVIDIA H100 SXM data sheet: dense BF16 tensor throughput at a 700 W power limit (a data-sheet figure, not a measurement)
+H100_BF16_DENSE_TFLOPS = 989.0
 
 
 def measured_peaks():
@@ -53,7 +55,7 @@ def measured_peaks():
         with open(path) as f:
             peaks = json.load(f)
         return float(peaks["bf16_tflops"]), float(peaks.get("bf16_tflops_sustained", peaks["bf16_tflops"])), "measured"
-    return 1590.0, 1400.0, "fallback"   # /opt/skills/guides/B200_PROFILING.md
+    return H100_BF16_DENSE_TFLOPS, H100_BF16_DENSE_TFLOPS, "fallback"
 
 
 class ClockSampler:
@@ -275,6 +277,23 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
+# O of a few heads (a fixed, seeded choice) and L of all heads: 16 MiB + 1 MiB at the default H = 64
+DUMP_O_HEADS = 8
+
+
+def dump_outputs(directory, bufs, Op, np, torch):
+    """Writes the arrays a caller of the timed path receives from its last step: O (FP32, sampled by head) and L (FP32),
+    plus the sampled head indices, so that two builds can be compared output for output on identical inputs."""
+    torch.cuda.synchronize()
+    os.makedirs(directory, exist_ok=True)
+    H = bufs[Op.O].shape[0]
+    heads = np.sort(np.random.default_rng(0).choice(H, size=min(DUMP_O_HEADS, H), replace=False))
+    index = torch.from_numpy(heads).to(bufs[Op.O].device)
+    np.save(os.path.join(directory, "O.npy"), bufs[Op.O].index_select(0, index).cpu().numpy().astype(np.float32))
+    np.save(os.path.join(directory, "L.npy"), bufs[Op.L].cpu().numpy().astype(np.float32))
+    np.save(os.path.join(directory, "O_heads.npy"), heads.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -288,6 +307,9 @@ def main():
     ap.add_argument("--no-sustained", action="store_true")
     ap.add_argument("--sustained-seconds", type=float, default=2.0)
     ap.add_argument("--config5-heads", type=int, default=2048, help="batch 64 x heads 32 of BASELINE.json configs[4]")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (a fixed sample of O, all of L) as "
+                         "DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -304,7 +326,7 @@ def main():
     import torch.distributed as dist
     import mfa_b200 as mfa   # raises if libmfa_b200.so is missing: there is no fallback path
 
-    assert torch.cuda.is_available(), "bench.py (our arm) needs a B200"
+    assert torch.cuda.is_available(), "bench.py (our arm) needs an H100"
     torch.cuda.set_device(local_rank)
     # this rank's host threads (and everything it allocates from here on: pinned staging buffers, NCCL proxies) stay on
     # the socket its GPU hangs off -- the H2D / D2H copies of the e2e leg never cross the inter-socket link
@@ -371,6 +393,8 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         elapsed_ms = float(t.item())
     ms_per_step = elapsed_ms / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, sets[(args.steps - 1) & 1], Op, np, torch)
     total_heads = H * world
     value = FMA_PER_HEAD * total_heads / (ms_per_step * 1e-3) / 1e9
     tflops = FLOP_PER_HEAD * total_heads / (ms_per_step * 1e-3) / 1e12
@@ -423,7 +447,7 @@ def main():
             mfa.hostFree(addr)
 
     # ---- literal single-head latency (BASELINE.json configs[1] as written): one (N=4096, D=128) problem per launch;
-    #      too few tiles to fill 148 SMs, so the library splits the key axis across SMs and merges (split-KV) --------
+    #      32 CTAs of 128 query rows: too few to fill the 132 SMs, so this leg measures latency --------
     single_head = None
     if rank == 0:
         d1 = mfa.AttentionDescriptor()
@@ -489,7 +513,7 @@ def main():
         "bound": "tensor", "achieved": per_gpu_tflops, "peak": peak_burst, "unit": "TFLOP/s",
         "frac": per_gpu_tflops / peak_burst, "traffic": NCU_TRAFFIC_BYTES_PER_LAUNCH,
         "peak_kind": f"{peak_kind} cuBLAS bf16 burst (MEASURED_PEAKS.json)" if peak_kind == "measured"
-                     else "fallback 1590 TF/s (B200_PROFILING.md)",
+                     else "H100 SXM data sheet, dense BF16, 700 W (989 TF/s; not measured)",
         "kernel": kernel.sourceName(), "flops_per_launch": FLOP_PER_HEAD * H,
         "kernel_ms": ms_per_step, "algorithmic_bytes_per_launch": H * (3 * N_SEQ * D_HEAD * 2 + N_SEQ * D_HEAD * 4 + N_SEQ * 4),
         "traffic_source": NCU_TRAFFIC_SOURCE,
@@ -519,7 +543,7 @@ def main():
                                "N=4096 D=128, bf16 Q/K/V, fp32 O and L (BASELINE.json configs[1] x heads)",
                    "seq_len": N_SEQ, "head_dim": D_HEAD, "heads_per_gpu_per_step": H,
                    "parallelism": f"heads sharded over {world} GPU(s), no data-path collective",
-                   "l2": "inputs per step (192 MiB at H=64) exceed the 126 MB L2; two buffer sets alternate"},
+                   "l2": "inputs per step (192 MiB at H=64) exceed the 50 MB L2; two buffer sets alternate"},
         "clocks": sampler.summary(), "e2e": e2e, "gpu_launches": args.steps * launches_per_step,
         "roofline": roofline, "cpu_baseline": cpu_baseline, "single_head": single_head,
         "sustained": sustained, "config5": config5, "numa_node": numa_node,

@@ -1,5 +1,5 @@
 /*
- * mfa_b200.h -- C ABI of the B200-native FlashAttention hot path that stands in for
+ * mfa_b200.h -- C ABI of the H100-native FlashAttention hot path that stands in for
  * philipturner/metal-flash-attention's attention path.
  *
  * The reference's boundary is a set of Swift value types that *describe* a kernel and hand the
@@ -7,7 +7,7 @@
  * dispatches (Tests/FlashAttentionTests/Attention/SquareAttentionTest.swift:226-380).  This
  * header keeps that shape 1:1 (same names, same fields, same validation rules) and moves the
  * part the reference leaves to its caller -- compile + bind + dispatch -- behind
- * mfa_attention_kernel_encode(), because on B200 the kernels are pre-compiled sm_100a CUDA.
+ * mfa_attention_kernel_encode(), because on H100 the kernels are pre-compiled sm_90a CUDA.
  *
  * Conventions
  *   - Plain C: pointers, sizes, enums with fixed raw values.  No torch / C++ types.
@@ -20,10 +20,10 @@
  *     host pointers and performs H2D -> kernels -> D2H itself.
  *   - A kernel handle is immutable after creation and may be encoded concurrently from several
  *     threads / streams.
- *   - There is NO CPU fallback: if no sm_100 device / driver is present, encode fails loudly
+ *   - There is NO CPU fallback: if no sm_90 device / driver is present, encode fails loudly
  *     with MFA_ERROR_NO_DEVICE.
  *
- * Reference citations use R/ = /root/reference/Sources/FlashAttention/.
+ * Reference citations use R/ = the reference's Sources/FlashAttention/.
  */
 #ifndef MFA_B200_H
 #define MFA_B200_H
@@ -50,15 +50,15 @@ typedef enum mfa_status {
   MFA_ERROR_INVALID_ARGUMENT = -2,      /* NULL pointer, enum out of range, operand without a buffer */
   MFA_ERROR_UNEXPECTED_OPERAND = -3,    /* "Unexpected operand: X"  AttentionDescriptor.swift:69-74 */
   MFA_ERROR_INVALID_PRECISIONS = -4,    /* "Invalid precisions."  AttentionKernel.swift:90-105 */
-  MFA_ERROR_UNSUPPORTED = -5,           /* shape outside what the sm_100a kernels cover (e.g. head > 512) */
-  MFA_ERROR_NO_DEVICE = -6,             /* no CUDA device / not sm_100 -- never falls back to a CPU path */
+  MFA_ERROR_UNSUPPORTED = -5,           /* shape outside what the sm_90a kernels cover (e.g. head > 512) */
+  MFA_ERROR_NO_DEVICE = -6,             /* no CUDA device / not sm_90 -- never falls back to a CPU path */
   MFA_ERROR_CUDA = -7                   /* a CUDA runtime / driver call failed; message has the detail */
 } mfa_status_t;
 
 /** Thread-local, NUL-terminated description of the last error on the calling thread. */
 MFA_API const char *mfa_last_error(void);
 
-/** Library version / build info ("mfa_b200 x.y sm_100a"). */
+/** Library version / build info ("mfa_b200 x.y sm_90a"). */
 MFA_API const char *mfa_version(void);
 
 /* ------------------------------------------------------------------------------------------ */
@@ -108,14 +108,14 @@ typedef struct mfa_attention_descriptor {
   uint32_t column;                     /* matrixDimensions.column (input sequence length C)  */
   uint16_t head;                       /* matrixDimensions.head   (head dimension D)         */
   uint8_t transpose_Q, transpose_K, transpose_V, transpose_O; /* transposeState :22 */
-  /* ---- B200 extensions; all-zero reproduces the reference exactly ---- */
+  /* ---- library extensions; all-zero reproduces the reference exactly ---- */
   uint8_t input_precision_override;    /* 0: reference policy (Q,K,V FP16 and dO BF16 when lowPrecisionInputs,
                                           AttentionDescriptor+Precisions.swift:13-23);
                                           MFA_BF16 (2): Q,K,V,dO are all BF16 in memory (north_star asks for bf16);
                                           MFA_FP16 (1): Q,K,V,dO are all FP16.
                                           Only meaningful with low_precision_inputs.  All three variants run on the
                                           tensor-core kernels (with the reference policy the backward kernels rewrite
-                                          the staged BF16 dO tiles as FP16 on chip: tcgen05 kind::f16 cannot mix
+                                          the staged BF16 dO tiles as FP16 on chip: wgmma cannot mix
                                           FP16 and BF16 operands in one MMA). */
   uint8_t reserved0;
   uint32_t batch_count;                /* 0 or 1: single head (reference). N > 1: N independent
@@ -140,7 +140,7 @@ MFA_API int mfa_attention_descriptor_register_precision(const mfa_attention_desc
 /* ------------------------------------------------------------------------------------------ */
 typedef enum mfa_backend {
   MFA_BACKEND_SIMT_FP32 = 0, /* CUDA-core FP32 FMA kernels: any R, C, D <= 512, any transposes/precisions */
-  MFA_BACKEND_TCGEN05 = 1    /* TMA + tcgen05.mma + TMEM kernels: 16-bit inputs, D % 8 == 0; forward D <= 256 (transposed
+  MFA_BACKEND_TCGEN05 = 1    /* TMA + wgmma kernels: 16-bit inputs, D % 8 == 0; forward D <= 256 (transposed
                                 operands too, where the transposed row pitch is a multiple of 16 bytes), backward D <= 128
                                 row-major */
 } mfa_backend_t;
@@ -150,7 +150,7 @@ typedef struct mfa_attention_kernel_descriptor {
   uint8_t has_block_dimensions;
   uint16_t block_parallelization, block_traversal, block_head;
   /* cacheState: bit i set <=> operand i is kept resident on chip for the whole traversal
-     (registers on Apple GPUs; SMEM / TMEM / registers on B200).                      :12    */
+     (registers on Apple GPUs; SMEM / registers on H100).                      :12    */
   uint16_t cache_state_valid_mask; /* which operands have an entry at all */
   uint16_t cache_state_mask;
   /* headDimension                                                                    :15    */
@@ -167,15 +167,15 @@ typedef struct mfa_attention_kernel_descriptor {
   uint16_t transpose_state_mask;
   /* type; 0xFF = nil                                                                 :44    */
   uint8_t type;
-  /* ---- B200 extension: which sm_100a kernel family the heuristic picked ---- */
+  /* ---- library extension: which sm_90a kernel family the heuristic picked ---- */
   uint8_t backend; /* mfa_backend_t */
-  /* ---- B200 extension: the tuning columns of the parameter-table row (tcgen05 family).  Like blockDimensions they
-     are plain data the caller may edit before AttentionKernel(descriptor:); kernel creation accepts every value that has
-     a compiled instantiation (exp2_fma_quarters <= mfa_max_exp2_fma_quarters(type)) and rejects the rest. ---- */
-  uint8_t exp2_fma_quarters; /* of every 4 element pairs of P, how many take exp2 on the FMA pipe (Cody-Waite +
-                                polynomial) instead of the MUFU pipe: selects the kernel instantiation */
-  uint8_t split_min_blocks;  /* small grids: a traversal range handed to one CTA has at least this many 128-key (or
-                                128-query) blocks; 0 = never split */
+  /* ---- library extension: the tuning columns of the parameter-table row (tensor-core family).  Like blockDimensions
+     they are plain data the caller may edit before AttentionKernel(descriptor:); kernel creation accepts
+     exp2_fma_quarters <= mfa_max_exp2_fma_quarters(type) and rejects the rest. ---- */
+  uint8_t exp2_fma_quarters; /* of every 4 element pairs of P, how many should take exp2 on the FMA pipe; validated and
+                                carried -- the sm_90a kernels take every exp2 on the MUFU pipe */
+  uint8_t split_min_blocks;  /* small grids: a traversal range handed to one CTA has at least this many traversal
+                                blocks (blockDimensions.traversal rows each); 0 = never split */
   uint8_t split_max;         /* small grids: at most this many ranges per tile (forward <= 16, backward <= 8) */
 } mfa_attention_kernel_descriptor_t;
 
@@ -200,21 +200,22 @@ MFA_API int mfa_attention_descriptor_kernel_descriptor(const mfa_attention_descr
 
 /** The parameter table text that kernelDescriptor(type:) would parse for this descriptor -- the analogue of
  *  AttentionDescriptor.parameterFile(type:) (AttentionDescriptor+Parameters.swift:13-39).  Rows are the reference's
- *  "| maxD | par | trav | head | cached |" with, for the tcgen05 family, three B200 tuning columns appended:
+ *  "| maxD | par | trav | head | cached |" with, for the tcgen05 family, three tuning columns appended:
  *  "| exp2 on the FMA pipe (quarters) | min blocks per split | max splits |".  The returned pointer stays valid until
  *  the table is replaced. */
 MFA_API const char *mfa_attention_descriptor_parameter_file(const mfa_attention_descriptor_t *descriptor,
                                                             mfa_kernel_type_t type);
 
-/** The tables are DATA: this replaces the tcgen05-family table of `type` (`transposed` != 0: the table used with transposed operands, i.e. of the
+/** The tables are DATA: this replaces the tensor-core-family table of `type` (`transposed` != 0: the table used with transposed operands, i.e. of the
  *  layout-generic kernels) with `text` in the format above; NULL restores the built-in table.  The text is
  *  parsed and validated first (unknown operand names, malformed rows, tuning values without a compiled kernel are
  *  rejected and the current table stays).  Kernels fetched from the descriptor-keyed cache afterwards follow the new
  *  table.  At load time the library also reads the file named by the environment variable MFA_B200_PARAMETER_FILE
- *  (sections "[forward]", "[backwardQuery]", "[backwardKeyValue]", each also as "[....transposed]"; scripts/sweep.py writes
- *  one from measurements on the current GPU).  Not thread-safe against concurrent kernelDescriptor() calls. */
+ *  (sections "[forward]", "[backwardQuery]", "[backwardKeyValue]", each also as "[....transposed]"; parameters/h100.txt is
+ *  one).  Not thread-safe against concurrent kernelDescriptor() calls. */
 MFA_API int mfa_set_parameter_table(mfa_kernel_type_t type, int transposed, const char *text);
-/** Largest exp2_fma_quarters with a compiled instantiation for `type`. */
+/** Largest exp2_fma_quarters the tables accept for `type` (validated and carried; the sm_90a kernels take every exp2 on
+ *  the MUFU pipe). */
 MFA_API int mfa_max_exp2_fma_quarters(mfa_kernel_type_t type);
 
 /** descriptor.setFunctionConstants(_:)  (AttentionDescriptor.swift:139-148): the two launch-time
@@ -240,7 +241,7 @@ MFA_API void mfa_attention_kernel_destroy(mfa_attention_kernel_t *kernel);
 
 /** kernel.blockDimensions  (:22): out[0..2] = parallelization, traversal, head. */
 MFA_API int mfa_attention_kernel_block_dimensions(const mfa_attention_kernel_t *kernel, uint16_t out[3]);
-/** kernel.threadgroupSize  (:268-270): threads per CTA of the selected sm_100a kernel. */
+/** kernel.threadgroupSize  (:268-270): threads per CTA of the selected sm_90a kernel. */
 MFA_API int mfa_attention_kernel_threadgroup_size(const mfa_attention_kernel_t *kernel, uint32_t *out);
 /** kernel.threadgroupMemoryAllocation  (:25, 272-363): dynamic shared memory bytes per CTA. */
 MFA_API int mfa_attention_kernel_threadgroup_memory_allocation(const mfa_attention_kernel_t *kernel,
@@ -306,18 +307,14 @@ MFA_API int mfa_attention_kernel_cache_size(void);
 MFA_API int mfa_attention_run_host(const mfa_attention_descriptor_t *descriptor, uint32_t run_mask,
                                    void *const host_buffers[MFA_BUFFER_COUNT], int device);
 
-/* Host-memory placement for the host-buffer path (B200 extension; the reference's buffers are Metal shared-storage
+/* Host-memory placement for the host-buffer path (library extension; the reference's buffers are Metal shared-storage
  * buffers, MTLContext+Buffers.swift:5-45, with no placement to speak of on a unified-memory SoC). */
 /** Page-locked host buffer for mfa_attention_run_host, allocated (first-touched) on the NUMA node `device` hangs
  *  off and portable across CUDA contexts.  The calling thread's CPU affinity is unchanged on return. */
 MFA_API int mfa_host_alloc(size_t bytes, int device, void **out);
 /** The same for buffers the host only WRITES and the GPU reads (Q, K, V, dO of mfa_attention_run_host): the pages are also
  *  write-combined, so the upload's PCIe reads are not snooped through the CPU caches and the buffers do not evict the
- *  host's working set.  Reading such a buffer with the CPU is very slow: do not use it for outputs.  Measured
- *  (profiles/r2_e2e_chunks.txt): with upload buffers alone the 201 MB + 135 MB step time is unchanged within the box-to-box
- *  noise (5.7-6.5 ms on that box either way); with the OUTPUT buffers write-combined as well it was 5.10 ms in every run
- *  against 5.3-6.5 ms -- the device-to-host writes into cacheable memory are what the host's cache hierarchy slows down --
- *  but outputs a CPU cannot read at speed are not a configuration this library measures or recommends. */
+ *  host's working set.  Reading such a buffer with the CPU is very slow: do not use it for outputs. */
 MFA_API int mfa_host_alloc_upload(size_t bytes, int device, void **out);
 MFA_API int mfa_host_free(void *ptr);
 /** Restricts the calling thread to the CPUs of `device`'s NUMA node (within the affinity it already has), so that

@@ -15,7 +15,7 @@ reference's names, field meanings and failure behaviour:
     AttentionKernel                Attention/AttentionKernel/AttentionKernel.swift:11-50, 268-363
     GEMMOperandPrecision           GEMM/GEMMOperandPrecision.swift:33-61
 
-All arithmetic happens in libmfa_b200.so (hand-written sm_100a CUDA).  There is no Python or CPU
+All arithmetic happens in libmfa_b200.so (hand-written sm_90a CUDA).  There is no Python or CPU
 fallback: if the shared library is missing, importing this package raises.  Where the reference traps
 with fatalError(...), this mirror raises MFAError carrying the same message.
 """
@@ -179,7 +179,7 @@ def releaseDeviceResources(device: int = 0) -> None:
 
 
 def setParameterTable(type: "AttentionKernelType", text: Optional[str], transposed: bool = False) -> None:
-    """mfa_set_parameter_table: replace (text) or restore (None) the tcgen05-family parameter table of `type`."""
+    """mfa_set_parameter_table: replace (text) or restore (None) the tensor-core-family parameter table of `type`."""
     _check(_lib.mfa_set_parameter_table(int(type), int(bool(transposed)),
                                         None if text is None else text.encode()))
 
@@ -260,7 +260,7 @@ class AttentionDescriptor:
         self.lowPrecisionIntermediates: bool = False
         self.matrixDimensions: Optional[Tuple[int, int, int]] = None
         self.transposeState: Optional[Tuple[bool, bool, bool, bool]] = None
-        # B200 extensions (include/mfa_b200.h): None = reference policy (FP16 inputs).
+        # library extensions (include/mfa_b200.h): None = reference policy (FP16 inputs).
         self.inputPrecisionOverride: Optional[GEMMOperandPrecision] = None
         self.batchCount: int = 1
 
@@ -439,7 +439,7 @@ class AttentionKernelDescriptor:
     def backend(self, value):
         self._c.backend = int(value)
 
-    # ---- B200 extension: the tuning columns of the parameter-table row (plain, editable data like blockDimensions)
+    # ---- library extension: the tuning columns of the parameter-table row (plain, editable data like blockDimensions)
     @property
     def exp2FmaQuarters(self) -> int:
         """Of every 4 element pairs of P, how many take exp2 on the FMA pipe: selects the kernel instantiation."""

@@ -1,8 +1,8 @@
-// AttentionDescriptor side of the C ABI: precision policy, B200 parameter tables, and the
+// AttentionDescriptor side of the C ABI: precision policy, H100 parameter tables, and the
 // descriptor -> kernel-descriptor heuristic.  Mirrors (does not copy) the reference's
 //   Sources/FlashAttention/Attention/AttentionDescriptor/AttentionDescriptor.swift
 //   .../AttentionDescriptor+Precisions.swift, +Parameters.swift, AttentionParameterRow.swift
-// The tables hold B200 tile shapes and on-chip residency instead of Apple register-cache choices.
+// The tables hold H100 tile shapes and on-chip residency instead of Apple register-cache choices.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -12,7 +12,7 @@
 #include "internal.h"
 
 namespace mfa {
-constexpr int kTableSlots = 6;  // parameter tables of the tcgen05 family (see table_slot)
+constexpr int kTableSlots = 6;  // parameter tables of the tensor-core family (see table_slot)
 
 thread_local std::string g_last_error;
 
@@ -49,9 +49,9 @@ int memory_precision(const mfa_attention_descriptor_t &d, int operand) {
   }
 }
 
-// registerPrecisions (AttentionDescriptor+Precisions.swift:149-215).  B200 has native BF16
+// registerPrecisions (AttentionDescriptor+Precisions.swift:149-215).  H100 has native BF16
 // conversion, so the `hasNativeBF16Casting` (Apple9) branch applies.  `type` selects the kernel whose registers are
-// described: the precision of P and dS depends on the kernel family that serves (descriptor, type) -- on the tcgen05
+// described: the precision of P and dS depends on the kernel family that serves (descriptor, type) -- on the tensor-core
 // family they are operands of a tensor-core MMA and therefore ALWAYS carried in the 16-bit input element type, whatever
 // lowPrecisionIntermediates says (the reference keeps them in FP32 registers when that flag is off, :203-205; this is a
 // documented deviation, DESIGN.md section 3, and the descriptor reports what the kernel really does).
@@ -68,18 +68,18 @@ int register_precision_for(const mfa_attention_descriptor_t &d, int operand, int
     case MFA_D:
       return d.low_precision_intermediates ? MFA_BF16 : MFA_FP32;
     case MFA_S:
-      // :197  S accumulates in FP16 only when both flags are set.  B200 tensor cores always
-      // accumulate S in FP32 in TMEM, which is the more accurate of the two; report FP32.
+      // :197  S accumulates in FP16 only when both flags are set.  H100 tensor cores always
+      // accumulate S in FP32 (wgmma accumulators), which is the more accurate of the two; report FP32.
       return MFA_FP32;
     case MFA_P:
-      // :198  P is a 16-bit value under lowPrecisionIntermediates; on the tcgen05 family it is always rounded to the
+      // :198  P is a 16-bit value under lowPrecisionIntermediates; on the tensor-core family it is always rounded to the
       // input element type (it is the A operand of O += P V, dV += P^T dO)
       if (tensorCore || d.low_precision_intermediates) return bf16Inputs ? MFA_BF16 : MFA_FP16;
       return MFA_FP32;
     case MFA_dP:
       return MFA_FP32;  // :199
     case MFA_dS:
-      // :200  BF16 under lowPrecisionIntermediates (Apple9); on the tcgen05 family the A operand of dQ += dS K,
+      // :200  BF16 under lowPrecisionIntermediates (Apple9); on the tensor-core family the A operand of dQ += dS K,
       // dK += dS^T Q, in the input element type
       if (tensorCore) return bf16Inputs ? MFA_BF16 : MFA_FP16;
       return d.low_precision_intermediates ? MFA_BF16 : MFA_FP32;
@@ -96,52 +96,48 @@ int register_precision(const mfa_attention_descriptor_t &d, int operand) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// B200 parameter tables.  Same text format as the reference's "parameter file"
+// H100 parameter tables.  Same text format as the reference's "parameter file"
 // (AttentionDescriptor+Parameters.swift:106-285):
 //     | max head dimension | parallelization | traversal | head block | resident operands |
 // First row with D <= max wins (:41-66); past the end, the last row applies.
-//   * tcgen05 family: parallelization = Q (or K/V) rows per CTA (two 128-row tcgen05 M-tiles for the
-//     forward ping-pong), traversal = keys per pipeline stage, head block = the whole padded head
-//     dimension (TMEM holds the accumulators, no D-blocking needed up to 256), resident = operands that
-//     stay in SMEM/TMEM for the entire traversal.
+//   * tensor-core family: parallelization = Q (or K/V) rows per CTA, traversal = keys (queries) per pipeline
+//     stage, head block = the padded head dimension (accumulators in registers up to 256), resident = operands
+//     that stay in shared memory / registers for the entire traversal.
 //   * SIMT family: 64 x 64 blocks, 32-wide head chunks, accumulators resident in registers.
 // ------------------------------------------------------------------------------------------------
-// tcgen05 rows carry three B200 tuning columns after the reference's five:
+// Tensor-core rows carry three tuning columns after the reference's five:
 //     | exp2 on the FMA pipe (quarters of the element pairs) | min blocks per split | max splits |
-// (measured values: scripts/sweep.py regenerates them on the current GPU and writes parameters/b200.txt, which these
-// strings reproduce; the raw timings are in profiles/r2_parameter_sweep.jsonl).
+// The exp2 column is validated and carried (every exp2 of the sm_90a kernels runs on the MUFU pipe).  The split
+// columns govern small grids: the forward cuts every query tile's key axis into equal ranges of at least `min blocks`
+// key blocks and merges the partials (split-KV); the backward kernels cut their traversal axis likewise and sum the
+// partial gradients.  0 min blocks turns splitting off.
+//   forward: 128 query rows per CTA (two warpgroups); 128-key blocks up to D = 128, 64-key blocks beyond
+//   backwardQuery: 128 query rows per CTA up to D = 128, 64 beyond (one warpgroup); 64-key blocks
+//   backwardKeyValue: 128 key rows per CTA up to D = 128, 64 beyond (dK / dV columns split over two warpgroups);
+//   64-query blocks
+// Transposed operands are staged row-major first and run the same kernels.
 static const char *kForwardTcgen05 =
-    "| 64  | 256 | 128 | 64  | Q, O | 1 | 2 | 8 |\n"
-    "| 128 | 256 | 128 | 128 | Q, O | 0 | 4 | 8 |\n"
-    "| 256 | 128 | 128 | 256 | Q, O | 0 | 0 | 1 |\n"
+    "| 64  | 128 | 128 | 64  | Q, O | 0 | 2 | 8 |\n"
+    "| 128 | 128 | 128 | 128 | Q, O | 0 | 4 | 8 |\n"
+    "| 256 | 128 | 64  | 256 | Q, O | 0 | 0 | 1 |\n"
     "\n";
-// forward with transposed operands: the layout-generic kernel (one 128-row tile per CTA, 128-key blocks)
 static const char *kForwardTcgen05Transposed =
+    "| 64  | 128 | 128 | 64  | Q, O | 0 | 0 | 1 |\n"
     "| 128 | 128 | 128 | 128 | Q, O | 0 | 0 | 1 |\n"
-    "| 256 | 128 | 128 | 256 | Q, O | 0 | 0 | 1 |\n"
+    "| 256 | 128 | 64  | 256 | Q, O | 0 | 0 | 1 |\n"
     "\n";
-// (the 256 rows and the transposed tables: the layout-generic backward kernels, 64-row traversal blocks;
-// backwardKeyValue keeps one accumulator resident per pass -- dV, then dK)
 static const char *kBackwardQueryTcgen05 =
-    "| 64  | 128 | 128 | 64  | Q, dO, dQ | 1 | 2 | 8 |\n"
-    "| 128 | 128 | 128 | 128 | Q, dO, dQ | 0 | 2 | 8 |\n"
-    "| 256 | 128 | 64  | 256 | Q, dO, dQ | 0 | 2 | 8 |\n"
-    "\n";
-static const char *kBackwardKeyValueTcgen05 =
-    "| 64  | 128 | 128 | 64  | K, V, dV, dK | 2 | 2 | 8 |\n"
-    "| 128 | 128 | 128 | 128 | K, V, dV, dK | 2 | 2 | 8 |\n"
-    "| 256 | 128 | 64  | 256 | K, V, dV, dK | 0 | 2 | 8 |\n"
-    "\n";
-static const char *kBackwardQueryTcgen05Transposed =
     "| 64  | 128 | 64  | 64  | Q, dO, dQ | 0 | 2 | 8 |\n"
     "| 128 | 128 | 64  | 128 | Q, dO, dQ | 0 | 2 | 8 |\n"
-    "| 256 | 128 | 64  | 256 | Q, dO, dQ | 0 | 2 | 8 |\n"
+    "| 256 | 64  | 64  | 256 | Q, dO, dQ | 0 | 2 | 8 |\n"
     "\n";
-static const char *kBackwardKeyValueTcgen05Transposed =
+static const char *kBackwardKeyValueTcgen05 =
     "| 64  | 128 | 64  | 64  | K, V, dV, dK | 0 | 2 | 8 |\n"
     "| 128 | 128 | 64  | 128 | K, V, dV, dK | 0 | 2 | 8 |\n"
-    "| 256 | 128 | 64  | 256 | K, V, dV, dK | 0 | 2 | 8 |\n"
+    "| 256 | 64  | 64  | 256 | K, V, dV, dK | 0 | 2 | 8 |\n"
     "\n";
+static const char *kBackwardQueryTcgen05Transposed = kBackwardQueryTcgen05;
+static const char *kBackwardKeyValueTcgen05Transposed = kBackwardKeyValueTcgen05;
 static const char *kForwardSimt =
     "| 512 | 64 | 64 | 32 | O |\n"
     "\n";
@@ -153,8 +149,8 @@ static const char *kBackwardKeyValueSimt =
     "| 512 | 64 | 64 | 32 |        |\n"
     "\n";
 
-// Which kernel family can serve this descriptor.  The tcgen05 family needs 16-bit row-major operands
-// whose row pitch is a multiple of 16 bytes (TMA global-stride rule), i.e. D % 8 == 0.
+// Which kernel family can serve this descriptor.  The tensor-core family needs 16-bit operands; its kernels read
+// row-major operands with D % 8 == 0 (TMA global-stride rule), anything else is staged into that form first.
 static bool any_transpose(const mfa_attention_descriptor_t &d) {
   return d.transpose_Q || d.transpose_K || d.transpose_V || d.transpose_O;
 }
@@ -163,8 +159,8 @@ int select_backend(const mfa_attention_descriptor_t &d, int type) {
   if (!d.low_precision_inputs || d.head == 0) return MFA_BACKEND_SIMT_FP32;
   const uint32_t padded = (static_cast<uint32_t>(d.head) + 7) / 8 * 8;
   if (any_transpose(d)) {
-    // transposed operands: the layout-generic kernels, where TMA can address the transposed view (row pitch = sequence
-    // length, a multiple of 8 elements)
+    // transposed operands: staged row-major for the tensor-core kernels where the transposed view has a 16-byte row
+    // pitch (sequence length a multiple of 8 elements)
     const bool ok = type == MFA_FORWARD
                         ? tcgen05_forward_transposes_ok(d.row, d.column, d.transpose_Q, d.transpose_K, d.transpose_V)
                         : tcgen05_backward_transposes_ok(d.row, d.column, d.transpose_Q, d.transpose_K, d.transpose_V,
@@ -172,11 +168,11 @@ int select_backend(const mfa_attention_descriptor_t &d, int type) {
     if (!ok) return MFA_BACKEND_SIMT_FP32;
     if (d.head % 8 != 0) return MFA_BACKEND_SIMT_FP32;  // (head-dimension padding is implemented for row-major operands)
   }
-  // D % 8 != 0 (row-major): the operands are staged with pad8(D) columns (kernels/pad_head.cu) and the tcgen05 kernels
+  // D % 8 != 0 (row-major): the operands are staged with pad8(D) columns (kernels/pad_head.cu) and the tensor-core kernels
   // run at the padded head dimension -- the reference's zero-padded async copies (+OuterProduct.swift:237-254)
   const uint32_t maxHead = (type == MFA_FORWARD) ? tcgen05_forward_max_head() : tcgen05_backward_max_head();
   if (padded > maxHead) return MFA_BACKEND_SIMT_FP32;
-  // (the reference's own policy, FP16 Q/K/V + BF16 dO, is served too: tcgen05 kind::f16 cannot mix element types
+  // (the reference's own policy, FP16 Q/K/V + BF16 dO, is served too: wgmma cannot mix element types
   // inside one MMA, so the backward kernels rewrite the staged dO tile as FP16 in shared memory)
   return MFA_BACKEND_TCGEN05;
 }
@@ -219,7 +215,7 @@ const char *parameter_file(const mfa_attention_descriptor_t &d, int type) {
 struct ParameterRow {
   unsigned maximumHeadDimension = 0;
   std::string parallelization, traversal, head, cachedOperands;
-  // B200 tuning columns (present in the tcgen05 tables; empty = defaults)
+  // tuning columns (present in the tensor-core tables; empty = defaults)
   std::string exp2FmaQuarters, splitMinBlocks, splitMax;
 };
 
@@ -363,7 +359,7 @@ int kernel_descriptor(const mfa_attention_descriptor_t &d, int type, mfa_attenti
   }
 
   out.backend = static_cast<uint8_t>(select_backend(d, type));
-  // tuning columns (tcgen05 tables); rows without them (the FP32 family) leave the defaults: no FMA-pipe exp2, no splits
+  // tuning columns (tensor-core tables); rows without them (the FP32 family) leave the defaults: no FMA-pipe exp2, no splits
   out.exp2_fma_quarters = 0;
   out.split_min_blocks = 0;
   out.split_max = 1;
@@ -376,7 +372,7 @@ int kernel_descriptor(const mfa_attention_descriptor_t &d, int type, mfa_attenti
     out.split_min_blocks = static_cast<uint8_t>(minBlocks);
     out.split_max = static_cast<uint8_t>(maxSplits < 1 ? 1 : maxSplits);
   }
-  // preferAsyncCache / preferAsyncLoad (:118-124): "async" == TMA bulk-tensor copies on B200.
+  // preferAsyncCache / preferAsyncLoad (:118-124): "async" == TMA bulk-tensor copies on H100.
   out.prefer_async_cache = out.backend == MFA_BACKEND_TCGEN05 ? 1 : 0;
   out.prefer_async_load = out.backend == MFA_BACKEND_TCGEN05 ? 1 : 0;
 
@@ -444,7 +440,7 @@ using namespace mfa;
 extern "C" {
 
 const char *mfa_last_error(void) { return g_last_error.c_str(); }
-const char *mfa_version(void) { return "mfa_b200 0.2 (sm_100a; tcgen05+TMA+TMEM forward / dQ / dK-dV, SIMT FP32 family)"; }
+const char *mfa_version(void) { return "mfa_b200 0.3 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family)"; }
 
 int mfa_precision_size(mfa_precision_t precision) { return precision == MFA_FP32 ? 4 : 2; }
 const char *mfa_precision_name(mfa_precision_t precision) {
@@ -556,7 +552,7 @@ int mfa_set_parameter_table(mfa_kernel_type_t type, int transposed, const char *
     for (int operand : operands)  // createCacheState's check (AttentionDescriptor.swift:69-74), applied to every row
       if (!(expected & (1u << operand)))
         return fail(MFA_ERROR_UNEXPECTED_OPERAND, std::string("Unexpected operand: ") + kOperandNames[operand]);
-    if (row.exp2FmaQuarters.empty()) return fail(MFA_ERROR_INVALID_ARGUMENT, "A tcgen05 table row needs the three tuning columns.");
+    if (row.exp2FmaQuarters.empty()) return fail(MFA_ERROR_INVALID_ARGUMENT, "A tensor-core table row needs the three tuning columns.");
     uint16_t quarters = 0, minBlocks = 0, maxSplits = 0;
     if (!parse_u16(row.exp2FmaQuarters, quarters) || !parse_u16(row.splitMinBlocks, minBlocks) ||
         !parse_u16(row.splitMax, maxSplits))

@@ -45,14 +45,26 @@ static const int *operands_of(int type, int *count) {
   }
 }
 
-// sm_100 check of the current device, cached per device ordinal (encode() of a microsecond-scale kernel must not pay
+static bool is_output(int type, int slot) {
+  return type == MFA_FORWARD ? slot == MFA_O : (type == MFA_BACKWARD_QUERY ? slot == MFA_dQ : (slot == MFA_dV || slot == MFA_dK));
+}
+
+// Whether the tensor-core family copies this operand into a row-major, pad8(D)-column staging buffer: every operand
+// with a head dimension when D % 8 != 0, and any operand stored transposed (L and D are per-row vectors, never staged).
+static bool stages_operand(int type, int slot, bool padded, uint16_t transpose_mask) {
+  if (slot == MFA_L || slot == MFA_D) return false;
+  if (type == MFA_BACKWARD_KEY_VALUE && slot == MFA_O) return false;  // (not read by dK/dV)
+  return padded || ((transpose_mask >> slot) & 1);
+}
+
+// sm_90 check of the current device, cached per device ordinal (encode() of a microsecond-scale kernel must not pay
 // two runtime queries per call)
 static int check_device() {
   const int device = current_device();
   if (device < 0)
     return fail(MFA_ERROR_NO_DEVICE, "No CUDA device (cudaGetDevice failed; this library has no CPU fallback).");
   static std::mutex mutex;
-  static int8_t verdict[kMaxDevices] = {};  // 0 unknown, 1 sm_100, -1 other
+  static int8_t verdict[kMaxDevices] = {};  // 0 unknown, 1 sm_90, -1 other
   if (device < kMaxDevices) {
     std::lock_guard<std::mutex> lock(mutex);
     if (verdict[device] == 1) return MFA_SUCCESS;
@@ -60,9 +72,9 @@ static int check_device() {
   int major = 0;
   cudaError_t e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device);
   if (e != cudaSuccess) return fail(MFA_ERROR_NO_DEVICE, std::string("cudaDeviceGetAttribute: ") + cudaGetErrorString(e));
-  if (major != 10)
-    return fail(MFA_ERROR_NO_DEVICE, "Device is not sm_100 (compute capability " + std::to_string(major) +
-                                         ".x); these kernels are built for sm_100a only.");
+  if (major != 9)
+    return fail(MFA_ERROR_NO_DEVICE, "Device is not sm_90 (compute capability " + std::to_string(major) +
+                                         ".x); these kernels are built for sm_90a only.");
   if (device < kMaxDevices) {
     std::lock_guard<std::mutex> lock(mutex);
     verdict[device] = 1;
@@ -135,7 +147,7 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
   const uint32_t D = kd->head_dimension;
 
   if (k->backend == MFA_BACKEND_TCGEN05) {
-    // The tcgen05 kernels only exist for 16-bit row-major operands; reject descriptors edited into
+    // The tensor-core kernels only exist for 16-bit row-major operands; reject descriptors edited into
     // something they cannot serve instead of silently computing something else.
     const uint8_t pq = kd->memory_precisions[MFA_Q];
     const uint32_t Dp = (D + 7) / 8 * 8;  // D % 8 != 0: operands are staged with pad8(D) columns (kernels/pad_head.cu)
@@ -162,15 +174,11 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
     if (kd->exp2_fma_quarters > max_quarters) {
       delete k;
       return fail(MFA_ERROR_UNSUPPORTED, "exp2-on-FMA-pipe fraction " + std::to_string(kd->exp2_fma_quarters) +
-                                             "/4 has no compiled sm_100a kernel (available: 0.." +
+                                             "/4 has no compiled sm_90a kernel (available: 0.." +
                                              std::to_string(max_quarters) + ").");
     }
-    if (k->type == MFA_FORWARD && transposed)
-      tcgen05_forward_generic_geometry(D, &k->threads, &k->smem_bytes, &k->par, &k->trav, &k->head);
-    else if (k->type == MFA_FORWARD)
+    if (k->type == MFA_FORWARD)
       tcgen05_forward_geometry(Dp, &k->threads, &k->smem_bytes, &k->par, &k->trav, &k->head);
-    else if (transposed || Dp > 128)
-      tcgen05_backward_generic_geometry(k->type, Dp, &k->threads, &k->smem_bytes, &k->par, &k->trav, &k->head);
     else
       tcgen05_backward_geometry(k->type, Dp, &k->threads, &k->smem_bytes, &k->par, &k->trav, &k->head);
   } else if (k->backend == MFA_BACKEND_SIMT_FP32) {
@@ -187,7 +195,7 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
   // block dimensions were edited away from a compiled configuration is rejected.
   if (kd->block_parallelization != k->par || kd->block_traversal != k->trav) {
     std::string msg = "Block dimensions " + std::to_string(kd->block_parallelization) + "x" +
-                      std::to_string(kd->block_traversal) + " have no compiled sm_100a kernel (available: " +
+                      std::to_string(kd->block_traversal) + " have no compiled sm_90a kernel (available: " +
                       std::to_string(k->par) + "x" + std::to_string(k->trav) + ").";
     delete k;
     return fail(MFA_ERROR_UNSUPPORTED, msg);
@@ -195,9 +203,6 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
   static const char *typeNames[] = {"forward", "backward_query", "backward_key_value"};
   k->source_name = std::string("attention_") + typeNames[k->type] +
                    (k->backend == MFA_BACKEND_TCGEN05 ? "_tcgen05" : "_simt_fp32") + "<D=" + std::to_string(D) +
-                   (k->backend == MFA_BACKEND_TCGEN05 && k->trav == 128 && D <= 128 && kd->exp2_fma_quarters
-                        ? ", exp2 on FMA pipe " + std::to_string(kd->exp2_fma_quarters) + "/4"
-                        : std::string()) +
                    ">";
   *out = k;
   return MFA_SUCCESS;
@@ -244,26 +249,19 @@ int mfa_attention_kernel_launch_count(const mfa_attention_kernel_t *kernel, cons
                                       uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   *out = 1;
-  const uint16_t forward_operands = (1u << MFA_Q) | (1u << MFA_K) | (1u << MFA_V) | (1u << MFA_O);
-  if (kernel->backend == MFA_BACKEND_TCGEN05 && kernel->type == MFA_FORWARD &&
-      !(kernel->descriptor.transpose_state_mask & forward_operands))  // (the layout-generic kernel never splits)
-    *out = tcgen05_forward_launch_count(c->row, c->column, kernel->descriptor.head_dimension,
-                                        c->batch_count ? c->batch_count : 1, kernel->descriptor.split_min_blocks,
-                                        kernel->descriptor.split_max);
-  if (kernel->backend == MFA_BACKEND_TCGEN05 && kernel->type != MFA_FORWARD) {
-    const uint16_t any = kernel->descriptor.transpose_state_mask & kernel->descriptor.transpose_state_valid_mask;
-    const uint32_t Dp = (kernel->descriptor.head_dimension + 7u) / 8u * 8u;
-    const uint32_t b = c->batch_count ? c->batch_count : 1;
-    const bool convert = kernel->descriptor.memory_precisions[MFA_dO] != kernel->descriptor.memory_precisions[MFA_Q];
-    *out = (any || Dp > 128)
-               ? tcgen05_backward_generic_launch_count(kernel->type, c->row, c->column, Dp, b, kernel->descriptor.split_min_blocks,
-                                                       kernel->descriptor.split_max, convert)
-               : tcgen05_backward_launch_count(kernel->type, c->row, c->column, b, kernel->descriptor.split_min_blocks,
-                                               kernel->descriptor.split_max, convert);
-  }
-  // head % 8 != 0 on the tensor-core family: one padding copy per staged input, one un-padding copy per output
-  if (kernel->backend == MFA_BACKEND_TCGEN05 && kernel->descriptor.head_dimension % 8 != 0)
-    *out += kernel->type == MFA_FORWARD ? 4 : (kernel->type == MFA_BACKWARD_QUERY ? 6 : 6);
+  if (kernel->backend != MFA_BACKEND_TCGEN05) return MFA_SUCCESS;
+  const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
+  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, b = c->batch_count ? c->batch_count : 1;
+  if (kernel->type == MFA_FORWARD)
+    *out = tcgen05_forward_launch_count(c->row, c->column, Dp, b, d.split_min_blocks, d.split_max);
+  else
+    *out = tcgen05_backward_launch_count(kernel->type, c->row, c->column, Dp, b, d.split_min_blocks, d.split_max,
+                                         d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q]);
+  // staged operands (head % 8 != 0, or stored transposed): one copy per staged input, one per output
+  int n = 0;
+  const int *ops = operands_of(kernel->type, &n);
+  for (int i = 0; i < n; ++i)
+    if (stages_operand(kernel->type, ops[i], d.head_dimension % 8 != 0, d.transpose_state_mask)) *out += 1;
   return MFA_SUCCESS;
 }
 
@@ -288,55 +286,50 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
     const size_t elements = (slot == sL || slot == sD) ? seq : seq * p.D;
     head_bytes[slot] = elements * (p.prec[slot] == FP32 ? 4 : 2);
   }
-  // D % 8 != 0 on the tensor-core family: stage the operands with pad8(D) columns, run the kernels at the padded head
-  // dimension (the softmax scale stays 1 / sqrt(D) of the true D), copy the FP32 outputs back without the padding.
-  const bool padded = kernel->backend == MFA_BACKEND_TCGEN05 && p.D % 8 != 0;
+  // Tensor-core family: operands with D % 8 != 0 or a transposed layout are staged row-major with pad8(D) columns, the
+  // kernels run at the padded head dimension (the softmax scale stays 1 / sqrt(D) of the true D), and the FP32 outputs
+  // are copied back to the caller's layout without the padding.
+  const bool tc = kernel->backend == MFA_BACKEND_TCGEN05;
+  const bool padded = tc && p.D % 8 != 0;
   const uint32_t Dp = (p.D + 7) / 8 * 8;
-  const int device = padded ? current_device() : 0;
+  int n = 0;
+  const int *ops = operands_of(kernel->type, &n);
+  bool staged = false;
+  for (int i = 0; i < n; ++i) staged |= tc && stages_operand(kernel->type, ops[i], padded, kernel->descriptor.transpose_state_mask);
+  const int device = staged ? current_device() : 0;
   for (uint32_t h0 = 0; h0 < batch; h0 += kMaxBatchPerLaunch) {
     AttentionParams q = p;
     q.batch = batch - h0 < kMaxBatchPerLaunch ? batch - h0 : kMaxBatchPerLaunch;
     for (int slot = 0; slot < kSlots; ++slot)
       if (q.buf[slot]) q.buf[slot] = static_cast<char *>(q.buf[slot]) + head_bytes[slot] * h0;
     cudaError_t e = cudaSuccess;
-    void *user_out[kSlots] = {};  // padded path: where the un-padded outputs go
-    if (padded) {
-      // operands with a head dimension, by kernel type: inputs are staged, outputs are computed into staging
-      static const int fwd_in[] = {sQ, sK, sV}, fwd_out[] = {sO};
-      static const int dq_in[] = {sQ, sK, sV, sO, sdO}, dq_out[] = {sdQ};
-      static const int dkv_in[] = {sQ, sK, sV, sdO}, dkv_out[] = {sdV, sdK};
-      const int *ins = kernel->type == MFA_FORWARD ? fwd_in : (kernel->type == MFA_BACKWARD_QUERY ? dq_in : dkv_in);
-      const int nin = kernel->type == MFA_FORWARD ? 3 : (kernel->type == MFA_BACKWARD_QUERY ? 5 : 4);
-      const int *outs = kernel->type == MFA_FORWARD ? fwd_out : (kernel->type == MFA_BACKWARD_QUERY ? dq_out : dkv_out);
-      const int nout = kernel->type == MFA_BACKWARD_KEY_VALUE ? 2 : 1;
-      auto rows_of = [&](int slot) -> uint64_t {
-        return static_cast<uint64_t>(q.batch) * ((slot == sK || slot == sV || slot == sdK || slot == sdV) ? p.C : p.R);
-      };
+    void *user_out[kSlots] = {};  // staged outputs: where the caller's copies go
+    if (staged) {
+      auto seq_of = [&](int slot) -> uint32_t { return (slot == sK || slot == sV || slot == sdK || slot == sdV) ? p.C : p.R; };
       auto bytes_of = [&](int slot) -> size_t {
-        return ((rows_of(slot) * Dp * (p.prec[slot] == FP32 ? 4 : 2)) + 255) & ~size_t(255);
+        return ((static_cast<size_t>(q.batch) * seq_of(slot) * Dp * (p.prec[slot] == FP32 ? 4 : 2)) + 255) & ~size_t(255);
       };
       size_t total = 0;
-      for (int i = 0; i < nin; ++i) total += bytes_of(ins[i]);
-      for (int i = 0; i < nout; ++i) total += bytes_of(outs[i]);
+      for (int i = 0; i < n; ++i)
+        if (stages_operand(kernel->type, ops[i], padded, kernel->descriptor.transpose_state_mask)) total += bytes_of(ops[i]);
       void *ws = nullptr;
       if ((e = workspace_for(device, stream, total, &ws, /*slot=*/1)) != cudaSuccess)
-        return fail(MFA_ERROR_CUDA, std::string("padding workspace: ") + cudaGetErrorString(e) + " " + last_launch_detail());
+        return fail(MFA_ERROR_CUDA, std::string("staging workspace: ") + cudaGetErrorString(e) + " " + last_launch_detail());
       char *cursor = static_cast<char *>(ws) + kWorkspaceCounterBytes;
-      for (int i = 0; i < nin && e == cudaSuccess; ++i) {
-        const int slot = ins[i];
-        e = launch_pad_columns(q.buf[slot], cursor, rows_of(slot), p.D, Dp, p.prec[slot] == FP32 ? 4 : 2, stream);
+      for (int i = 0; i < n && e == cudaSuccess; ++i) {
+        const int slot = ops[i];
+        if (!stages_operand(kernel->type, slot, padded, kernel->descriptor.transpose_state_mask)) continue;
+        if (is_output(kernel->type, slot))
+          user_out[slot] = q.buf[slot];
+        else
+          e = launch_stage_operand(q.buf[slot], cursor, q.batch, seq_of(slot), p.D, Dp, p.prec[slot] == FP32 ? 4 : 2,
+                                   q.transposed[slot], stream);
         q.buf[slot] = cursor;
         cursor += bytes_of(slot);
       }
-      for (int i = 0; i < nout; ++i) {
-        const int slot = outs[i];
-        user_out[slot] = q.buf[slot];
-        q.buf[slot] = cursor;
-        cursor += bytes_of(slot);
-      }
+      for (int slot = 0; slot < kSlots; ++slot) q.transposed[slot] = 0;
       q.D = Dp;  // (q.scale / q.scale_log2 keep the true head dimension)
-      if (e != cudaSuccess)
-        return fail(MFA_ERROR_CUDA, std::string("head-dimension padding failed: ") + cudaGetErrorString(e));
+      if (e != cudaSuccess) return fail(MFA_ERROR_CUDA, std::string("operand staging failed: ") + cudaGetErrorString(e));
     }
     if (kernel->backend == MFA_BACKEND_TCGEN05) {
       switch (kernel->type) {
@@ -354,33 +347,21 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
     if (e != cudaSuccess)
       return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " failed: " + cudaGetErrorString(e) +
                                       " " + last_launch_detail());
-    if (padded) {
+    if (staged) {
       for (int slot = 0; slot < kSlots && e == cudaSuccess; ++slot)
         if (user_out[slot]) {
-          const uint64_t rows = static_cast<uint64_t>(q.batch) * ((slot == sdK || slot == sdV) ? p.C : p.R);
-          e = launch_unpad_columns(q.buf[slot], user_out[slot], rows, p.D, Dp, stream);
+          const uint32_t seq = (slot == sdK || slot == sdV) ? p.C : p.R;
+          e = launch_unstage_output(static_cast<const float *>(q.buf[slot]), static_cast<float *>(user_out[slot]), q.batch,
+                                    seq, p.D, Dp, p.transposed[slot], stream);
         }
-      if (e != cudaSuccess)
-        return fail(MFA_ERROR_CUDA, std::string("head-dimension un-padding failed: ") + cudaGetErrorString(e));
+      if (e != cudaSuccess) return fail(MFA_ERROR_CUDA, std::string("copy-back of staged outputs failed: ") + cudaGetErrorString(e));
     }
   }
   return MFA_SUCCESS;
 }
 
-// Debug-only export (deliberately absent from include/mfa_b200.h): forward with pipeline timestamps.
-MFA_API int mfa_debug_forward_trace(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
-                                    void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, long long *trace) {
-  if (!kernel || !constants || !buffers || !trace) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  AttentionParams p;
-  int status = build_params(kernel, constants, buffers, p);
-  if (status != MFA_SUCCESS) return status;
-  cudaError_t e = p.D > 128 ? launch_tcgen05_forward_d256_trace(p, static_cast<cudaStream_t>(cuda_stream), trace)
-                            : launch_tcgen05_forward_trace(p, static_cast<cudaStream_t>(cuda_stream), trace);
-  if (e != cudaSuccess) return fail(MFA_ERROR_CUDA, std::string("trace launch failed: ") + cudaGetErrorString(e));
-  return MFA_SUCCESS;
-}
-
-// Debug-only export: 0 forces split-KV onto its scratch + combine fallback (tests cover both forms).
+// Debug-only export (deliberately absent from include/mfa_b200.h): 1 merges split-KV partials inside the attention
+// kernel (one launch), 0 (default) in a second launch (tests cover both forms).
 MFA_API void mfa_debug_set_forward_fused(int enabled) { tcgen05_forward_set_fused(enabled); }
 
 // ------------------------------------------------------------------------------------------------
@@ -499,7 +480,7 @@ void destroy_scratch(Scratch &s) {
 // (copy launch overheads), at most kMaxChunks chunks, and no chunking at all for a single problem
 uint32_t chunk_heads(uint32_t batch, size_t bytes_per_head) {
   if (batch <= 1) return 1;
-  // tuning knob (scripts/gpu_runs: chunk-count sweep of the host-buffer path): MFA_B200_HOST_CHUNKS=<n>
+  // tuning knob (chunk-count sweeps of the host-buffer path): MFA_B200_HOST_CHUNKS=<n>
   if (const char *env = getenv("MFA_B200_HOST_CHUNKS")) {
     const uint32_t n = static_cast<uint32_t>(atoi(env));
     if (n >= 1 && n <= kMaxChunks) return (batch + n - 1) / n;

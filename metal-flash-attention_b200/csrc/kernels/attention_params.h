@@ -1,4 +1,4 @@
-// Internal launch interface between the C-ABI host layer (csrc/*.cpp) and the sm_100a kernels.
+// Internal launch interface between the C-ABI host layer (csrc/*.cpp) and the sm_90a kernels.
 // Not part of the public ABI (include/mfa_b200.h is).
 #pragma once
 #include <cuda_runtime.h>
@@ -23,8 +23,8 @@ struct AttentionParams {
   uint8_t transposed[kSlots];  // 1: stored [D][seq] (leading dim = seq), 0: [seq][D]
   float scale;       // 1/sqrt(D)          (AttentionKernel+Softmax.swift:17-26)
   float scale_log2;  // log2(e)/sqrt(D)
-  // tuning columns of the parameter-table row the kernel was created from (tcgen05 family)
-  uint8_t exp2_fma_quarters;  // selects the kernel instantiation
+  // tuning columns of the parameter-table row the kernel was created from (tensor-core family)
+  uint8_t exp2_fma_quarters;  // validated and carried; the sm_90a kernels take every exp2 on the MUFU pipe
   uint8_t split_min_blocks;   // 0 = never split small grids
   uint8_t split_max;
 };
@@ -39,44 +39,31 @@ cudaError_t launch_simt_backward_key_value(const AttentionParams &p, cudaStream_
 void simt_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
                    uint32_t *head);
 
-// ---- tcgen05 / TMA / TMEM family (16-bit row-major inputs, D % 8 == 0) ----------------------
-struct Tcgen05Plan;  // owns tensor maps; defined in tcgen05_common.h
-bool tcgen05_forward_supported(const AttentionParams &p);
+// ---- tensor-core family (wgmma_attention.cu; the backend keeps its historical name "tcgen05" in the ABI) --------
+// 16-bit row-major operands with D % 8 == 0 and D <= 256; kernel.cpp stages every other layout into that form.
 cudaError_t launch_tcgen05_forward(const AttentionParams &p, cudaStream_t stream);
-void tcgen05_forward_geometry(uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
-                              uint32_t *head);
-uint32_t tcgen05_forward_launch_count(uint32_t R, uint32_t C, uint32_t D, uint32_t batch, uint32_t min_blocks,
-                                      uint32_t max_splits);
-cudaError_t launch_tcgen05_forward_d256(const AttentionParams &p, cudaStream_t stream);  // 128 < D <= 256
-cudaError_t launch_tcgen05_forward_generic(const AttentionParams &p, cudaStream_t stream);  // transposed operands, D <= 256
-bool tcgen05_forward_transposes_ok(uint32_t R, uint32_t C, bool tQ, bool tK, bool tV);
-void tcgen05_forward_generic_geometry(uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
-                                      uint32_t *head);
-void tcgen05_forward_d256_geometry(uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav);
-bool tcgen05_backward_supported(const AttentionParams &p);
 cudaError_t launch_tcgen05_backward_query(const AttentionParams &p, cudaStream_t stream);
 cudaError_t launch_tcgen05_backward_key_value(const AttentionParams &p, cudaStream_t stream);
-uint32_t tcgen05_backward_launch_count(int type, uint32_t R, uint32_t C, uint32_t batch, uint32_t min_blocks,
+uint32_t tcgen05_forward_launch_count(uint32_t R, uint32_t C, uint32_t D, uint32_t batch, uint32_t min_blocks,
+                                      uint32_t max_splits);
+uint32_t tcgen05_backward_launch_count(int type, uint32_t R, uint32_t C, uint32_t D, uint32_t batch, uint32_t min_blocks,
                                        uint32_t max_splits, bool convert_dO);
-bool tcgen05_backward_converts_dO_first(uint32_t C, uint32_t batch);
+void tcgen05_forward_set_fused(int enabled);  // debug: 1 = split-KV merged inside the attention kernel (one launch)
+void tcgen05_forward_geometry(uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
+                              uint32_t *head);
 void tcgen05_backward_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par,
                                uint32_t *trav, uint32_t *head);
-// layout-generic backward (tcgen05_backward_generic.cu): 128 < D <= 256, and transposed operands at any D <= 256
+bool tcgen05_forward_transposes_ok(uint32_t R, uint32_t C, bool tQ, bool tK, bool tV);
 bool tcgen05_backward_transposes_ok(uint32_t R, uint32_t C, bool tQ, bool tK, bool tV, bool tO);
-cudaError_t launch_tcgen05_backward_generic(const AttentionParams &p, cudaStream_t stream, bool key_value);
-uint32_t tcgen05_backward_generic_launch_count(int type, uint32_t R, uint32_t C, uint32_t D, uint32_t batch,
-                                               uint32_t min_blocks, uint32_t max_splits, bool convert_dO);
-void tcgen05_backward_generic_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par,
-                                       uint32_t *trav, uint32_t *head);
 
-void tcgen05_forward_set_fused(int enabled);  // debug: 0 = split-KV through scratch + combine kernel (two launches)
-cudaError_t launch_tcgen05_forward_trace(const AttentionParams &p, cudaStream_t stream, long long *trace);  // debug
-cudaError_t launch_tcgen05_forward_d256_trace(const AttentionParams &p, cudaStream_t stream, long long *trace);  // debug
-// head-dimension padding for D % 8 != 0 on the tensor-core family (pad_head.cu)
-cudaError_t launch_pad_columns(const void *src, void *dst, uint64_t rows, uint32_t D, uint32_t Dp, uint32_t element_bytes,
-                               cudaStream_t stream);
+// operand staging for the tensor-core family (pad_head.cu): a [batch][seq][D] (or, transposed, [batch][D][seq]) operand
+// is copied to row-major [batch][seq][Dp] with zero padding columns, and an FP32 output computed in that form is copied
+// back to the caller's layout
+cudaError_t launch_stage_operand(const void *src, void *dst, uint32_t batch, uint32_t seq, uint32_t D, uint32_t Dp,
+                                 uint32_t element_bytes, bool transposed, cudaStream_t stream);
+cudaError_t launch_unstage_output(const float *src, float *dst, uint32_t batch, uint32_t seq, uint32_t D, uint32_t Dp,
+                                  bool transposed, cudaStream_t stream);
 cudaError_t launch_bf16_to_f16(const void *src, void *dst, uint64_t elements, cudaStream_t stream);
-cudaError_t launch_unpad_columns(const void *src, void *dst, uint64_t rows, uint32_t D, uint32_t Dp, cudaStream_t stream);
 const char *last_launch_detail();  // thread-local detail string for MFA_ERROR_CUDA messages
 
 }  // namespace mfa

@@ -1,13 +1,12 @@
-// Pieces shared by the backward kernels (tcgen05_backward.cu: D <= 128 row-major; tcgen05_backward_generic.cu:
-// D <= 256 and transposed operands): statistic loads / stores, the on-chip BF16 -> FP16 rewrite of dO, and the
-// deterministic merge of a traversal split.
+// Pieces shared by the tensor-core kernels (wgmma_attention.cu) and the staging copies (pad_head.cu): statistic loads /
+// stores and the BF16 -> FP16 rewrite of dO.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "attention_params.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace mfa {
 namespace bwd {
@@ -31,79 +30,14 @@ __device__ __forceinline__ void store_stat(void *p, size_t i, int prec, float v)
 }
 
 // dO arrives as BF16 while Q, K, V are FP16 (the reference's own low-precision policy,
-// AttentionDescriptor+Precisions.swift:13-23); tcgen05 kind::f16 cannot mix the two element types in one MMA, so the
-// staged dO tile is rewritten in place as FP16 before any MMA reads it.  BF16 -> FP16 is exact for 2^-14 <= |x| < 65504
+// AttentionDescriptor+Precisions.swift:13-23); wgmma cannot mix the two element types in one MMA, so dO is
+// rewritten as FP16 before any MMA reads it.  BF16 -> FP16 is exact for 2^-14 <= |x| < 65504
 // (8 significant bits fit FP16's 11); gradients outside that range would not survive FP16 Q/K/V either.
 __device__ __forceinline__ uint32_t bf16x2_to_f16x2(uint32_t w) {
   return pack_f16x2(__uint_as_float(w << 16), __uint_as_float(w & 0xFFFF0000u));
 }
 __device__ __forceinline__ uint4 bf16x8_to_f16x8(uint4 v) {
   return make_uint4(bf16x2_to_f16x2(v.x), bf16x2_to_f16x2(v.y), bf16x2_to_f16x2(v.z), bf16x2_to_f16x2(v.w));
-}
-
-// Sums the partial accumulators of a traversal split: out[t][i] = sum_s part[s][t][i] (t = tensor: dQ, or dV and dK).
-// The backward pass needs no softmax re-normalisation across splits (L and D are inputs), so unlike the forward's
-// split-KV merge this is a plain, deterministic sum -- still no atomics (README.md:11).  Every load of a thread is
-// issued before the first add; launched with programmatic stream serialisation.
-template <uint32_t kMaxSplits>
-__global__ void __launch_bounds__(256)
-    sum_splits(const float4 *__restrict__ part, float4 *__restrict__ out0, float4 *__restrict__ out1, size_t tensor_quads,
-               size_t split_stride_quads, uint32_t num_splits) {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= tensor_quads) return;
-  const float4 *src = part + blockIdx.y * tensor_quads + i;
-  float4 v[kMaxSplits];
-#pragma unroll
-  for (uint32_t s = 0; s < kMaxSplits; ++s)
-    v[s] = s < num_splits ? __ldcg(src + s * split_stride_quads) : make_float4(0.f, 0.f, 0.f, 0.f);
-  float4 acc = v[0];
-#pragma unroll
-  for (uint32_t s = 1; s < kMaxSplits; ++s) {
-    acc.x += v[s].x;
-    acc.y += v[s].y;
-    acc.z += v[s].z;
-    acc.w += v[s].w;
-  }
-  (blockIdx.y == 0 ? out0 : out1)[i] = acc;
-}
-
-// How many ranges to cut the traversal axis into: only when the SMs would otherwise idle (a single head at N = 4096 is
-// 32 CTAs for 148 SMs), at least two blocks per range, at most 8 ranges.
-// (min_blocks and max_splits are the row's tuning columns; min_blocks = 0 turns splitting off)
-inline uint32_t choose_blocks_per_split(uint32_t ctas, uint32_t total_blocks, uint32_t sm_count, uint32_t min_blocks,
-                                        uint32_t max_splits) {
-  if (ctas * 2 > sm_count || min_blocks == 0 || total_blocks < 2 * min_blocks) return total_blocks;
-  if (max_splits > 8) max_splits = 8;  // sum_splits<8>
-  uint32_t splits = sm_count / ctas;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 2) return total_blocks;
-  uint32_t per = (total_blocks + splits - 1) / splits;
-  if (per < min_blocks) per = min_blocks;
-  return per;
-}
-
-
-// Launches sum_splits behind `stream`'s previous kernel with programmatic stream serialisation (the producer kernel
-// executes griddepcontrol.launch_dependents early; the sum's griddepcontrol.wait holds it until that grid has
-// completed and flushed).  `tensors` = 1 (out0) or 2 (out0, out1) consecutive tensors per split slice.
-inline cudaError_t launch_sum_splits(const float *scratch, float *out0, float *out1, size_t tensor_elems, uint32_t tensors,
-                                     size_t split_stride, uint32_t splits, cudaStream_t stream) {
-  const size_t quads = tensor_elems / 4;  // D % 8 == 0
-  cudaLaunchAttribute attr;
-  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr.val.programmaticStreamSerializationAllowed = 1;
-  cudaLaunchConfig_t config = {};
-  config.gridDim = dim3(static_cast<uint32_t>((quads + 255) / 256), tensors, 1);
-  config.blockDim = dim3(256, 1, 1);
-  config.stream = stream;
-  config.attrs = &attr;
-  config.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&config, sum_splits<8>, reinterpret_cast<const float4 *>(scratch),
-                                     reinterpret_cast<float4 *>(out0), reinterpret_cast<float4 *>(out1), quads,
-                                     split_stride / 4, splits);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  return e;
 }
 
 }  // namespace bwd

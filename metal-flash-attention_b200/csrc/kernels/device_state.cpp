@@ -21,13 +21,13 @@ int current_device() {
 uint32_t device_sm_count(int device) {
   static std::mutex mutex;
   static int cached[kMaxDevices] = {};
-  if (device < 0) return 148;
+  if (device < 0) return 132;
   std::lock_guard<std::mutex> lock(mutex);
   if (device < kMaxDevices && cached[device] > 0) return static_cast<uint32_t>(cached[device]);
   int count = 0;
   if (cudaDeviceGetAttribute(&count, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || count <= 0) {
     cudaGetLastError();
-    return 148;
+    return 132;
   }
   if (device < kMaxDevices) cached[device] = count;
   return static_cast<uint32_t>(count);

@@ -14,7 +14,7 @@ constexpr int kMaxDevices = 64;
 // cudaGetDevice with the error folded into the return value (-1)
 int current_device();
 
-// multiprocessors of `device` (cached per device; 148 on B200)
+// multiprocessors of `device` (cached per device; 148 on H100)
 uint32_t device_sm_count(int device);
 
 // cudaFuncSetAttribute(kernel, MaxDynamicSharedMemorySize, bytes) once per (kernel, device)

@@ -1,17 +1,17 @@
-// SIMT FP32 attention kernels for sm_100a: forward, backward-dQ, backward-dK/dV.
+// SIMT FP32 attention kernels for sm_90a: forward, backward-dQ, backward-dK/dV.
 //
-// This family is the B200 counterpart of the reference's FP32 code path: every contraction is an
+// This family is the H100 counterpart of the reference's FP32 code path: every contraction is an
 // FP32 FMA on the CUDA cores (the reference's FP32 simdgroup_matrix MMAs are ALU FMAs as well), so
 // results meet the reference's FP32 tolerance (2e-5 absolute, SquareAttentionTest.swift:547-554).
 // It accepts everything the reference's API accepts: any R, C, any D <= 512, per-operand
-// transposes, FP32/FP16/BF16 memory precisions.  The tensor-core (tcgen05) family in
-// tcgen05_forward.cu covers the 16-bit hot path.
+// transposes, FP32/FP16/BF16 memory precisions.  The tensor-core family in
+// wgmma_attention.cu covers the 16-bit hot path.
 //
 // Algorithm follows the reference kernels' structure, not their code:
 //   forward         loopForward           AttentionKernel+Source.swift:158-200
 //   backward dQ     loopBackwardQuery     AttentionKernel+Source.swift:202-242, computeD +Softmax.swift:32-221
 //   backward dK/dV  loopBackwardKeyValue  AttentionKernel+Source.swift:244-293
-// Numerical conventions (Appendix A of SURVEY.md): log2-domain running max m, L = m + log2(l),
+// Numerical conventions: log2-domain running max m, L = m + log2(l),
 // D stored pre-scaled by 1/sqrt(D), BF16 stores truncate, edge columns masked before softmax.
 //
 // Tiling: one CTA = 256 threads = a 64 x 64 block of the attention matrix; thread (tx, ty) owns

@@ -40,7 +40,7 @@ struct AttentionKernelDescriptor {  // AttentionKernelDescriptor.swift:7-48
   std::optional<uint16_t> headDimension() const {
     return c.has_head_dimension ? std::optional<uint16_t>(c.head_dimension) : std::nullopt;
   }
-  // B200 extension: the tuning columns of the parameter-table row (editable like every other field)
+  // library extension: the tuning columns of the parameter-table row (editable like every other field)
   uint8_t &exp2FmaQuarters() { return c.exp2_fma_quarters; }
   uint8_t &splitMinBlocks() { return c.split_min_blocks; }
   uint8_t &splitMax() { return c.split_max; }
@@ -57,8 +57,8 @@ struct AttentionDescriptor {  // AttentionDescriptor.swift:10-27
   bool lowPrecisionIntermediates = false;
   std::optional<MatrixDimensions> matrixDimensions;
   std::optional<TransposeState> transposeState;
-  std::optional<GEMMOperandPrecision> inputPrecisionOverride;  // B200 extension
-  uint32_t batchCount = 1;                                     // B200 extension
+  std::optional<GEMMOperandPrecision> inputPrecisionOverride;  // library extension
+  uint32_t batchCount = 1;                                     // library extension
 
   mfa_attention_descriptor_t c() const {
     mfa_attention_descriptor_t d;
@@ -151,7 +151,7 @@ class AttentionKernel {  // AttentionKernel.swift:11-50
   bool owned_ = true;
 };
 
-// Page-locked host buffers on the GPU's NUMA node for AttentionDescriptor::runHost (B200 extension; the reference's
+// Page-locked host buffers on the GPU's NUMA node for AttentionDescriptor::runHost (library extension; the reference's
 // buffers are Metal shared-storage buffers, MTLContext+Buffers.swift:5-45)
 struct HostMemory {
   // upload: write-combined pages for buffers the host only writes and the GPU reads (Q, K, V, dO)

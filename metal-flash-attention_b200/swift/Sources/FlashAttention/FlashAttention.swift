@@ -1,5 +1,5 @@
 //
-//  FlashAttention.swift -- drop-in Swift surface over the B200 C ABI.
+//  FlashAttention.swift -- drop-in Swift surface over the H100 C ABI.
 //
 //  Same public names, fields and failure behaviour as the reference package
 //  (Sources/FlashAttention/Attention/*.swift), minus everything Metal-specific:
@@ -46,9 +46,9 @@ public struct AttentionDescriptor {
   public var lowPrecisionIntermediates: Bool = false
   public var matrixDimensions: (row: UInt32, column: UInt32, head: UInt16)?
   public var transposeState: (Q: Bool, K: Bool, V: Bool, O: Bool)?
-  /// B200 extension: BF16 Q/K/V/dO in memory (nil = the reference's FP16 policy).
+  /// library extension: BF16 Q/K/V/dO in memory (nil = the reference's FP16 policy).
   public var inputPrecisionOverride: GEMMOperandPrecision?
-  /// B200 extension: number of independent single-head problems stored back to back.
+  /// library extension: number of independent single-head problems stored back to back.
   public var batchCount: UInt32 = 1
 
   public init() {}
@@ -112,7 +112,7 @@ public struct AttentionDescriptor {
     check(mfa_attention_descriptor_set_function_constants(&descriptor, &constants))
   }
 
-  /// The B200 parameter table this descriptor reads for `type` (AttentionDescriptor+Parameters.swift:106-285 format).
+  /// The H100 parameter table this descriptor reads for `type` (AttentionDescriptor+Parameters.swift:106-285 format).
   public func parameterFile(type: AttentionKernelType) -> String {
     var descriptor = c
     return String(cString: mfa_attention_descriptor_parameter_file(&descriptor, mfa_kernel_type_t(type.rawValue)))
@@ -143,7 +143,7 @@ public struct AttentionDescriptor {
   }
 }
 
-/// Page-locked host buffers on the GPU's NUMA node for `AttentionDescriptor.runHost` (B200 extension).
+/// Page-locked host buffers on the GPU's NUMA node for `AttentionDescriptor.runHost` (library extension).
 public enum HostMemory {
   /// `upload`: write-combined pages for buffers the host only writes and the GPU reads (Q, K, V, dO).
   public static func allocate(byteCount: Int, device: Int32 = 0, upload: Bool = false) -> UnsafeMutableRawPointer {
@@ -162,7 +162,7 @@ public enum HostMemory {
   public static func releaseResources(device: Int32) { check(mfa_release_device_resources(device)) }
 }
 
-/// Which kernel family serves a descriptor (B200 extension; the reference has one family).
+/// Which kernel family serves a descriptor (library extension; the reference has one family).
 public enum AttentionBackend: UInt8 {
   case simtFP32 = 0
   case tcgen05 = 1
@@ -241,7 +241,7 @@ public struct AttentionKernelDescriptor {
     set { Self.setPrecisions(&c, register: true, newValue) }
   }
 
-  /// :22  preferAsyncCache ("async" == TMA bulk-tensor copies on B200)
+  /// :22  preferAsyncCache ("async" == TMA bulk-tensor copies on H100)
   public var preferAsyncCache: Bool? {
     get { c.prefer_async_cache == 0xFF ? nil : c.prefer_async_cache != 0 }
     set { c.prefer_async_cache = newValue.map { $0 ? 1 : 0 } ?? 0xFF }
@@ -277,12 +277,12 @@ public struct AttentionKernelDescriptor {
     set { c.type = newValue.map { UInt8($0.rawValue) } ?? 0xFF }
   }
 
-  /// B200 extension: the kernel family `AttentionDescriptor.kernelDescriptor(type:)` selected.
+  /// library extension: the kernel family `AttentionDescriptor.kernelDescriptor(type:)` selected.
   public var backend: AttentionBackend {
     get { AttentionBackend(rawValue: c.backend) ?? .simtFP32 }
     set { c.backend = newValue.rawValue }
   }
-  /// B200 extension: tuning columns of the parameter-table row.  Of every 4 element pairs of P, how many take exp2 on
+  /// library extension: tuning columns of the parameter-table row.  Of every 4 element pairs of P, how many take exp2 on
   /// the FMA pipe (selects the kernel instantiation); small-grid split policy (minimum blocks per range, 0 = never;
   /// maximum ranges).
   public var exp2FmaQuarters: UInt8 {

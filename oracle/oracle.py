@@ -1,5 +1,5 @@
 """ctypes wrapper over oracle/_build/liboracle.so (C restatement of the reference's `Network`,
-/root/reference/Tests/FlashAttentionTests/Utilities/Network.swift:70-403).
+the reference's Tests/FlashAttentionTests/Utilities/Network.swift:70-403).
 
 TEST INFRASTRUCTURE: parity unpinned against reference-generated vectors (none exist; the
 reference cannot run here) -- pinned instead by oracle_np.py (float64) + finite differences, see

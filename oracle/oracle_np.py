@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE. Independent float64 numpy formulation of single-head attention and its
 gradients (matrix form, not row-at-a-time) used ONLY to pin oracle/network_oracle.c
-(tests/test_oracle.py). Math per /root/reference/README.md:41-46 and Network.swift:134-402."""
+(tests/test_oracle.py). Math per the reference's README.md:41-46 and Network.swift:134-402."""
 import numpy as np
 
 

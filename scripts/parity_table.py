@@ -1,7 +1,7 @@
 """Measured parity of the CUDA path against the CPU oracle at the BASELINE.json configs, one JSON line per
 (config, dtype policy, output): max-abs, max-rel and relative RMS error.
 
-  max_rel = max |a - b| / max(|b|, 1e-3 * rms(b))       (SURVEY.md section 8(c))
+  max_rel = max |a - b| / max(|b|, 1e-3 * rms(b))
   rel_rms = rms(a - b) / rms(b)
 
 The oracle (oracle/network_oracle.c, the C restatement of the reference's Network.swift) runs on the inputs AFTER

@@ -63,7 +63,7 @@ def test_memory_precisions_follow_reference_policy():
     for flags in ((True, True), (True, False), (False, True)):
         m = make(lowIn=flags[0], lowMid=flags[1]).memoryPrecisions
         assert all(m[op] == P.FP32 for op in (Op.O, Op.dV, Op.dK, Op.dQ))   # :140-143 outputs always FP32
-    m = make(lowIn=True, bf16=True).memoryPrecisions                         # B200 extension
+    m = make(lowIn=True, bf16=True).memoryPrecisions                         # library extension
     assert (m[Op.Q], m[Op.K], m[Op.V], m[Op.dO]) == (P.BF16,) * 4
 
 
@@ -80,7 +80,7 @@ def test_register_precisions():
 
 
 def test_register_precisions_report_what_the_tensor_core_kernels_do():
-    """On the tcgen05 family P and dS are MMA operands: always the 16-bit input element type, whatever
+    """On the tensor-core family P and dS are MMA operands: always the 16-bit input element type, whatever
     lowPrecisionIntermediates says (documented deviation from AttentionDescriptor+Precisions.swift:203-205) -- the
     descriptor must not advertise FP32 registers the kernel does not have."""
     for lowMid in (False, True):
@@ -134,13 +134,13 @@ def test_heuristic_selects_tensor_core_family_only_where_it_applies():
     # ... as far as the kernels reach (pad8(D) <= 256), and not for transposed operands
     assert make(64, 64, 199, lowIn=True).kernelDescriptor(KT.forward).backend == mfa.Backend.tcgen05
     kd199 = make(64, 64, 199, lowIn=True).kernelDescriptor(KT.backwardQuery)
-    assert kd199.backend == mfa.Backend.tcgen05 and kd199.blockDimensions == (128, 64, 200)   # wide-head kernels
+    assert kd199.backend == mfa.Backend.tcgen05 and kd199.blockDimensions == (64, 64, 200)   # wide-head dQ: one warpgroup
     assert make(64, 64, 260, lowIn=True).kernelDescriptor(KT.backwardQuery).backend == mfa.Backend.simtFP32
     assert make(64, 64, 260, lowIn=True).kernelDescriptor(KT.forward).backend == mfa.Backend.simtFP32
     assert make(64, 64, 77, lowIn=True, transposes=(True, False, False, False)).kernelDescriptor(
         KT.forward).backend == mfa.Backend.simtFP32
-    # transposed operands: the layout-generic tensor-core kernels where TMA can address the transposed view (row pitch =
-    # sequence length, a multiple of 8 elements)
+    # transposed operands: staged row-major for the tensor-core kernels where the transposed view has a 16-byte row pitch
+    # (sequence length a multiple of 8 elements)
     tK = make(64, 64, 64, lowIn=True, transposes=(False, True, False, False))
     assert tK.kernelDescriptor(KT.forward).backend == mfa.Backend.tcgen05
     assert tK.kernelDescriptor(KT.forward).blockDimensions == (128, 128, 64)
@@ -164,14 +164,14 @@ def test_heuristic_selects_tensor_core_family_only_where_it_applies():
     b = mfa.AttentionKernel.cached(make(77, 64, 64, lowIn=True, transposes=(True, False, False, False)), KT.forward)
     assert a._handle.value != b._handle.value and "tcgen05" in a.sourceName() and "simt" in b.sourceName()
     kd = make(4096, 4096, 128, lowIn=True, bf16=True).kernelDescriptor(KT.forward)
-    assert kd.preferAsyncLoad and kd.preferAsyncCache           # "async" == TMA on B200
-    assert kd.cacheState == {Op.Q: True, Op.O: True}             # Q resident in SMEM, O resident in TMEM
+    assert kd.preferAsyncLoad and kd.preferAsyncCache           # "async" == TMA on H100
+    assert kd.cacheState == {Op.Q: True, Op.O: True}             # Q resident in SMEM, O resident in registers
 
 
 def test_parameter_file_has_reference_format():
     text = make(4096, 4096, 128, lowIn=True, bf16=True).parameterFile(KT.forward)
     rows = [line for line in text.split("\n") if line.strip()]
-    # the reference's five segments (AttentionParameterRow.swift:46-49) + three B200 tuning columns on the tcgen05 family
+    # the reference's five segments (AttentionParameterRow.swift:46-49) + three tuning columns on the tensor-core family
     assert rows and all(len([c for c in row.split("|") if c != ""]) == 8 for row in rows)
     simt = make(64, 64, 35).parameterFile(KT.forward)
     assert all(len([c for c in row.split("|") if c != ""]) == 5 for row in simt.split("\n") if row.strip())
@@ -208,7 +208,7 @@ def test_invalid_precision_pairs_are_rejected():
 def test_edited_descriptor_outside_compiled_kernels_is_rejected():
     kd = make(lowIn=True, head=64).kernelDescriptor(KT.forward)
     kd.blockDimensions = (32, 80, 16)                                          # an Apple tile shape
-    with pytest.raises(mfa.MFAError, match="no compiled sm_100a kernel"):
+    with pytest.raises(mfa.MFAError, match="no compiled sm_90a kernel"):
         mfa.AttentionKernel(kd)
     with pytest.raises(mfa.MFAError, match="exceeds 512"):
         mfa.AttentionKernel(make(head=600).kernelDescriptor(KT.forward))
@@ -257,7 +257,7 @@ def test_kernel_cache_returns_one_object_per_descriptor_and_type():
         KT.forward)).blockDimensions
     del a, b, c, d, e                                  # library-owned handles: dropping the wrappers must not free them
     again = mfa.AttentionKernel.cached(make(4096, 4096, 120, lowIn=True, bf16=True), KT.forward)
-    assert again.threadgroupSize == 384 and mfa.AttentionKernel.cacheSize() == before + 4
+    assert again.threadgroupSize == 256 and mfa.AttentionKernel.cacheSize() == before + 4
     with pytest.raises(mfa.MFAError, match="Descriptor was incomplete"):
         mfa.AttentionKernel.cached(mfa.AttentionDescriptor(), KT.forward)
 
@@ -308,18 +308,18 @@ int main() {
     subprocess.check_call(["g++", "-std=c++17", "-I", ROOT, str(src), "-o", str(exe), "-L", libdir, "-lmfa_b200",
                            f"-Wl,-rpath,{libdir}"])
     out = subprocess.check_output([str(exe)], text=True).splitlines()
-    assert out[0] == "256 128 128 384 384" and out[1] == "Descriptor was incomplete."
+    assert out[0] == "128 128 128 256 256" and out[1] == "Descriptor was incomplete."
 
 
-FORWARD_TABLE = ("| 64  | 256 | 128 | 64  | Q, O | 2 | 8 | 4 |\n"
-                 "| 128 | 256 | 128 | 128 | Q, O | 1 | 2 | 16 |\n"
-                 "| 256 | 128 | 128 | 256 | Q, O | 0 | 0 | 1 |\n")
+FORWARD_TABLE = ("| 64  | 128 | 128 | 64  | Q, O | 2 | 8 | 4 |\n"
+                 "| 128 | 128 | 128 | 128 | Q, O | 1 | 2 | 16 |\n"
+                 "| 256 | 128 | 64  | 256 | Q, O | 0 | 0 | 1 |\n")
 
 
 def test_parameter_table_is_live_data():
-    """The B200 parameter table drives the kernel (AttentionDescriptor+Parameters.swift:106-285 analogue): editing a row
-    changes the kernel descriptor, the launched instantiation (source name) and the small-grid split policy; every
-    compiled variant is accepted, anything else is rejected and leaves the current table in place."""
+    """The H100 parameter table drives the kernel (AttentionDescriptor+Parameters.swift:106-285 analogue): editing a row
+    changes the kernel descriptor, the cached kernel object and the small-grid split policy; every compiled variant is
+    accepted, anything else is rejected and leaves the current table in place."""
     d = make(4096, 4096, 128, lowIn=True, bf16=True)
     c = mfa.FunctionConstantValues()
     d.setFunctionConstants(c)
@@ -327,15 +327,15 @@ def test_parameter_table_is_live_data():
         kd = d.kernelDescriptor(KT.forward)
         assert kd.exp2FmaQuarters == 0 and kd.splitPolicy == (4, 8)
         k = mfa.AttentionKernel(kd)
-        assert "exp2" not in k.sourceName() and k.launchCount(c) == 2        # 32 blocks / 8 ranges of >= 4
-        cached_before = mfa.AttentionKernel.cached(d, KT.forward).sourceName()
+        assert "exp2" not in k.sourceName() and k.launchCount(c) == 2        # 32 blocks / 4 ranges of >= 4
+        cached_before = mfa.AttentionKernel.cached(d, KT.forward)._handle.value
 
         mfa.setParameterTable(KT.forward, FORWARD_TABLE)
         assert d.parameterFile(KT.forward) == FORWARD_TABLE
         kd = d.kernelDescriptor(KT.forward)
         assert kd.exp2FmaQuarters == 1 and kd.splitPolicy == (2, 16)
-        assert "exp2 on FMA pipe 1/4" in mfa.AttentionKernel(kd).sourceName()
-        assert mfa.AttentionKernel.cached(d, KT.forward).sourceName() != cached_before   # the cache follows the table
+        mfa.AttentionKernel(kd)
+        assert mfa.AttentionKernel.cached(d, KT.forward)._handle.value != cached_before   # the cache follows the table
         kd64 = make(2048, 2048, 64, lowIn=True).kernelDescriptor(KT.forward)
         assert kd64.exp2FmaQuarters == 2 and kd64.splitPolicy == (8, 4)
 
@@ -346,7 +346,7 @@ def test_parameter_table_is_live_data():
             kd.exp2FmaQuarters = q
             mfa.AttentionKernel(kd)
         kd.exp2FmaQuarters = mfa.maxExp2FmaQuarters(KT.forward) + 1
-        with pytest.raises(mfa.MFAError, match="no compiled sm_100a kernel"):
+        with pytest.raises(mfa.MFAError, match="no compiled sm_90a kernel"):
             mfa.AttentionKernel(kd)
 
         # rejected tables leave the installed one untouched
@@ -358,8 +358,10 @@ def test_parameter_table_is_live_data():
                 mfa.setParameterTable(KT.forward, bad)
             assert d.parameterFile(KT.forward) == FORWARD_TABLE
         # the backward kernels have their own tables and a wider compiled range
-        mfa.setParameterTable(KT.backwardQuery, "| 128 | 128 | 128 | 128 | Q, dO, dQ | 3 | 2 | 8 |\n")
-        assert "exp2 on FMA pipe 3/4" in mfa.AttentionKernel(d.kernelDescriptor(KT.backwardQuery)).sourceName()
+        mfa.setParameterTable(KT.backwardQuery, "| 128 | 128 | 64 | 128 | Q, dO, dQ | 3 | 2 | 8 |\n")
+        kdq = d.kernelDescriptor(KT.backwardQuery)
+        assert kdq.exp2FmaQuarters == 3 and kdq.splitPolicy == (2, 8)
+        mfa.AttentionKernel(kdq)
     finally:
         for t in KT:
             mfa.setParameterTable(t, None)
@@ -367,10 +369,10 @@ def test_parameter_table_is_live_data():
 
 
 def test_parameter_file_from_the_environment(tmp_path):
-    """MFA_B200_PARAMETER_FILE: the tables scripts/sweep.py writes are picked up when the library is loaded."""
+    """MFA_B200_PARAMETER_FILE: tables in that file are picked up when the library is loaded."""
     path = tmp_path / "tables.txt"
     path.write_text("# comment\n[forward]\n" + FORWARD_TABLE + "[backwardKeyValue]\n"
-                    "| 64  | 128 | 128 | 64  | K, V, dV, dK | 1 | 2 | 4 |\n| 128 | 128 | 128 | 128 | K, V, dV, dK | 2 | 2 | 8 |\n")
+                    "| 64  | 128 | 64  | 64  | K, V, dV, dK | 1 | 2 | 4 |\n| 128 | 128 | 64  | 128 | K, V, dV, dK | 2 | 2 | 8 |\n")
     code = ("import mfa_b200 as mfa\n"
             "d = mfa.AttentionDescriptor(); d.lowPrecisionInputs = True\n"
             "d.matrixDimensions = (512, 512, 64); d.transposeState = (False,) * 4\n"
@@ -378,7 +380,7 @@ def test_parameter_file_from_the_environment(tmp_path):
             "print([(d.kernelDescriptor(t).exp2FmaQuarters,) + d.kernelDescriptor(t).splitPolicy for t in KT])\n")
     out = subprocess.check_output([sys.executable, "-c", code], cwd=ROOT, text=True,
                                   env=dict(os.environ, MFA_B200_PARAMETER_FILE=str(path)))
-    assert out.strip() == "[(2, 8, 4), (1, 2, 8), (1, 2, 4)]"   # forward and dK-dV from the file, dQ built in
+    assert out.strip() == "[(2, 8, 4), (0, 2, 8), (1, 2, 4)]"   # forward and dK-dV from the file, dQ built in
 
 
 def test_transposed_tables_are_separate_and_live(tmp_path):
@@ -387,7 +389,7 @@ def test_transposed_tables_are_separate_and_live(tmp_path):
     plain = make(512, 512, 64, lowIn=True)
     trans = make(512, 512, 64, lowIn=True, transposes=(False, True, False, False))
     assert trans.kernelDescriptor(KT.backwardKeyValue).blockDimensions == (128, 64, 64)
-    assert plain.kernelDescriptor(KT.backwardKeyValue).blockDimensions == (128, 128, 64)
+    assert plain.kernelDescriptor(KT.backwardKeyValue).blockDimensions == (128, 64, 64)
     try:
         mfa.setParameterTable(KT.backwardKeyValue, "| 256 | 128 | 64 | 256 | K, V, dV, dK | 0 | 4 | 2 |\n", transposed=True)
         assert trans.kernelDescriptor(KT.backwardKeyValue).splitPolicy == (4, 2)
@@ -411,9 +413,9 @@ def test_transposed_tables_are_separate_and_live(tmp_path):
 
 
 def test_committed_parameter_file_matches_the_builtin_tables():
-    """metal-flash-attention_b200/parameters/b200.txt (written by scripts/sweep.py on a B200) is the source of the
-    built-in defaults: loading it must not change any table."""
-    path = os.path.join(ROOT, "metal-flash-attention_b200", "parameters", "b200.txt")
+    """metal-flash-attention_b200/parameters/h100.txt states the built-in defaults: loading it must not change any
+    table."""
+    path = os.path.join(ROOT, "metal-flash-attention_b200", "parameters", "h100.txt")
     if not os.path.exists(path):
         pytest.skip("no committed sweep result")
     code = ("import mfa_b200 as mfa\n"

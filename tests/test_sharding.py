@@ -1,5 +1,5 @@
 """Multi-GPU host logic on CPU: world_size-2 (and 3) gloo process groups exercise the head partition and the
-scatter/gather plumbing bench.py and clients use around the single-GPU kernels (SURVEY.md section 8(e))."""
+scatter/gather plumbing bench.py and clients use around the single-GPU kernels."""
 import os
 import socket
 

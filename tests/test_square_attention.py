@@ -1,5 +1,5 @@
 """The reference's SquareAttentionTest.testCorrectness (Tests/FlashAttentionTests/Attention/
-SquareAttentionTest.swift:5-26 -> validateProblemSize :214-555) against the sm_100a kernels through the
+SquareAttentionTest.swift:5-26 -> validateProblemSize :214-555) against the sm_90a kernels through the
 C ABI: the same 20 (N, D) shapes, FP32 everywhere, forward + dQ + dK/dV, absolute tolerance 2e-5 on
 O, L, D, dV, dK, dQ (:547-554).  Inputs are seeded (the reference's are not); failures assert (the
 reference only prints)."""

@@ -1,12 +1,11 @@
-"""Parity of the tensor-core backward kernels (dQ and dK/dV, TMA + tcgen05 + TMEM) with the CPU oracle, on inputs
+"""Parity of the tensor-core backward kernels (dQ and dK/dV, TMA + wgmma) with the CPU oracle, on inputs
 rounded to the kernels' 16-bit memory format.  Forward runs first (it produces O and L), then backwardQuery (writes
 D and dQ), then backwardKeyValue -- the reference's order (SquareAttentionTest.swift:355-368).
 
 Stated tolerances: the reference's mixed-precision bars (D 1e-1, gradients 5e-2, RectangularAttentionTest.swift:
 459-464) and, tighter, relative RMS error of every gradient <= 2.5e-3 for BF16 / 3e-4 for FP16: the quantisation floor
 of the 16-bit MMA operands P and dS (2^-s / sqrt(6) per rounded operand, s = 8 / 11 significant bits: 1.6e-3 / 2.0e-4;
-measured 1.64-1.71e-3 and 2.1-2.2e-4 at the BASELINE configs, profiles/r2_parity.jsonl; small shapes scatter a little
-above the asymptotic value)."""
+small shapes scatter a little above the asymptotic value)."""
 import numpy as np
 import pytest
 
@@ -29,7 +28,7 @@ def _run(R, C, D, bf16, seed, lowMid=False, referencePolicy=False, transpose=(Fa
     desc.transposeState = tuple(transpose)
     if referencePolicy:
         # the reference's own policy: FP16 Q, K, V and BF16 dO (AttentionDescriptor+Precisions.swift:13-23); the
-        # kernels rewrite the staged dO tiles as FP16 on chip (tcgen05 kind::f16 cannot mix FP16 and BF16 operands)
+        # kernels rewrite the staged dO tiles as FP16 on chip (wgmma cannot mix FP16 and BF16 operands)
         assert not bf16
         prec = desc.memoryPrecisions
         assert prec[mfa.AttentionOperand.Q] == mfa.GEMMOperandPrecision.FP16
@@ -76,7 +75,7 @@ def test_backward_fp16_matches_oracle(R, C, D):
 @pytest.mark.parametrize("R,C,D,bf16,referencePolicy", [(700, 900, 128, True, False), (900, 700, 64, False, True),
                                                         (2048, 2048, 128, True, False), (1000, 520, 72, False, False)])
 def test_backward_traversal_split_small_grids(R, C, D, bf16, referencePolicy):
-    """Few CTAs for 148 SMs: the traversal axis (keys for dQ, queries for dK/dV) is cut into ranges handled by separate
+    """Few CTAs for 132 SMs: the traversal axis (keys for dQ, queries for dK/dV) is cut into ranges handled by separate
     CTAs whose partial accumulators a sum kernel adds up; ragged last ranges, ragged last blocks."""
     import mfa_b200 as mfa
     desc = mfa.AttentionDescriptor()
@@ -110,7 +109,7 @@ def test_backward_reference_policy_fp16_inputs_bf16_dO(R, C, D, lowMid):
 
 @pytest.mark.gpu
 def test_config3_fwd_bwd_n2048_d64():
-    """BASELINE.json configs[2]: forward + backward (dQ, dK/dV) N=2048 D=64 on one B200 through the tensor-core family:
+    """BASELINE.json configs[2]: forward + backward (dQ, dK/dV) N=2048 D=64 on one H100 through the tensor-core family:
     the reference's policy (FP16 Q/K/V + BF16 dO, as the reference would run "fp16"), all-FP16 and all-BF16."""
     _run(2048, 2048, 64, False, seed=2, referencePolicy=True)
     _run(2048, 2048, 64, False, seed=0)
@@ -126,13 +125,14 @@ def test_every_compiled_table_variant_matches_the_oracle(D):
     import mfa_b200 as mfa
     KT = mfa.AttentionKernelType
     resident = {KT.forward: "Q, O", KT.backwardQuery: "Q, dO, dQ", KT.backwardKeyValue: "K, V, dV, dK"}
-    par = {KT.forward: 256, KT.backwardQuery: 128, KT.backwardKeyValue: 128}
+    par = {KT.forward: 128, KT.backwardQuery: 128, KT.backwardKeyValue: 128}
+    trav = {KT.forward: 128, KT.backwardQuery: 64, KT.backwardKeyValue: 64}
     try:
         for q in range(4):
             for policy in ((2, 8), (4, 3)):
                 for t in KT:
                     qq = min(q, mfa.maxExp2FmaQuarters(t))
-                    mfa.setParameterTable(t, f"| 128 | {par[t]} | 128 | 128 | {resident[t]} | {qq} | {policy[0]} | {policy[1]} |\n")
+                    mfa.setParameterTable(t, f"| 128 | {par[t]} | {trav[t]} | 128 | {resident[t]} | {qq} | {policy[0]} | {policy[1]} |\n")
                 _run(1024, 1536, D, True, seed=q + D)
             _run(200, 333, D, False, seed=q + D + 1, referencePolicy=True)
     finally:
@@ -175,7 +175,7 @@ def test_persistent_backward_many_items_per_cta():
 @pytest.mark.parametrize("policy", ["reference", "bf16"])
 def test_head_dimensions_that_are_not_multiples_of_8_run_on_the_tensor_cores(R, C, D, policy):
     """16-bit operands with D % 8 != 0 (the reference's own shapes: D = 35, 77, 95, ... SquareAttentionTest.swift:6-25) are
-    staged with pad8(D) zero-padded columns and run on the tcgen05 kernels (kernels/pad_head.cu); outputs come back
+    staged with pad8(D) zero-padded columns and run on the tensor-core kernels (kernels/pad_head.cu); outputs come back
     un-padded, and nothing is written past them (the harness checks the poisoned tails)."""
     _run(R, C, D, policy == "bf16", seed=R + C + D, referencePolicy=policy == "reference")
 
@@ -199,7 +199,7 @@ def test_padded_forward_beyond_the_backward_kernels_reach():
     assert _rel_rms(out["O"], O) <= 1e-3
 
 
-# ---- layout-generic / wide-head kernels (tcgen05_backward_generic.cu): 128 < D <= 256, transposed operands ----
+# ---- wide heads (128 < D <= 256) and transposed (staged) operands ----
 WIDE_SHAPES = [(256, 256, 256), (200, 333, 192), (77, 129, 136), (1, 1, 136), (512, 640, 256), (130, 64, 160),
                (64, 1000, 256)]
 
@@ -208,7 +208,7 @@ WIDE_SHAPES = [(256, 256, 256), (200, 333, 192), (77, 129, 136), (1, 1, 136), (5
 @pytest.mark.parametrize("R,C,D", WIDE_SHAPES)
 @pytest.mark.parametrize("mode", ["bf16", "fp16", "reference"])
 def test_backward_wide_heads_match_oracle(R, C, D, mode):
-    """128 < D <= 256 on the tensor cores: 64-row traversal blocks, dK / dV as two passes."""
+    """128 < D <= 256 on the tensor cores: 64-row tiles, dK / dV columns split over the two warpgroups."""
     _run(R, C, D, mode == "bf16", seed=R + 5 * C + D, referencePolicy=mode == "reference")
 
 
@@ -217,7 +217,7 @@ def test_backward_wide_heads_match_oracle(R, C, D, mode):
 @pytest.mark.parametrize("R,C,D", [(136, 200, 64), (256, 384, 128), (200, 136, 256)])
 def test_backward_transposed_operands_match_oracle(R, C, D, mask):
     """Every transpose state (Q, K, V, O; dO / dQ / dK / dV follow their primal, AttentionKernel.swift:189-195) through
-    the layout-generic backward kernels; the forward runs its own layout-generic kernel."""
+    the tensor-core kernels (operands staged row-major first)."""
     t = tuple(bool(mask & (1 << i)) for i in range(4))
     bf16 = bool(mask & 1)
     _run(R, C, D, bf16, seed=mask + R, transpose=t, referencePolicy=(not bf16) and mask % 4 == 2)
@@ -232,8 +232,8 @@ def test_backward_transposed_low_precision_intermediates():
 @pytest.mark.parametrize("R,C,D,transpose", [(1024, 1024, 256, (False,) * 4), (904, 712, 256, (True, True, False, True)),
                                              (2048, 2048, 128, (False, True, True, False))])
 def test_backward_generic_traversal_split(R, C, D, transpose):
-    """Few CTAs: the generic kernels split the traversal axis like the D <= 128 ones, each pass with its own
-    deterministic merge."""
+    """Few CTAs, wide heads and transposed operands: the traversal axis is split as for D <= 128, with one
+    deterministic merge per kernel; transposed operands add one staging copy each."""
     import mfa_b200 as mfa
     desc = mfa.AttentionDescriptor()
     desc.lowPrecisionInputs = True
@@ -242,10 +242,16 @@ def test_backward_generic_traversal_split(R, C, D, transpose):
     desc.transposeState = transpose
     constants = mfa.FunctionConstantValues()
     desc.setFunctionConstants(constants)
-    assert mfa.AttentionKernel(desc.kernelDescriptor(mfa.AttentionKernelType.backwardQuery)).launchCount(constants) == 2
-    # D <= 128: dK and dV in one pass (+ one merge); beyond, the dV pass and the dK pass, each with its merge
+    # a transposed operand is copied row-major before the kernel (an output: back after it); derived operands follow
+    # their primal (dQ ~ Q, dK ~ K, dV ~ V, dO ~ O)
+    t = dict(zip("QKVO", transpose))
+    staged_q = 2 * t["Q"] + t["K"] + t["V"] + 2 * t["O"]     # Q, dQ, K, V, O, dO
+    staged_kv = t["Q"] + 2 * t["K"] + 2 * t["V"] + t["O"]    # Q, K, dK, V, dV, dO
+    # kernel + sum of the split partials (dK and dV in one pass at every D)
+    assert mfa.AttentionKernel(desc.kernelDescriptor(mfa.AttentionKernelType.backwardQuery)).launchCount(constants) == (
+        2 + staged_q)
     assert mfa.AttentionKernel(desc.kernelDescriptor(mfa.AttentionKernelType.backwardKeyValue)).launchCount(constants) == (
-        4 if D > 128 else 2)
+        2 + staged_kv)
     _run(R, C, D, True, seed=R + C, transpose=transpose)
 
 

@@ -1,12 +1,11 @@
-"""Parity of the tensor-core forward (TMA + tcgen05 + TMEM) with the CPU oracle.
+"""Parity of the tensor-core forward (TMA + wgmma) with the CPU oracle.
 
 The oracle runs on the inputs AFTER rounding to the kernel's 16-bit memory format, so the comparison
 isolates the kernel's own arithmetic.  Stated tolerances (north_star: "within 1e-3 relative"):
   O : relative RMS error  rms(O - O_ref) / rms(O_ref) <= 3e-4 for FP16 and <= 2e-3 for BF16.  These are the
       quantisation floors of P, the A operand of O += P V, which is rounded to the MMA input type: round-to-nearest with
       s significant bits has a relative error uniform in +-2^-s / (1 + f), rms 2^-s / sqrt(6) -- 1.99e-4 for FP16
-      (s = 11), 1.59e-3 for BF16 (s = 8) -- and the row sum does not average it away relative to O.  Measured
-      (profiles/r2_parity.jsonl): 1.98e-4 and 1.59e-3 at N = 4096, D = 128.  And element-wise
+      (s = 11), 1.59e-3 for BF16 (s = 8) -- and the row sum does not average it away relative to O.  And element-wise
       |err| <= eps_P * max|V| + 1e-5 with eps_P = 2^-8 (bf16) or 2^-10 (fp16): P is rounded to the 16-bit MMA
       input type before O += P V, so each element carries at most half an ulp of P times the V it multiplies
       (the bound is reached when C is tiny and nothing averages out);
@@ -70,7 +69,7 @@ def test_forward_matches_oracle(R, C, D, bf16):
 SPLIT_KV_CASES = [(4096, 4096, 128, True),   # 16 items x 8 splits: the headline single head
                   (256, 2048, 64, False),    # 1 item x 4 splits
                   (300, 2000, 128, True),    # ragged rows and a ragged last key block
-                  (512, 1536, 96, True),     # 12 key blocks -> 3 splits: uneven row slices in the fused merge
+                  (512, 1536, 96, True),     # 12 key blocks -> 3 splits
                   (1, 4096, 128, False),     # a single query row
                   (2048, 2048, 64, True)]    # BASELINE configs[2] shape
 
@@ -79,10 +78,10 @@ SPLIT_KV_CASES = [(4096, 4096, 128, True),   # 16 items x 8 splits: the headline
 @pytest.mark.parametrize("fused", [True, False], ids=["fused-one-launch", "scratch-combine"])
 @pytest.mark.parametrize("R,C,D,bf16", SPLIT_KV_CASES)
 def test_split_kv_small_grids(R, C, D, bf16, fused):
-    """Few (head, tile pair) items: the key axis is split across SMs.  Default form: normalised partials in the library's
-    workspace + the combine kernel (2 launches); one-launch form: every split CTA publishes its raw partial, waits on the
-    tile pair's arrival counter and merges a slice of the rows inside the attention kernel.  Both must match the oracle, also
-    when run back to back (the fused form must leave its counters at zero)."""
+    """Few (head, query tile) items: the key axis is split across SMs.  Default form: normalised partials in the library's
+    workspace + the merge kernel (2 launches); one-launch form: the split CTA of a tile that arrives last on the tile's
+    counter merges the tile's rows inside the attention kernel.  Both must match the oracle, also when run back to back
+    (the one-launch form must leave its counters at zero)."""
     import mfa_b200 as mfa
     desc = _descriptor(R, C, D, bf16)
     kernel = mfa.AttentionKernel(desc.kernelDescriptor(mfa.AttentionKernelType.forward))
@@ -94,7 +93,7 @@ def test_split_kv_small_grids(R, C, D, bf16, fused):
         _run_and_check(R, C, D, bf16, seed=R + C + D)
         _run_and_check(R, C, D, bf16, seed=R + C + D + 1)
     finally:
-        mfa._lib.mfa_debug_set_forward_fused(0)   # library default: scratch + combine (measured faster)
+        mfa._lib.mfa_debug_set_forward_fused(0)   # library default: scratch + combine (two launches)
 
 
 @pytest.mark.gpu
@@ -146,7 +145,7 @@ def test_config2_full_size_bf16_n4096_d128():
 
 @pytest.mark.gpu
 def test_config4_large_head_bf16_n8192_d256():
-    """BASELINE.json configs[3]: the large-D path, forward bf16 N=8192 D=256 (one tile per CTA, O in 256 TMEM columns)."""
+    """BASELINE.json configs[3]: the large-D path, forward bf16 N=8192 D=256 (O in 64 x 256 register accumulators per warpgroup)."""
     errO, errL = _run_and_check(8192, 8192, 256, True, seed=4, threads=64)
     print(f"config4 max|dO|={errO:.3e} max|dL|={errL:.3e}")
 
@@ -174,9 +173,8 @@ def test_adversarial_growing_max_forces_rescale():
 @pytest.mark.gpu
 @pytest.mark.parametrize("C", [512, 417, 33])
 def test_adversarial_growing_max_large_head(C):
-    """Same adversarial construction on the 128 < D <= 256 kernel, whose rows are split over two warps that take the
-    rescale decision jointly (named barrier with OR reduction) and rescale half of the O columns each; the ragged
-    column counts put the masked tail into one warp's half only."""
+    """Same adversarial construction on the 128 < D <= 256 kernel (64-key blocks); the ragged column counts put the
+    masked tail into the last block."""
     import mfa_b200 as mfa
     import oracle
     from tests.attention_harness import run_attention, check
@@ -201,8 +199,8 @@ def test_adversarial_growing_max_large_head(C):
 @pytest.mark.parametrize("mask", range(1, 16))
 def test_forward_transposed_operands(R, C, D, mask):
     """Every combination of transposed Q, K, V, O (stored [D][seq], AttentionKernel.swift:189-195;
-    RectangularAttentionTest.swift:88-138) on the layout-generic tensor-core kernel: transposed Q / K tiles are MN-major
-    MMA operands, a transposed V is K-major, a transposed O is stored straight from registers."""
+    RectangularAttentionTest.swift:88-138) on the tensor-core kernel: transposed operands are staged row-major first and O
+    is copied back transposed."""
     import mfa_b200 as mfa
     import oracle
     from tests.attention_harness import run_attention, check
@@ -213,7 +211,7 @@ def test_forward_transposed_operands(R, C, D, mask):
     desc = _descriptor(R, C, D, bf16)
     desc.transposeState = tuple(bool(mask & (1 << i)) for i in range(4))
     kd = desc.kernelDescriptor(mfa.AttentionKernelType.forward)
-    assert kd.backend == mfa.Backend.tcgen05 and kd.blockDimensions[:2] == (128, 128)
+    assert kd.backend == mfa.Backend.tcgen05 and kd.blockDimensions[:2] == (128, 128 if D <= 128 else 64)
     net = oracle.Network(R, C, D, seed=mask + R, threads=8)
     net.round_inputs(oracle.BF16 if bf16 else oracle.FP16)
     out = run_attention(desc, net, types=[mfa.AttentionKernelType.forward])

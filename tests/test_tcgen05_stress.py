@@ -2,7 +2,7 @@
 every D % 8 == 0, the three 16-bit operand policies, small batches -- chosen so that the split paths (forward split-KV,
 backward traversal split, ragged last ranges), the D <= 256 kernel's masked tails and the reference-policy dO conversion
 all get exercised against the CPU oracle; a second list draws random transpose states (sequence lengths rounded to
-multiples of 8, which the transposed TMA views need) for the layout-generic kernels.  Tolerances as in test_tcgen05_forward.py / test_tcgen05_backward.py."""
+multiples of 8, which the transposed TMA views need) for the staged (transposed) path.  Tolerances as in test_tcgen05_forward.py / test_tcgen05_backward.py."""
 import numpy as np
 import pytest
 
