@@ -140,9 +140,9 @@ MFA_API int mfa_attention_descriptor_register_precision(const mfa_attention_desc
 /* ------------------------------------------------------------------------------------------ */
 typedef enum mfa_backend {
   MFA_BACKEND_SIMT_FP32 = 0, /* CUDA-core FP32 FMA kernels: any R, C, D <= 512, any transposes/precisions */
-  MFA_BACKEND_TCGEN05 = 1    /* TMA + wgmma kernels: 16-bit inputs, D % 8 == 0; forward D <= 256 (transposed
-                                operands too, where the transposed row pitch is a multiple of 16 bytes), backward D <= 128
-                                row-major */
+  MFA_BACKEND_TCGEN05 = 1    /* TMA + wgmma kernels: 16-bit inputs, pad8(D) <= 256 for all three kernel types
+                                (transposed operands too, with D % 8 == 0, where the transposed row pitch is a multiple
+                                of 16 bytes) */
 } mfa_backend_t;
 
 typedef struct mfa_attention_kernel_descriptor {
@@ -159,7 +159,7 @@ typedef struct mfa_attention_kernel_descriptor {
   /* memoryPrecisions / registerPrecisions; 0xFF = no entry                           :17,25 */
   uint8_t memory_precisions[MFA_OPERAND_COUNT];
   uint8_t register_precisions[MFA_OPERAND_COUNT];
-  /* preferAsyncCache / preferAsyncLoad: 0 false, 1 true, 0xFF nil.  On B200 "async" means the
+  /* preferAsyncCache / preferAsyncLoad: 0 false, 1 true, 0xFF nil.  On H100 "async" means the
      TMA (cp.async.bulk.tensor) path; both are true for MFA_BACKEND_TCGEN05.          :20,23 */
   uint8_t prefer_async_cache, prefer_async_load;
   /* transposeState: bit i set <=> operand i is stored [D][seq] (leading dim = seq).   :27-42 */
@@ -170,10 +170,7 @@ typedef struct mfa_attention_kernel_descriptor {
   /* ---- library extension: which sm_90a kernel family the heuristic picked ---- */
   uint8_t backend; /* mfa_backend_t */
   /* ---- library extension: the tuning columns of the parameter-table row (tensor-core family).  Like blockDimensions
-     they are plain data the caller may edit before AttentionKernel(descriptor:); kernel creation accepts
-     exp2_fma_quarters <= mfa_max_exp2_fma_quarters(type) and rejects the rest. ---- */
-  uint8_t exp2_fma_quarters; /* of every 4 element pairs of P, how many should take exp2 on the FMA pipe; validated and
-                                carried -- the sm_90a kernels take every exp2 on the MUFU pipe */
+     they are plain data the caller may edit before AttentionKernel(descriptor:). ---- */
   uint8_t split_min_blocks;  /* small grids: a traversal range handed to one CTA has at least this many traversal
                                 blocks (blockDimensions.traversal rows each); 0 = never split */
   uint8_t split_max;         /* small grids: at most this many ranges per tile (forward <= 16, backward <= 8) */
@@ -189,7 +186,7 @@ MFA_API int mfa_attention_kernel_descriptor_get_precision(const mfa_attention_ke
 MFA_API void mfa_attention_kernel_descriptor_set_precision(mfa_attention_kernel_descriptor_t *kernel_descriptor,
                                                            mfa_operand_t operand, int register_file, int value);
 
-/** descriptor.kernelDescriptor(type:)  (AttentionDescriptor.swift:33-130): looks up the B200
+/** descriptor.kernelDescriptor(type:)  (AttentionDescriptor.swift:33-130): looks up the H100
  *  parameter table for (type, precision class), picks the first row with head <= max head
  *  (AttentionDescriptor+Parameters.swift:41-66), clamps the head block to pad8(D) (:41-54),
  *  validates the cached-operand list (:56-86) and mirrors the transposes onto dO/dV/dK/dQ
@@ -200,23 +197,19 @@ MFA_API int mfa_attention_descriptor_kernel_descriptor(const mfa_attention_descr
 
 /** The parameter table text that kernelDescriptor(type:) would parse for this descriptor -- the analogue of
  *  AttentionDescriptor.parameterFile(type:) (AttentionDescriptor+Parameters.swift:13-39).  Rows are the reference's
- *  "| maxD | par | trav | head | cached |" with, for the tcgen05 family, three tuning columns appended:
- *  "| exp2 on the FMA pipe (quarters) | min blocks per split | max splits |".  The returned pointer stays valid until
- *  the table is replaced. */
+ *  "| maxD | par | trav | head | cached |" with, for the tcgen05 family, two tuning columns appended:
+ *  "| min blocks per split | max splits |".  The returned pointer stays valid until the table is replaced. */
 MFA_API const char *mfa_attention_descriptor_parameter_file(const mfa_attention_descriptor_t *descriptor,
                                                             mfa_kernel_type_t type);
 
 /** The tables are DATA: this replaces the tensor-core-family table of `type` (`transposed` != 0: the table used with transposed operands, i.e. of the
  *  layout-generic kernels) with `text` in the format above; NULL restores the built-in table.  The text is
- *  parsed and validated first (unknown operand names, malformed rows, tuning values without a compiled kernel are
+ *  parsed and validated first (unknown operand names, malformed rows and rows without the two tuning columns are
  *  rejected and the current table stays).  Kernels fetched from the descriptor-keyed cache afterwards follow the new
  *  table.  At load time the library also reads the file named by the environment variable MFA_B200_PARAMETER_FILE
  *  (sections "[forward]", "[backwardQuery]", "[backwardKeyValue]", each also as "[....transposed]"; parameters/h100.txt is
  *  one).  Not thread-safe against concurrent kernelDescriptor() calls. */
 MFA_API int mfa_set_parameter_table(mfa_kernel_type_t type, int transposed, const char *text);
-/** Largest exp2_fma_quarters the tables accept for `type` (validated and carried; the sm_90a kernels take every exp2 on
- *  the MUFU pipe). */
-MFA_API int mfa_max_exp2_fma_quarters(mfa_kernel_type_t type);
 
 /** descriptor.setFunctionConstants(_:)  (AttentionDescriptor.swift:139-148): the two launch-time
  *  constants R (index 0) and C (index 1), plus the batch extension. */
@@ -270,8 +263,10 @@ MFA_API int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel,
                                         const mfa_function_constants_t *constants,
                                         void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
 
-/** Number of CUDA kernels one encode() launches (1; +1 when a small grid is split along the traversal axis and a
- *  merge kernel follows: split-KV combine for the forward, a plain sum of partial accumulators for dQ and dK/dV). */
+/** Number of CUDA kernels one encode() launches.  Per slice of at most 16384 problems of the batch: 1; +1 when a small
+ *  grid is split along the traversal axis and a merge kernel follows (split-KV combine for the forward, a plain sum of
+ *  partial accumulators for dQ and dK/dV); +1 per operand staged row-major (head % 8 != 0 or stored transposed) and
+ *  per output copied back from such a staging buffer; +1 when dK/dV converts a BF16 dO to FP16 in a pass of its own. */
 MFA_API int mfa_attention_kernel_launch_count(const mfa_attention_kernel_t *kernel,
                                               const mfa_function_constants_t *constants, uint32_t *out);
 

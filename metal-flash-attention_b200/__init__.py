@@ -82,7 +82,6 @@ class _CKernelDescriptor(ctypes.Structure):
         ("transpose_state_mask", ctypes.c_uint16),
         ("type", ctypes.c_uint8),
         ("backend", ctypes.c_uint8),
-        ("exp2_fma_quarters", ctypes.c_uint8),
         ("split_min_blocks", ctypes.c_uint8),
         ("split_max", ctypes.c_uint8),
     ]
@@ -182,10 +181,6 @@ def setParameterTable(type: "AttentionKernelType", text: Optional[str], transpos
     """mfa_set_parameter_table: replace (text) or restore (None) the tensor-core-family parameter table of `type`."""
     _check(_lib.mfa_set_parameter_table(int(type), int(bool(transposed)),
                                         None if text is None else text.encode()))
-
-
-def maxExp2FmaQuarters(type: "AttentionKernelType") -> int:
-    return _lib.mfa_max_exp2_fma_quarters(int(type))
 
 
 def library_path() -> str:
@@ -441,15 +436,6 @@ class AttentionKernelDescriptor:
 
     # ---- library extension: the tuning columns of the parameter-table row (plain, editable data like blockDimensions)
     @property
-    def exp2FmaQuarters(self) -> int:
-        """Of every 4 element pairs of P, how many take exp2 on the FMA pipe: selects the kernel instantiation."""
-        return self._c.exp2_fma_quarters
-
-    @exp2FmaQuarters.setter
-    def exp2FmaQuarters(self, value):
-        self._c.exp2_fma_quarters = int(value)
-
-    @property
     def splitPolicy(self) -> Tuple[int, int]:
         """(minimum blocks per traversal range, maximum ranges) for small grids; minimum 0 = never split."""
         return (self._c.split_min_blocks, self._c.split_max)
@@ -541,5 +527,5 @@ class AttentionKernel:
 __all__ = [
     "AttentionDescriptor", "AttentionKernelDescriptor", "AttentionKernel", "AttentionKernelType",
     "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError",
-    "library_path", "version", "setParameterTable", "maxExp2FmaQuarters", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
+    "library_path", "version", "setParameterTable", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
 ]

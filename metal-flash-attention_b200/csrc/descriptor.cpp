@@ -105,10 +105,9 @@ int register_precision(const mfa_attention_descriptor_t &d, int operand) {
 //     that stay in shared memory / registers for the entire traversal.
 //   * SIMT family: 64 x 64 blocks, 32-wide head chunks, accumulators resident in registers.
 // ------------------------------------------------------------------------------------------------
-// Tensor-core rows carry three tuning columns after the reference's five:
-//     | exp2 on the FMA pipe (quarters of the element pairs) | min blocks per split | max splits |
-// The exp2 column is validated and carried (every exp2 of the sm_90a kernels runs on the MUFU pipe).  The split
-// columns govern small grids: the forward cuts every query tile's key axis into equal ranges of at least `min blocks`
+// Tensor-core rows carry two tuning columns after the reference's five:
+//     | min blocks per split | max splits |
+// They govern small grids: the forward cuts every query tile's key axis into equal ranges of at least `min blocks`
 // key blocks and merges the partials (split-KV); the backward kernels cut their traversal axis likewise and sum the
 // partial gradients.  0 min blocks turns splitting off.
 //   forward: 128 query rows per CTA (two warpgroups); 128-key blocks up to D = 128, 64-key blocks beyond
@@ -116,28 +115,28 @@ int register_precision(const mfa_attention_descriptor_t &d, int operand) {
 //   backwardKeyValue: 128 key rows per CTA up to D = 128, 64 beyond (dK / dV columns split over two warpgroups);
 //   64-query blocks
 // Transposed operands are staged row-major first and run the same kernels.
-static const char *kForwardTcgen05 =
-    "| 64  | 128 | 128 | 64  | Q, O | 0 | 2 | 8 |\n"
-    "| 128 | 128 | 128 | 128 | Q, O | 0 | 4 | 8 |\n"
-    "| 256 | 128 | 64  | 256 | Q, O | 0 | 0 | 1 |\n"
+static const char *kForwardWgmma =
+    "| 64  | 128 | 128 | 64  | Q, O | 2 | 8 |\n"
+    "| 128 | 128 | 128 | 128 | Q, O | 4 | 8 |\n"
+    "| 256 | 128 | 64  | 256 | Q, O | 0 | 1 |\n"
     "\n";
-static const char *kForwardTcgen05Transposed =
-    "| 64  | 128 | 128 | 64  | Q, O | 0 | 0 | 1 |\n"
-    "| 128 | 128 | 128 | 128 | Q, O | 0 | 0 | 1 |\n"
-    "| 256 | 128 | 64  | 256 | Q, O | 0 | 0 | 1 |\n"
+static const char *kForwardWgmmaTransposed =
+    "| 64  | 128 | 128 | 64  | Q, O | 0 | 1 |\n"
+    "| 128 | 128 | 128 | 128 | Q, O | 0 | 1 |\n"
+    "| 256 | 128 | 64  | 256 | Q, O | 0 | 1 |\n"
     "\n";
-static const char *kBackwardQueryTcgen05 =
-    "| 64  | 128 | 64  | 64  | Q, dO, dQ | 0 | 2 | 8 |\n"
-    "| 128 | 128 | 64  | 128 | Q, dO, dQ | 0 | 2 | 8 |\n"
-    "| 256 | 64  | 64  | 256 | Q, dO, dQ | 0 | 2 | 8 |\n"
+static const char *kBackwardQueryWgmma =
+    "| 64  | 128 | 64  | 64  | Q, dO, dQ | 2 | 8 |\n"
+    "| 128 | 128 | 64  | 128 | Q, dO, dQ | 2 | 8 |\n"
+    "| 256 | 64  | 64  | 256 | Q, dO, dQ | 2 | 8 |\n"
     "\n";
-static const char *kBackwardKeyValueTcgen05 =
-    "| 64  | 128 | 64  | 64  | K, V, dV, dK | 0 | 2 | 8 |\n"
-    "| 128 | 128 | 64  | 128 | K, V, dV, dK | 0 | 2 | 8 |\n"
-    "| 256 | 64  | 64  | 256 | K, V, dV, dK | 0 | 2 | 8 |\n"
+static const char *kBackwardKeyValueWgmma =
+    "| 64  | 128 | 64  | 64  | K, V, dV, dK | 2 | 8 |\n"
+    "| 128 | 128 | 64  | 128 | K, V, dV, dK | 2 | 8 |\n"
+    "| 256 | 64  | 64  | 256 | K, V, dV, dK | 2 | 8 |\n"
     "\n";
-static const char *kBackwardQueryTcgen05Transposed = kBackwardQueryTcgen05;
-static const char *kBackwardKeyValueTcgen05Transposed = kBackwardKeyValueTcgen05;
+static const char *kBackwardQueryWgmmaTransposed = kBackwardQueryWgmma;
+static const char *kBackwardKeyValueWgmmaTransposed = kBackwardKeyValueWgmma;
 static const char *kForwardSimt =
     "| 512 | 64 | 64 | 32 | O |\n"
     "\n";
@@ -155,29 +154,29 @@ static bool any_transpose(const mfa_attention_descriptor_t &d) {
   return d.transpose_Q || d.transpose_K || d.transpose_V || d.transpose_O;
 }
 
+// Transposed operands are staged row-major where the transposed view has a 16-byte row pitch (sequence length % 8 ==
+// 0): Q^T and (backward only) dO^T, which follows O, are addressed through R, K^T and V^T through C.
+static bool transposes_ok(const mfa_attention_descriptor_t &d, int type) {
+  return (!d.transpose_Q || d.row % 8 == 0) && (!d.transpose_K || d.column % 8 == 0) &&
+         (!d.transpose_V || d.column % 8 == 0) && (type == MFA_FORWARD || !d.transpose_O || d.row % 8 == 0);
+}
+
 int select_backend(const mfa_attention_descriptor_t &d, int type) {
   if (!d.low_precision_inputs || d.head == 0) return MFA_BACKEND_SIMT_FP32;
   const uint32_t padded = (static_cast<uint32_t>(d.head) + 7) / 8 * 8;
   if (any_transpose(d)) {
-    // transposed operands: staged row-major for the tensor-core kernels where the transposed view has a 16-byte row
-    // pitch (sequence length a multiple of 8 elements)
-    const bool ok = type == MFA_FORWARD
-                        ? tcgen05_forward_transposes_ok(d.row, d.column, d.transpose_Q, d.transpose_K, d.transpose_V)
-                        : tcgen05_backward_transposes_ok(d.row, d.column, d.transpose_Q, d.transpose_K, d.transpose_V,
-                                                         d.transpose_O);
-    if (!ok) return MFA_BACKEND_SIMT_FP32;
+    if (!transposes_ok(d, type)) return MFA_BACKEND_SIMT_FP32;
     if (d.head % 8 != 0) return MFA_BACKEND_SIMT_FP32;  // (head-dimension padding is implemented for row-major operands)
   }
   // D % 8 != 0 (row-major): the operands are staged with pad8(D) columns (kernels/pad_head.cu) and the tensor-core kernels
   // run at the padded head dimension -- the reference's zero-padded async copies (+OuterProduct.swift:237-254)
-  const uint32_t maxHead = (type == MFA_FORWARD) ? tcgen05_forward_max_head() : tcgen05_backward_max_head();
-  if (padded > maxHead) return MFA_BACKEND_SIMT_FP32;
+  if (padded > kWgmmaMaxHead) return MFA_BACKEND_SIMT_FP32;
   // (the reference's own policy, FP16 Q/K/V + BF16 dO, is served too: wgmma cannot mix element types
   // inside one MMA, so the backward kernels rewrite the staged dO tile as FP16 in shared memory)
   return MFA_BACKEND_TCGEN05;
 }
 
-// The tcgen05 tables are data: mfa_set_parameter_table() / MFA_B200_PARAMETER_FILE replace them at run time.
+// The tensor-core tables are data: mfa_set_parameter_table() / MFA_B200_PARAMETER_FILE replace them at run time.
 // slot 0 forward, 2 backwardQuery, 4 backwardKeyValue; +1: the table used with transposed operands; empty = built-in
 static std::string g_table_override[kTableSlots];
 static bool g_table_overridden[kTableSlots] = {false, false, false, false, false, false};
@@ -186,12 +185,12 @@ unsigned parameter_table_generation() { return g_table_generation; }
 
 static const char *builtin_table(int slot) {
   switch (slot) {
-    case 0: return kForwardTcgen05;
-    case 1: return kForwardTcgen05Transposed;
-    case 2: return kBackwardQueryTcgen05;
-    case 3: return kBackwardQueryTcgen05Transposed;
-    case 4: return kBackwardKeyValueTcgen05;
-    default: return kBackwardKeyValueTcgen05Transposed;
+    case 0: return kForwardWgmma;
+    case 1: return kForwardWgmmaTransposed;
+    case 2: return kBackwardQueryWgmma;
+    case 3: return kBackwardQueryWgmmaTransposed;
+    case 4: return kBackwardKeyValueWgmma;
+    default: return kBackwardKeyValueWgmmaTransposed;
   }
 }
 static int table_slot(int type, bool transposed) {
@@ -216,7 +215,7 @@ struct ParameterRow {
   unsigned maximumHeadDimension = 0;
   std::string parallelization, traversal, head, cachedOperands;
   // tuning columns (present in the tensor-core tables; empty = defaults)
-  std::string exp2FmaQuarters, splitMinBlocks, splitMax;
+  std::string splitMinBlocks, splitMax;
 };
 
 static std::string strip_spaces(const std::string &s) {
@@ -245,7 +244,7 @@ static int parse_table(const char *file, std::vector<ParameterRow> &rows) {
       if (!seg.empty()) segments.push_back(strip_spaces(seg));
       p = bar + 1;
     }
-    if (segments.size() != 5 && segments.size() != 8)  // the reference's five columns, or five + three tuning columns
+    if (segments.size() != 5 && segments.size() != 7)  // the reference's five columns, or five + two tuning columns
       return fail(MFA_ERROR_INVALID_ARGUMENT, "Number of segments was invalid: " + std::to_string(segments.size()));
     ParameterRow row;
     char *end = nullptr;
@@ -257,10 +256,9 @@ static int parse_table(const char *file, std::vector<ParameterRow> &rows) {
     row.traversal = segments[2];
     row.head = segments[3];
     row.cachedOperands = segments[4];
-    if (segments.size() == 8) {
-      row.exp2FmaQuarters = segments[5];
-      row.splitMinBlocks = segments[6];
-      row.splitMax = segments[7];
+    if (segments.size() == 7) {
+      row.splitMinBlocks = segments[5];
+      row.splitMax = segments[6];
     }
     rows.push_back(row);
   }
@@ -359,16 +357,14 @@ int kernel_descriptor(const mfa_attention_descriptor_t &d, int type, mfa_attenti
   }
 
   out.backend = static_cast<uint8_t>(select_backend(d, type));
-  // tuning columns (tensor-core tables); rows without them (the FP32 family) leave the defaults: no FMA-pipe exp2, no splits
-  out.exp2_fma_quarters = 0;
+  // tuning columns (tensor-core tables); rows without them (the FP32 family) leave the default: no splits
   out.split_min_blocks = 0;
   out.split_max = 1;
-  if (!row->exp2FmaQuarters.empty()) {
-    uint16_t quarters = 0, minBlocks = 0, maxSplits = 0;
-    if (!parse_u16(row->exp2FmaQuarters, quarters) || !parse_u16(row->splitMinBlocks, minBlocks) ||
-        !parse_u16(row->splitMax, maxSplits) || quarters > 4 || minBlocks > 255 || maxSplits > 255)
+  if (!row->splitMinBlocks.empty()) {
+    uint16_t minBlocks = 0, maxSplits = 0;
+    if (!parse_u16(row->splitMinBlocks, minBlocks) || !parse_u16(row->splitMax, maxSplits) || minBlocks > 255 ||
+        maxSplits > 255)
       return fail(MFA_ERROR_INVALID_ARGUMENT, "Could not decode tuning columns.");
-    out.exp2_fma_quarters = static_cast<uint8_t>(quarters);
     out.split_min_blocks = static_cast<uint8_t>(minBlocks);
     out.split_max = static_cast<uint8_t>(maxSplits < 1 ? 1 : maxSplits);
   }
@@ -440,7 +436,7 @@ using namespace mfa;
 extern "C" {
 
 const char *mfa_last_error(void) { return g_last_error.c_str(); }
-const char *mfa_version(void) { return "mfa_b200 0.3 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family)"; }
+const char *mfa_version(void) { return "mfa_b200 0.4 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family)"; }
 
 int mfa_precision_size(mfa_precision_t precision) { return precision == MFA_FP32 ? 4 : 2; }
 const char *mfa_precision_name(mfa_precision_t precision) {
@@ -522,10 +518,6 @@ const char *mfa_attention_descriptor_parameter_file(const mfa_attention_descript
   return parameter_file(*descriptor, type);
 }
 
-int mfa_max_exp2_fma_quarters(mfa_kernel_type_t type) {
-  return type == MFA_FORWARD ? static_cast<int>(kMaxForwardExp2Quarters) : static_cast<int>(kMaxBackwardExp2Quarters);
-}
-
 int mfa_set_parameter_table(mfa_kernel_type_t type, int transposed, const char *text) {
   if (type < MFA_FORWARD || type > MFA_BACKWARD_KEY_VALUE) return fail(MFA_ERROR_INVALID_ARGUMENT, "Unrecognized kernel type.");
   const int slot = table_slot(type, transposed != 0);
@@ -535,7 +527,7 @@ int mfa_set_parameter_table(mfa_kernel_type_t type, int transposed, const char *
     ++g_table_generation;
     return MFA_SUCCESS;
   }
-  // validate before installing: rows parse, operands are the expected ones, tuning values have a compiled kernel
+  // validate before installing: rows parse, operands are the expected ones, tuning values decode
   std::vector<ParameterRow> rows;
   int status = parse_table(text, rows);
   if (status != MFA_SUCCESS) return status;
@@ -552,15 +544,10 @@ int mfa_set_parameter_table(mfa_kernel_type_t type, int transposed, const char *
     for (int operand : operands)  // createCacheState's check (AttentionDescriptor.swift:69-74), applied to every row
       if (!(expected & (1u << operand)))
         return fail(MFA_ERROR_UNEXPECTED_OPERAND, std::string("Unexpected operand: ") + kOperandNames[operand]);
-    if (row.exp2FmaQuarters.empty()) return fail(MFA_ERROR_INVALID_ARGUMENT, "A tensor-core table row needs the three tuning columns.");
-    uint16_t quarters = 0, minBlocks = 0, maxSplits = 0;
-    if (!parse_u16(row.exp2FmaQuarters, quarters) || !parse_u16(row.splitMinBlocks, minBlocks) ||
-        !parse_u16(row.splitMax, maxSplits))
+    if (row.splitMinBlocks.empty()) return fail(MFA_ERROR_INVALID_ARGUMENT, "A tensor-core table row needs the two tuning columns.");
+    uint16_t minBlocks = 0, maxSplits = 0;
+    if (!parse_u16(row.splitMinBlocks, minBlocks) || !parse_u16(row.splitMax, maxSplits))
       return fail(MFA_ERROR_INVALID_ARGUMENT, "Could not decode tuning columns.");
-    if (quarters > static_cast<uint16_t>(mfa_max_exp2_fma_quarters(type)))
-      return fail(MFA_ERROR_UNSUPPORTED, "exp2-on-FMA-pipe fraction " + std::to_string(quarters) +
-                                             "/4 has no compiled kernel (largest: " +
-                                             std::to_string(mfa_max_exp2_fma_quarters(type)) + "/4).");
   }
   g_table_override[slot] = text;
   g_table_overridden[slot] = true;

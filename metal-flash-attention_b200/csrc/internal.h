@@ -18,8 +18,4 @@ const char *parameter_file(const mfa_attention_descriptor_t &d, int type);
 unsigned parameter_table_generation();  // bumped by mfa_set_parameter_table: cached kernels of older tables are stale
 int kernel_descriptor(const mfa_attention_descriptor_t &d, int type, mfa_attention_kernel_descriptor_t &out);
 
-// Largest head dimension the compiled tensor-core kernels cover (kernels/wgmma_attention.cu).
-uint32_t tcgen05_forward_max_head();
-uint32_t tcgen05_backward_max_head();
-
 }  // namespace mfa

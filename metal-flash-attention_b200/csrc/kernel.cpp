@@ -5,7 +5,6 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <map>
 #include <mutex>
@@ -49,12 +48,33 @@ static bool is_output(int type, int slot) {
   return type == MFA_FORWARD ? slot == MFA_O : (type == MFA_BACKWARD_QUERY ? slot == MFA_dQ : (slot == MFA_dV || slot == MFA_dK));
 }
 
-// Whether the tensor-core family copies this operand into a row-major, pad8(D)-column staging buffer: every operand
-// with a head dimension when D % 8 != 0, and any operand stored transposed (L and D are per-row vectors, never staged).
-static bool stages_operand(int type, int slot, bool padded, uint16_t transpose_mask) {
-  if (slot == MFA_L || slot == MFA_D) return false;
-  if (type == MFA_BACKWARD_KEY_VALUE && slot == MFA_O) return false;  // (not read by dK/dV)
-  return padded || ((transpose_mask >> slot) & 1);
+// The operands (bit = buffer slot) the tensor-core family copies into a row-major, pad8(D)-column staging buffer: every
+// operand with a head dimension when D % 8 != 0, and any operand stored transposed (L and D are per-row vectors, never
+// staged).  encode() stages each input and copies each output back: one launch apiece.
+static uint32_t staged_operands(const mfa_attention_kernel *k) {
+  if (k->backend != MFA_BACKEND_TCGEN05) return 0;
+  const bool padded = k->descriptor.head_dimension % 8 != 0;
+  uint32_t mask = 0;
+  int n = 0;
+  const int *ops = operands_of(k->type, &n);
+  for (int i = 0; i < n; ++i)
+    if (ops[i] != MFA_L && ops[i] != MFA_D && (padded || ((k->descriptor.transpose_state_mask >> ops[i]) & 1)))
+      mask |= 1u << ops[i];
+  return mask;
+}
+
+// Several kernels carry the batch in gridDim.y (limit 65535; the SIMT dK/dV kernel multiplies it by up to four head
+// slices): larger batches go out as several launches over slices of the batch -- the problems are independent and
+// stored back to back, so a slice is just a pointer offset.  Calls f(first problem, problems) per slice and stops at
+// the first status other than MFA_SUCCESS.
+template <class F>
+static int for_each_batch_slice(uint32_t batch, F f) {
+  constexpr uint32_t kMaxBatchPerLaunch = 16384;
+  for (uint32_t h0 = 0; h0 < batch; h0 += kMaxBatchPerLaunch) {
+    const int status = f(h0, batch - h0 < kMaxBatchPerLaunch ? batch - h0 : kMaxBatchPerLaunch);
+    if (status != MFA_SUCCESS) return status;
+  }
+  return MFA_SUCCESS;
 }
 
 // sm_90 check of the current device, cached per device ordinal (encode() of a microsecond-scale kernel must not pay
@@ -99,7 +119,6 @@ static int build_params(const mfa_attention_kernel *k, const mfa_function_consta
   p.scale = 1.0f / std::sqrt(static_cast<float>(p.D));
   p.scale_log2 = 1.442695041f * p.scale;
   // the tuning columns of the parameter-table row this kernel was created from
-  p.exp2_fma_quarters = k->descriptor.exp2_fma_quarters;
   p.split_min_blocks = k->descriptor.split_min_blocks;
   p.split_max = k->descriptor.split_max ? k->descriptor.split_max : 1;
   int n = 0;
@@ -152,8 +171,7 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
     const uint8_t pq = kd->memory_precisions[MFA_Q];
     const uint32_t Dp = (D + 7) / 8 * 8;  // D % 8 != 0: operands are staged with pad8(D) columns (kernels/pad_head.cu)
     bool ok = (pq == MFA_FP16 || pq == MFA_BF16) && kd->memory_precisions[MFA_K] == pq &&
-              kd->memory_precisions[MFA_V] == pq &&
-              Dp <= (k->type == MFA_FORWARD ? tcgen05_forward_max_head() : tcgen05_backward_max_head());
+              kd->memory_precisions[MFA_V] == pq && Dp <= kWgmmaMaxHead;
     bool transposed = false;
     for (int i = 0; i < n; ++i)
       if ((kd->transpose_state_mask >> ops[i]) & 1) transposed = true;
@@ -169,18 +187,13 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
                   "type, or BF16 with FP16 Q,K,V) and pad8(head) <= the compiled maximum; use MFA_BACKEND_SIMT_FP32 for this "
                   "descriptor.");
     }
-    // tuning columns: every compiled exp2 variant is accepted, anything else is rejected with the list of what exists
-    const uint32_t max_quarters = k->type == MFA_FORWARD ? kMaxForwardExp2Quarters : kMaxBackwardExp2Quarters;
-    if (kd->exp2_fma_quarters > max_quarters) {
-      delete k;
-      return fail(MFA_ERROR_UNSUPPORTED, "exp2-on-FMA-pipe fraction " + std::to_string(kd->exp2_fma_quarters) +
-                                             "/4 has no compiled sm_90a kernel (available: 0.." +
-                                             std::to_string(max_quarters) + ").");
-    }
-    if (k->type == MFA_FORWARD)
-      tcgen05_forward_geometry(Dp, &k->threads, &k->smem_bytes, &k->par, &k->trav, &k->head);
-    else
-      tcgen05_backward_geometry(k->type, Dp, &k->threads, &k->smem_bytes, &k->par, &k->trav, &k->head);
+    // (only the geometry fields are used: they depend on neither the problem size nor the device)
+    const WgmmaPlan plan = wgmma_plan(k->type, Dp, 1, 1, 1, 0, 1, false, 1);
+    k->threads = plan.threads;
+    k->smem_bytes = plan.smem_bytes;
+    k->par = plan.par;
+    k->trav = plan.trav;
+    k->head = plan.head;
   } else if (k->backend == MFA_BACKEND_SIMT_FP32) {
     if (D > 512) {
       delete k;
@@ -248,21 +261,18 @@ const char *mfa_attention_kernel_source_name(const mfa_attention_kernel_t *kerne
 int mfa_attention_kernel_launch_count(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                       uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  *out = 1;
-  if (kernel->backend != MFA_BACKEND_TCGEN05) return MFA_SUCCESS;
   const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
-  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, b = c->batch_count ? c->batch_count : 1;
-  if (kernel->type == MFA_FORWARD)
-    *out = tcgen05_forward_launch_count(c->row, c->column, Dp, b, d.split_min_blocks, d.split_max);
-  else
-    *out = tcgen05_backward_launch_count(kernel->type, c->row, c->column, Dp, b, d.split_min_blocks, d.split_max,
-                                         d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q]);
-  // staged operands (head % 8 != 0, or stored transposed): one copy per staged input, one per output
-  int n = 0;
-  const int *ops = operands_of(kernel->type, &n);
-  for (int i = 0; i < n; ++i)
-    if (stages_operand(kernel->type, ops[i], d.head_dimension % 8 != 0, d.transpose_state_mask)) *out += 1;
-  return MFA_SUCCESS;
+  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, staged = __builtin_popcount(staged_operands(kernel));
+  const uint32_t sm_count = kernel->backend == MFA_BACKEND_TCGEN05 ? device_sm_count(current_device()) : 0;
+  *out = 0;
+  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, [&](uint32_t, uint32_t batch) -> int {
+    *out += kernel->backend != MFA_BACKEND_TCGEN05
+                ? 1
+                : staged + wgmma_plan(kernel->type, Dp, c->row, c->column, batch, d.split_min_blocks, d.split_max,
+                                      d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q], sm_count)
+                               .launches;
+    return MFA_SUCCESS;
+  });
 }
 
 int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
@@ -275,50 +285,39 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
   if (status != MFA_SUCCESS) return status;
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
 
-  // Several kernels carry the batch in gridDim.y (limit 65535; the SIMT dK/dV kernel multiplies it by up to four head
-  // slices): larger batches go out as several launches over slices of the batch -- the problems are independent and
-  // stored back to back, so a slice is just a pointer offset.
-  constexpr uint32_t kMaxBatchPerLaunch = 16384;
-  const uint32_t batch = p.batch;
+  // Tensor-core family: operands with D % 8 != 0 or a transposed layout are staged row-major with pad8(D) columns, the
+  // kernels run at the padded head dimension (the softmax scale stays 1 / sqrt(D) of the true D), and the FP32 outputs
+  // are copied back to the caller's layout without the padding.
   size_t head_bytes[kSlots];
   for (int slot = 0; slot < kSlots; ++slot) {
     const size_t seq = (slot == sK || slot == sV || slot == sdK || slot == sdV) ? p.C : p.R;
     const size_t elements = (slot == sL || slot == sD) ? seq : seq * p.D;
     head_bytes[slot] = elements * (p.prec[slot] == FP32 ? 4 : 2);
   }
-  // Tensor-core family: operands with D % 8 != 0 or a transposed layout are staged row-major with pad8(D) columns, the
-  // kernels run at the padded head dimension (the softmax scale stays 1 / sqrt(D) of the true D), and the FP32 outputs
-  // are copied back to the caller's layout without the padding.
-  const bool tc = kernel->backend == MFA_BACKEND_TCGEN05;
-  const bool padded = tc && p.D % 8 != 0;
+  const uint32_t staged = staged_operands(kernel);
   const uint32_t Dp = (p.D + 7) / 8 * 8;
-  int n = 0;
-  const int *ops = operands_of(kernel->type, &n);
-  bool staged = false;
-  for (int i = 0; i < n; ++i) staged |= tc && stages_operand(kernel->type, ops[i], padded, kernel->descriptor.transpose_state_mask);
   const int device = staged ? current_device() : 0;
-  for (uint32_t h0 = 0; h0 < batch; h0 += kMaxBatchPerLaunch) {
+  auto seq_of = [&](int slot) -> uint32_t { return (slot == sK || slot == sV || slot == sdK || slot == sdV) ? p.C : p.R; };
+  return for_each_batch_slice(p.batch, [&](uint32_t h0, uint32_t batch) -> int {
     AttentionParams q = p;
-    q.batch = batch - h0 < kMaxBatchPerLaunch ? batch - h0 : kMaxBatchPerLaunch;
+    q.batch = batch;
     for (int slot = 0; slot < kSlots; ++slot)
       if (q.buf[slot]) q.buf[slot] = static_cast<char *>(q.buf[slot]) + head_bytes[slot] * h0;
     cudaError_t e = cudaSuccess;
     void *user_out[kSlots] = {};  // staged outputs: where the caller's copies go
     if (staged) {
-      auto seq_of = [&](int slot) -> uint32_t { return (slot == sK || slot == sV || slot == sdK || slot == sdV) ? p.C : p.R; };
       auto bytes_of = [&](int slot) -> size_t {
         return ((static_cast<size_t>(q.batch) * seq_of(slot) * Dp * (p.prec[slot] == FP32 ? 4 : 2)) + 255) & ~size_t(255);
       };
       size_t total = 0;
-      for (int i = 0; i < n; ++i)
-        if (stages_operand(kernel->type, ops[i], padded, kernel->descriptor.transpose_state_mask)) total += bytes_of(ops[i]);
+      for (int slot = 0; slot < kSlots; ++slot)
+        if ((staged >> slot) & 1) total += bytes_of(slot);
       void *ws = nullptr;
       if ((e = workspace_for(device, stream, total, &ws, /*slot=*/1)) != cudaSuccess)
         return fail(MFA_ERROR_CUDA, std::string("staging workspace: ") + cudaGetErrorString(e) + " " + last_launch_detail());
-      char *cursor = static_cast<char *>(ws) + kWorkspaceCounterBytes;
-      for (int i = 0; i < n && e == cudaSuccess; ++i) {
-        const int slot = ops[i];
-        if (!stages_operand(kernel->type, slot, padded, kernel->descriptor.transpose_state_mask)) continue;
+      char *cursor = static_cast<char *>(ws);
+      for (int slot = 0; slot < kSlots && e == cudaSuccess; ++slot) {
+        if (!((staged >> slot) & 1)) continue;
         if (is_output(kernel->type, slot))
           user_out[slot] = q.buf[slot];
         else
@@ -333,9 +332,9 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
     }
     if (kernel->backend == MFA_BACKEND_TCGEN05) {
       switch (kernel->type) {
-        case MFA_FORWARD: e = launch_tcgen05_forward(q, stream); break;
-        case MFA_BACKWARD_QUERY: e = launch_tcgen05_backward_query(q, stream); break;
-        default: e = launch_tcgen05_backward_key_value(q, stream); break;
+        case MFA_FORWARD: e = launch_wgmma_forward(q, stream); break;
+        case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, stream); break;
+        default: e = launch_wgmma_backward_key_value(q, stream); break;
       }
     } else {
       switch (kernel->type) {
@@ -347,22 +346,14 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
     if (e != cudaSuccess)
       return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " failed: " + cudaGetErrorString(e) +
                                       " " + last_launch_detail());
-    if (staged) {
-      for (int slot = 0; slot < kSlots && e == cudaSuccess; ++slot)
-        if (user_out[slot]) {
-          const uint32_t seq = (slot == sdK || slot == sdV) ? p.C : p.R;
-          e = launch_unstage_output(static_cast<const float *>(q.buf[slot]), static_cast<float *>(user_out[slot]), q.batch,
-                                    seq, p.D, Dp, p.transposed[slot], stream);
-        }
-      if (e != cudaSuccess) return fail(MFA_ERROR_CUDA, std::string("copy-back of staged outputs failed: ") + cudaGetErrorString(e));
-    }
-  }
-  return MFA_SUCCESS;
+    for (int slot = 0; slot < kSlots && e == cudaSuccess; ++slot)
+      if (user_out[slot])
+        e = launch_unstage_output(static_cast<const float *>(q.buf[slot]), static_cast<float *>(user_out[slot]), q.batch,
+                                  seq_of(slot), p.D, Dp, p.transposed[slot], stream);
+    if (e != cudaSuccess) return fail(MFA_ERROR_CUDA, std::string("copy-back of staged outputs failed: ") + cudaGetErrorString(e));
+    return MFA_SUCCESS;
+  });
 }
-
-// Debug-only export (deliberately absent from include/mfa_b200.h): 1 merges split-KV partials inside the attention
-// kernel (one launch), 0 (default) in a second launch (tests cover both forms).
-MFA_API void mfa_debug_set_forward_fused(int enabled) { tcgen05_forward_set_fused(enabled); }
 
 // ------------------------------------------------------------------------------------------------
 // Kernel cache keyed by descriptor -- the useful half of the reference's pipeline cache
@@ -480,11 +471,6 @@ void destroy_scratch(Scratch &s) {
 // (copy launch overheads), at most kMaxChunks chunks, and no chunking at all for a single problem
 uint32_t chunk_heads(uint32_t batch, size_t bytes_per_head) {
   if (batch <= 1) return 1;
-  // tuning knob (chunk-count sweeps of the host-buffer path): MFA_B200_HOST_CHUNKS=<n>
-  if (const char *env = getenv("MFA_B200_HOST_CHUNKS")) {
-    const uint32_t n = static_cast<uint32_t>(atoi(env));
-    if (n >= 1 && n <= kMaxChunks) return (batch + n - 1) / n;
-  }
   uint32_t heads = (batch + 15) / 16;
   const size_t kMinChunkBytes = size_t(4) << 20;
   if (bytes_per_head * heads < kMinChunkBytes)
@@ -583,8 +569,7 @@ int mfa_attention_run_host(const mfa_attention_descriptor_t *descriptor, uint32_
   // per-row statistics (L, D: a few KB per head) are not worth one copy per chunk: they come back in ONE copy after the
   // last chunk (the download stream is then behind every kernel)
   uint32_t small_outputs = 0;
-  const char *stats_env = getenv("MFA_B200_HOST_BATCH_STATS");  // tuning knob: 0 = one copy per chunk, as for O
-  if (per_chunk < batch && !(stats_env && stats_env[0] == '0'))
+  if (per_chunk < batch)
     for (int op = 0; op < MFA_BUFFER_COUNT; ++op)
       if ((outputs & (1u << op)) && host_buffers[op] && head_bytes[op] * batch <= (size_t(4) << 20)) small_outputs |= 1u << op;
   uint32_t chunk_index = 0;

@@ -24,13 +24,9 @@ struct AttentionParams {
   float scale;       // 1/sqrt(D)          (AttentionKernel+Softmax.swift:17-26)
   float scale_log2;  // log2(e)/sqrt(D)
   // tuning columns of the parameter-table row the kernel was created from (tensor-core family)
-  uint8_t exp2_fma_quarters;  // validated and carried; the sm_90a kernels take every exp2 on the MUFU pipe
-  uint8_t split_min_blocks;   // 0 = never split small grids
+  uint8_t split_min_blocks;  // 0 = never split small grids
   uint8_t split_max;
 };
-
-// compiled exp2-on-the-FMA-pipe variants (quarters of the element pairs): forward 0..2, backward 0..3
-constexpr uint32_t kMaxForwardExp2Quarters = 2, kMaxBackwardExp2Quarters = 3;
 
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
 cudaError_t launch_simt_forward(const AttentionParams &p, cudaStream_t stream);
@@ -40,21 +36,24 @@ void simt_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes
                    uint32_t *head);
 
 // ---- tensor-core family (wgmma_attention.cu; the backend keeps its historical name "tcgen05" in the ABI) --------
-// 16-bit row-major operands with D % 8 == 0 and D <= 256; kernel.cpp stages every other layout into that form.
-cudaError_t launch_tcgen05_forward(const AttentionParams &p, cudaStream_t stream);
-cudaError_t launch_tcgen05_backward_query(const AttentionParams &p, cudaStream_t stream);
-cudaError_t launch_tcgen05_backward_key_value(const AttentionParams &p, cudaStream_t stream);
-uint32_t tcgen05_forward_launch_count(uint32_t R, uint32_t C, uint32_t D, uint32_t batch, uint32_t min_blocks,
-                                      uint32_t max_splits);
-uint32_t tcgen05_backward_launch_count(int type, uint32_t R, uint32_t C, uint32_t D, uint32_t batch, uint32_t min_blocks,
-                                       uint32_t max_splits, bool convert_dO);
-void tcgen05_forward_set_fused(int enabled);  // debug: 1 = split-KV merged inside the attention kernel (one launch)
-void tcgen05_forward_geometry(uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
-                              uint32_t *head);
-void tcgen05_backward_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par,
-                               uint32_t *trav, uint32_t *head);
-bool tcgen05_forward_transposes_ok(uint32_t R, uint32_t C, bool tQ, bool tK, bool tV);
-bool tcgen05_backward_transposes_ok(uint32_t R, uint32_t C, bool tQ, bool tK, bool tV, bool tO);
+// 16-bit row-major operands with D % 8 == 0 and D <= kWgmmaMaxHead; kernel.cpp stages every other layout into that form.
+constexpr uint32_t kWgmmaMaxHead = 256;
+cudaError_t launch_wgmma_forward(const AttentionParams &p, cudaStream_t stream);
+cudaError_t launch_wgmma_backward_query(const AttentionParams &p, cudaStream_t stream);
+cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream_t stream);
+
+// How the launcher of kernel `type` (mfa_kernel_type_t) runs one problem of padded head dimension D; every field is
+// derived from the kernels' compile-time configurations.  R, C and batch do not affect the geometry fields.
+struct WgmmaPlan {
+  uint32_t threads, smem_bytes;        // per CTA
+  uint32_t par, trav, head;            // blockDimensions: rows per CTA, rows per pipeline stage, head block
+  dim3 grid;                           // (tiles, batch, splits)
+  uint32_t blocks_per_split, splits;   // traversal blocks per CTA; ranges of the traversal axis (1 = not split)
+  bool convert_dO_first;               // dK/dV: the BF16 dO is converted to FP16 in a pass of its own
+  uint32_t launches;                   // kernels the launcher issues
+};
+WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t min_blocks,
+                     uint32_t max_splits, bool convert_dO, uint32_t sm_count);
 
 // operand staging for the tensor-core family (pad_head.cu): a [batch][seq][D] (or, transposed, [batch][D][seq]) operand
 // is copied to row-major [batch][seq][Dp] with zero padding columns, and an FP32 output computed in that form is copied

@@ -20,9 +20,12 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "attention_params.h"
 #include "backward_common.cuh"
 #include "device_state.h"
+#include "mfa_b200.h"
 #include "sm90_ptx.cuh"
 #include "tma_host.h"
 #include "wgmma.cuh"
@@ -103,17 +106,19 @@ __device__ __forceinline__ void store_acc(const float (&acc)[NR], float *out, ui
 // ================================================================================================ forward
 // Split-KV (few query tiles for 132 SMs): the key axis of every tile is cut into `splits` equal ranges handled by
 // separate CTAs (blockIdx.z), each leaving a normalised partial O and its log2-sum-exp in the library's workspace,
-// laid out [split][head][row].  The partials are merged either by merge_splits (a second launch) or, in the one-launch
-// form, by the CTA of each tile that arrives last on the tile's counter.
+// laid out [split][head][row].  merge_splits, a second launch, merges the partials.
 struct SplitArgs {
   uint32_t blocks_per_split, splits, batch;
   float *O_part, *L_part;  // [split][head][R][D], [split][head][R]
-  uint32_t *counters;      // one-launch form: arrivals per (head, tile), returned to zero; nullptr: merged by merge_splits
 };
 
-// O[row][4 quad ..] and L[row] from the partials of every split (row = head * R + r)
-__device__ __forceinline__ void merge_quad(const SplitArgs &sp, float *O, void *L, int l_prec, uint64_t rows_total,
-                                           uint64_t row, uint32_t quad, uint32_t D) {
+// O[row][4 quad ..] and L[row] from the partials of every split (row = head * R + r): one thread per (row, 4 columns)
+__global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O, void *L, int l_prec, uint64_t rows_total,
+                                                    uint32_t D) {
+  const uint64_t idx = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const uint64_t row = idx / (D / 4);
+  if (row >= rows_total) return;
+  const uint32_t quad = static_cast<uint32_t>(idx % (D / 4));
   float lmax = -INFINITY;
   for (uint32_t s = 0; s < sp.splits; ++s) lmax = fmaxf(lmax, __ldcg(sp.L_part + s * rows_total + row));
   float denom = 0.f;
@@ -132,28 +137,22 @@ __device__ __forceinline__ void merge_quad(const SplitArgs &sp, float *O, void *
   if (quad == 0) store_stat(L, row, l_prec, lmax + log2f(denom));
 }
 
-// second launch of the two-launch form: one thread per (row, 4 columns)
-__global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O, void *L, int l_prec, uint64_t rows_total,
-                                                    uint32_t D) {
-  const uint64_t idx = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const uint64_t row = idx / (D / 4);
-  if (row < rows_total) merge_quad(sp, O, L, l_prec, rows_total, row, static_cast<uint32_t>(idx % (D / 4)), D);
-}
-
-template <uint32_t DCH, uint32_t BN>
+// kPar / kTrav: rows of the parallelization / traversal axis per CTA / per pipeline stage (every *Cfg has them)
+template <uint32_t DCH>
 struct FwdCfg {
-  static constexpr uint32_t kThreads = 2 * kWG, kTileM = 2 * kRows;
+  static constexpr uint32_t kThreads = 2 * kWG, kTileM = 2 * kRows, BN = DCH == 4 ? 64 : 128;
+  static constexpr uint32_t kPar = kTileM, kTrav = BN;
   static constexpr uint32_t kQBytes = DCH * kTileM * 128, kKVBytes = DCH * BN * 128;
   static constexpr uint32_t kSmemBytes = 1024 + kQBytes + 2 * 2 * kKVBytes + kBarBytes;
 };
 
-template <uint32_t DCH, uint32_t BN, bool kBF16>
+template <uint32_t DCH, bool kBF16>
 __global__ void __launch_bounds__(2 * kWG, 1)
     attention_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                             const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
                             uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp) {
-  using Cfg = FwdCfg<DCH, BN>;
-  constexpr uint32_t NO = DCH * 64;
+  using Cfg = FwdCfg<DCH>;
+  constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *base = align1024(smem_raw);
   uint8_t *kv = base + Cfg::kQBytes;  // stage s: K at kv + 2 s kKVBytes, V right after it
@@ -275,23 +274,6 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     if (r < R) store_stat(Lout, hb + r, prec, m0 + log2f(l0));
     if (r + 8 < R) store_stat(Lout, hb + r + 8, prec, m1 + log2f(l1));
   }
-  if (sp.splits == 1 || sp.counters == nullptr) return;
-
-  // one-launch form: the last CTA of this tile to arrive merges the tile's rows
-  __shared__ uint32_t last;
-  __threadfence();
-  __syncthreads();
-  uint32_t *counter = sp.counters + head * gridDim.x + blockIdx.x;
-  if (tid == 0) last = atomicAdd(counter, 1u) == sp.splits - 1;
-  __syncthreads();
-  if (!last) return;
-  __threadfence();
-  const uint64_t rows_total = static_cast<uint64_t>(sp.batch) * R;
-  for (uint32_t idx = tid; idx < Cfg::kTileM * (D / 4); idx += Cfg::kThreads) {
-    const uint32_t r = row_base + idx / (D / 4);
-    if (r < R) merge_quad(sp, O, L, l_prec, rows_total, static_cast<uint64_t>(head) * R + r, idx % (D / 4), D);
-  }
-  if (tid == 0) *counter = 0;
 }
 
 // ================================================================================================ backward dQ
@@ -299,6 +281,7 @@ template <uint32_t DCH>
 struct QCfg {
   static constexpr uint32_t kWarpgroups = DCH == 4 ? 1 : 2;
   static constexpr uint32_t kThreads = kWarpgroups * kWG, kTileM = kWarpgroups * kRows, BN = 64;
+  static constexpr uint32_t kPar = kTileM, kTrav = BN;
   static constexpr uint32_t kQBytes = DCH * kTileM * 128, kKVBytes = DCH * BN * 128;
   static constexpr uint32_t kSmemBytes = 1024 + 2 * kQBytes + 2 * 2 * kKVBytes + kBarBytes;
 };
@@ -434,6 +417,7 @@ template <uint32_t DCH>
 struct KVCfg {
   static constexpr bool kSplitD = DCH == 4;  // both warpgroups on the same 64 keys, half of the D columns each
   static constexpr uint32_t kThreads = 2 * kWG, kTileN = kSplitD ? kRows : 2 * kRows, BM = 64;
+  static constexpr uint32_t kPar = kTileN, kTrav = BM;
   static constexpr uint32_t kAcc = kSplitD ? 128 : DCH * 64;  // accumulator columns per warpgroup
   static constexpr uint32_t kKBytes = DCH * kTileN * 128, kQBytes = DCH * BM * 128;
   static constexpr uint32_t kSmemBytes = 1024 + 2 * kKBytes + 2 * 2 * kQBytes + kBarBytes;
@@ -598,7 +582,15 @@ static uint32_t choose_blocks_per_split(uint32_t ctas, uint32_t total_blocks, ui
   return per;
 }
 
-static int g_forward_fused = 0;  // split-KV merge: 0 = merge_splits launch, 1 = inside the attention kernel
+// Calls f(std::integral_constant<uint32_t, DCH>()) for the column-chunk count of the kernels that serve head dimension D
+template <class F>
+static auto with_chunks(uint32_t D, F f) {
+  switch (chunks(D)) {
+    case 1: return f(std::integral_constant<uint32_t, 1>());
+    case 2: return f(std::integral_constant<uint32_t, 2>());
+    default: return f(std::integral_constant<uint32_t, 4>());
+  }
+}
 
 // ================================================================================================ launchers
 template <typename Kernel>
@@ -606,33 +598,30 @@ static cudaError_t prepare(Kernel kernel, uint32_t smem) {
   return ensure_max_dynamic_smem(reinterpret_cast<const void *>(kernel), smem, current_device());
 }
 
-template <uint32_t DCH, uint32_t BN, bool kBF16>
-cudaError_t launch_forward(const AttentionParams &p, cudaStream_t stream) {
-  using Cfg = FwdCfg<DCH, BN>;
-  auto kernel = attention_forward_wgmma<DCH, BN, kBF16>;
+template <uint32_t DCH, bool kBF16>
+cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
+  using Cfg = FwdCfg<DCH>;
+  auto kernel = attention_forward_wgmma<DCH, kBF16>;
   cudaError_t e;
   if ((e = prepare(kernel, Cfg::kSmemBytes)) != cudaSuccess) return e;
   CUtensorMap mapQ, mapK, mapV;
   if ((e = make_tensor_map_16bit(&mapQ, p.buf[sQ], p.R, p.D, p.batch, Cfg::kTileM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch, BN)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch, BN)) != cudaSuccess) return e;
-  const int device = current_device();
-  const uint32_t tiles = (p.R + Cfg::kTileM - 1) / Cfg::kTileM, total_blocks = (p.C + BN - 1) / BN;
-  const uint32_t splits = choose_splits(tiles * p.batch, total_blocks, device_sm_count(device), p.split_min_blocks, p.split_max);
-  SplitArgs sp{total_blocks / splits, splits, p.batch, nullptr, nullptr, nullptr};
+  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch, Cfg::BN)) != cudaSuccess) return e;
+  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch, Cfg::BN)) != cudaSuccess) return e;
+  SplitArgs sp{plan.blocks_per_split, plan.splits, p.batch, nullptr, nullptr};
   const uint64_t rows_total = static_cast<uint64_t>(p.batch) * p.R;
-  if (splits > 1) {
+  if (plan.splits > 1) {
     void *ws = nullptr;
-    const size_t o_elems = splits * rows_total * p.D;
-    if ((e = workspace_for(device, stream, (o_elems + splits * rows_total) * sizeof(float), &ws)) != cudaSuccess) return e;
-    sp.O_part = reinterpret_cast<float *>(static_cast<char *>(ws) + kWorkspaceCounterBytes);
+    const size_t o_elems = plan.splits * rows_total * p.D;
+    if ((e = workspace_for(current_device(), stream, (o_elems + plan.splits * rows_total) * sizeof(float), &ws)) !=
+        cudaSuccess)
+      return e;
+    sp.O_part = static_cast<float *>(ws);
     sp.L_part = sp.O_part + o_elems;
-    if (g_forward_fused && tiles * p.batch * sizeof(uint32_t) <= kWorkspaceCounterBytes) sp.counters = static_cast<uint32_t *>(ws);
   }
-  const dim3 grid(tiles, p.batch, splits);
-  kernel<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapK, mapV, static_cast<float *>(p.buf[sO]), p.buf[sL],
-                                                           p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp);
-  if ((e = cudaGetLastError()) != cudaSuccess || splits == 1 || sp.counters) return e;
+  kernel<<<plan.grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapK, mapV, static_cast<float *>(p.buf[sO]),
+                                                                p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp);
+  if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
   const uint64_t threads = rows_total * (p.D / 4);
   merge_splits<<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(sp, static_cast<float *>(p.buf[sO]),
                                                                                  p.buf[sL], p.prec[sL], rows_total, p.D);
@@ -645,7 +634,7 @@ static cudaError_t split_scratch(BwdArgs &a, uint32_t splits, uint32_t tensors, 
   void *ws = nullptr;
   cudaError_t e = workspace_for(current_device(), stream, splits * tensors * tensor_elems * sizeof(float), &ws);
   if (e != cudaSuccess) return e;
-  *scratch = reinterpret_cast<float *>(static_cast<char *>(ws) + kWorkspaceCounterBytes);
+  *scratch = static_cast<float *>(ws);
   a.split_stride = tensors * tensor_elems;
   return cudaSuccess;
 }
@@ -659,7 +648,7 @@ static cudaError_t launch_sum(const float *scratch, float *out0, float *out1, si
   return cudaGetLastError();
 }
 
-static BwdArgs backward_args(const AttentionParams &p) {
+static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
   BwdArgs a;
   a.O = static_cast<const float *>(p.buf[sO]);
   a.dO = p.buf[sdO];
@@ -668,6 +657,7 @@ static BwdArgs backward_args(const AttentionParams &p) {
   a.dQ = static_cast<float *>(p.buf[sdQ]);
   a.dK = static_cast<float *>(p.buf[sdK]);
   a.dV = static_cast<float *>(p.buf[sdV]);
+  a.blocks_per_split = plan.blocks_per_split;
   a.R = p.R;
   a.C = p.C;
   a.D = p.D;
@@ -680,7 +670,7 @@ static BwdArgs backward_args(const AttentionParams &p) {
 }
 
 template <uint32_t DCH, bool kBF16, bool kConvertDO>
-cudaError_t launch_query(const AttentionParams &p, cudaStream_t stream) {
+cudaError_t launch_query(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
   using Cfg = QCfg<DCH>;
   auto kernel = attention_backward_query_wgmma<DCH, kBF16, kConvertDO>;
   cudaError_t e;
@@ -690,24 +680,21 @@ cudaError_t launch_query(const AttentionParams &p, cudaStream_t stream) {
   if ((e = make_tensor_map_16bit(&mapdO, p.buf[sdO], p.R, p.D, p.batch, Cfg::kTileM)) != cudaSuccess) return e;
   if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch, Cfg::BN)) != cudaSuccess) return e;
   if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch, Cfg::BN)) != cudaSuccess) return e;
-  BwdArgs a = backward_args(p);
-  const uint32_t tiles = (p.R + Cfg::kTileM - 1) / Cfg::kTileM, total_blocks = (p.C + Cfg::BN - 1) / Cfg::BN;
-  a.blocks_per_split = choose_blocks_per_split(tiles * p.batch, total_blocks, device_sm_count(current_device()),
-                                               p.split_min_blocks, p.split_max);
-  const uint32_t splits = (total_blocks + a.blocks_per_split - 1) / a.blocks_per_split;
+  BwdArgs a = backward_args(p, plan);
   const size_t tensor_elems = static_cast<size_t>(p.batch) * p.R * p.D;
   float *scratch = nullptr;
-  if (splits > 1) {
-    if ((e = split_scratch(a, splits, 1, tensor_elems, stream, &scratch)) != cudaSuccess) return e;
+  if (plan.splits > 1) {
+    if ((e = split_scratch(a, plan.splits, 1, tensor_elems, stream, &scratch)) != cudaSuccess) return e;
     a.dQ = scratch;
   }
-  kernel<<<dim3(tiles, p.batch, splits), Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapdO, mapK, mapV, a);
-  if ((e = cudaGetLastError()) != cudaSuccess || splits == 1) return e;
-  return launch_sum(scratch, static_cast<float *>(p.buf[sdQ]), nullptr, tensor_elems, 1, a.split_stride, splits, stream);
+  kernel<<<plan.grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapdO, mapK, mapV, a);
+  if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
+  return launch_sum(scratch, static_cast<float *>(p.buf[sdQ]), nullptr, tensor_elems, 1, a.split_stride, plan.splits,
+                    stream);
 }
 
 template <uint32_t DCH, bool kBF16, bool kConvertDO>
-cudaError_t launch_key_value(const AttentionParams &p, cudaStream_t stream) {
+cudaError_t launch_key_value(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
   using Cfg = KVCfg<DCH>;
   auto kernel = attention_backward_key_value_wgmma<DCH, kBF16, kConvertDO>;
   cudaError_t e;
@@ -717,64 +704,93 @@ cudaError_t launch_key_value(const AttentionParams &p, cudaStream_t stream) {
   if ((e = make_tensor_map_16bit(&mapdO, p.buf[sdO], p.R, p.D, p.batch, Cfg::BM)) != cudaSuccess) return e;
   if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch, Cfg::kTileN)) != cudaSuccess) return e;
   if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch, Cfg::kTileN)) != cudaSuccess) return e;
-  BwdArgs a = backward_args(p);
-  const uint32_t tiles = (p.C + Cfg::kTileN - 1) / Cfg::kTileN, total_blocks = (p.R + Cfg::BM - 1) / Cfg::BM;
-  a.blocks_per_split = choose_blocks_per_split(tiles * p.batch, total_blocks, device_sm_count(current_device()),
-                                               p.split_min_blocks, p.split_max);
-  const uint32_t splits = (total_blocks + a.blocks_per_split - 1) / a.blocks_per_split;
+  BwdArgs a = backward_args(p, plan);
   const size_t tensor_elems = static_cast<size_t>(p.batch) * p.C * p.D;
   float *scratch = nullptr;
-  if (splits > 1) {
-    if ((e = split_scratch(a, splits, 2, tensor_elems, stream, &scratch)) != cudaSuccess) return e;
+  if (plan.splits > 1) {
+    if ((e = split_scratch(a, plan.splits, 2, tensor_elems, stream, &scratch)) != cudaSuccess) return e;
     a.dV = scratch;
     a.dK = scratch + tensor_elems;
   }
-  kernel<<<dim3(tiles, p.batch, splits), Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapdO, mapK, mapV, a);
-  if ((e = cudaGetLastError()) != cudaSuccess || splits == 1) return e;
+  kernel<<<plan.grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapdO, mapK, mapV, a);
+  if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
   return launch_sum(scratch, static_cast<float *>(p.buf[sdV]), static_cast<float *>(p.buf[sdK]), tensor_elems, 2,
-                    a.split_stride, splits, stream);
+                    a.split_stride, plan.splits, stream);
 }
 
-// dK/dV with BF16 dO beside FP16 Q/K/V: a grid of more than one wave converts dO once, in a pass of its own
-static bool key_value_converts_dO_first(uint32_t C, uint32_t D, uint32_t batch) {
-  const uint32_t tile = chunks(D) == 4 ? KVCfg<4>::kTileN : KVCfg<1>::kTileN;
-  return static_cast<uint64_t>((C + tile - 1) / tile) * batch > device_sm_count(current_device());
+// Calls f(DCH, kBF16, kConvertDO), each as a std::integral_constant, for the kernel instantiation that serves p
+template <class F>
+static cudaError_t dispatch(const AttentionParams &p, bool convert_dO, F f) {
+  return with_chunks(p.D, [&](auto dch) {
+    if (convert_dO) return f(dch, std::false_type(), std::true_type());
+    if (p.prec[sQ] == BF16) return f(dch, std::true_type(), std::false_type());
+    return f(dch, std::false_type(), std::false_type());
+  });
 }
 
 }  // namespace hop
 
-void tcgen05_forward_set_fused(int enabled) { hop::g_forward_fused = enabled; }
+WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t min_blocks,
+                     uint32_t max_splits, bool convert_dO, uint32_t sm_count) {
+  WgmmaPlan p{};
+  auto geometry = [&](auto cfg) {
+    using Cfg = decltype(cfg);
+    p.threads = Cfg::kThreads;
+    p.smem_bytes = Cfg::kSmemBytes;
+    p.par = Cfg::kPar;
+    p.trav = Cfg::kTrav;
+  };
+  hop::with_chunks(D, [&](auto dch) {
+    constexpr uint32_t DCH = decltype(dch)::value;
+    if (type == MFA_FORWARD)
+      geometry(hop::FwdCfg<DCH>());
+    else if (type == MFA_BACKWARD_QUERY)
+      geometry(hop::QCfg<DCH>());
+    else
+      geometry(hop::KVCfg<DCH>());
+  });
+  const uint32_t padded = (D + 7) / 8 * 8, columns = hop::chunks(D) * 64;
+  p.head = columns < padded ? columns : padded;
 
-uint32_t tcgen05_forward_max_head() { return 256; }
-uint32_t tcgen05_backward_max_head() { return 256; }
-
-// Transposed operands are staged row-major by kernel.cpp; the descriptor heuristic keeps the shapes whose transposed
-// view has a 16-byte row pitch (sequence length % 8 == 0) on the tensor cores, as it always has.
-bool tcgen05_forward_transposes_ok(uint32_t R, uint32_t C, bool tQ, bool tK, bool tV) {
-  return (!tQ || R % 8 == 0) && (!tK || C % 8 == 0) && (!tV || C % 8 == 0);
-}
-bool tcgen05_backward_transposes_ok(uint32_t R, uint32_t C, bool tQ, bool tK, bool tV, bool tO) {
-  return (!tQ || R % 8 == 0) && (!tK || C % 8 == 0) && (!tV || C % 8 == 0) && (!tO || R % 8 == 0);
+  const bool key_value = type == MFA_BACKWARD_KEY_VALUE;
+  const uint32_t tiles = ((key_value ? C : R) + p.par - 1) / p.par, total = ((key_value ? R : C) + p.trav - 1) / p.trav;
+  if (type == MFA_FORWARD) {
+    p.splits = hop::choose_splits(tiles * batch, total, sm_count, min_blocks, max_splits);
+    p.blocks_per_split = total / p.splits;
+  } else {
+    p.blocks_per_split = hop::choose_blocks_per_split(tiles * batch, total, sm_count, min_blocks, max_splits);
+    p.splits = (total + p.blocks_per_split - 1) / p.blocks_per_split;
+  }
+  p.grid = dim3(tiles, batch, p.splits);
+  // dK/dV with BF16 dO beside FP16 Q/K/V: a grid of more than one wave converts dO once, in a pass of its own (a
+  // smaller one converts each streamed dO tile in shared memory)
+  p.convert_dO_first = key_value && convert_dO && static_cast<uint64_t>(tiles) * batch > sm_count;
+  // the kernel, + merge_splits / sum_splits when split, + the dO conversion pass
+  p.launches = 1 + (p.splits > 1 ? 1 : 0) + (p.convert_dO_first ? 1 : 0);
+  return p;
 }
 
 static bool row_major_16bit(const AttentionParams &p) {
   for (int s = 0; s < kSlots; ++s)
     if (p.transposed[s]) return false;
   return (p.prec[sQ] == FP16 || p.prec[sQ] == BF16) && p.prec[sK] == p.prec[sQ] && p.prec[sV] == p.prec[sQ] &&
-         p.D % 8 == 0 && p.D <= 256;
+         p.D % 8 == 0 && p.D <= kWgmmaMaxHead;
 }
 
-cudaError_t launch_tcgen05_forward(const AttentionParams &p, cudaStream_t stream) {
+static WgmmaPlan plan_for(int type, const AttentionParams &p, bool convert_dO) {
+  return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.split_min_blocks, p.split_max, convert_dO,
+                    device_sm_count(current_device()));
+}
+
+cudaError_t launch_wgmma_forward(const AttentionParams &p, cudaStream_t stream) {
   if (!row_major_16bit(p) || p.prec[sO] != FP32) {
     set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
     return cudaErrorInvalidValue;
   }
-  const bool bf16 = p.prec[sQ] == BF16;
-  switch (hop::chunks(p.D)) {
-    case 1: return bf16 ? hop::launch_forward<1, 128, true>(p, stream) : hop::launch_forward<1, 128, false>(p, stream);
-    case 2: return bf16 ? hop::launch_forward<2, 128, true>(p, stream) : hop::launch_forward<2, 128, false>(p, stream);
-    default: return bf16 ? hop::launch_forward<4, 64, true>(p, stream) : hop::launch_forward<4, 64, false>(p, stream);
-  }
+  const WgmmaPlan plan = plan_for(MFA_FORWARD, p, false);
+  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto) {
+    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value>(p, plan, stream);
+  });
 }
 
 static bool backward_ok(const AttentionParams &p) {
@@ -783,101 +799,38 @@ static bool backward_ok(const AttentionParams &p) {
          p.prec[sdV] == FP32;
 }
 
-cudaError_t launch_tcgen05_backward_query(const AttentionParams &p, cudaStream_t stream) {
-  if (!backward_ok(p)) {
-    set_launch_detail("descriptor is outside the wgmma backward kernels' domain");
-    return cudaErrorInvalidValue;
-  }
-  const bool bf16 = p.prec[sQ] == BF16, convert = p.prec[sdO] != p.prec[sQ];
-#define MFA_Q_DISPATCH(DCH_)                                                     \
-  if (convert) return hop::launch_query<DCH_, false, true>(p, stream);          \
-  return bf16 ? hop::launch_query<DCH_, true, false>(p, stream) : hop::launch_query<DCH_, false, false>(p, stream);
-  switch (hop::chunks(p.D)) {
-    case 1: { MFA_Q_DISPATCH(1) }
-    case 2: { MFA_Q_DISPATCH(2) }
-    default: { MFA_Q_DISPATCH(4) }
-  }
-#undef MFA_Q_DISPATCH
-}
-
-cudaError_t launch_tcgen05_backward_key_value(const AttentionParams &p, cudaStream_t stream) {
+cudaError_t launch_wgmma_backward_query(const AttentionParams &p, cudaStream_t stream) {
   if (!backward_ok(p)) {
     set_launch_detail("descriptor is outside the wgmma backward kernels' domain");
     return cudaErrorInvalidValue;
   }
   const bool convert = p.prec[sdO] != p.prec[sQ];
-  if (convert && hop::key_value_converts_dO_first(p.C, p.D, p.batch)) {
-    AttentionParams q = p;
+  const WgmmaPlan plan = plan_for(MFA_BACKWARD_QUERY, p, convert);
+  return hop::dispatch(p, convert, [&](auto dch, auto bf16, auto cvt) {
+    return hop::launch_query<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value>(p, plan, stream);
+  });
+}
+
+cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream_t stream) {
+  if (!backward_ok(p)) {
+    set_launch_detail("descriptor is outside the wgmma backward kernels' domain");
+    return cudaErrorInvalidValue;
+  }
+  const bool convert = p.prec[sdO] != p.prec[sQ];
+  const WgmmaPlan plan = plan_for(MFA_BACKWARD_KEY_VALUE, p, convert);
+  AttentionParams q = p;
+  if (plan.convert_dO_first) {
     const uint64_t elements = static_cast<uint64_t>(p.batch) * p.R * p.D;
-    void *ws = nullptr;
-    cudaError_t e = workspace_for(current_device(), stream, elements * 2, &ws, /*slot=*/2);
+    void *converted = nullptr;
+    cudaError_t e = workspace_for(current_device(), stream, elements * 2, &converted, /*slot=*/2);
     if (e != cudaSuccess) return e;
-    void *converted = static_cast<char *>(ws) + kWorkspaceCounterBytes;
     if ((e = launch_bf16_to_f16(p.buf[sdO], converted, elements, stream)) != cudaSuccess) return e;
     q.buf[sdO] = converted;
     q.prec[sdO] = q.prec[sQ];
-    return launch_tcgen05_backward_key_value(q, stream);
   }
-  const bool bf16 = p.prec[sQ] == BF16;
-#define MFA_KV_DISPATCH(DCH_)                                                    \
-  if (convert) return hop::launch_key_value<DCH_, false, true>(p, stream);      \
-  return bf16 ? hop::launch_key_value<DCH_, true, false>(p, stream) : hop::launch_key_value<DCH_, false, false>(p, stream);
-  switch (hop::chunks(p.D)) {
-    case 1: { MFA_KV_DISPATCH(1) }
-    case 2: { MFA_KV_DISPATCH(2) }
-    default: { MFA_KV_DISPATCH(4) }
-  }
-#undef MFA_KV_DISPATCH
-}
-
-// 1 launch, or 2 (attention + merge_splits) when split-KV engages with the two-launch merge
-uint32_t tcgen05_forward_launch_count(uint32_t R, uint32_t C, uint32_t D, uint32_t batch, uint32_t min_blocks,
-                                      uint32_t max_splits) {
-  const uint32_t bn = hop::chunks(D) == 4 ? 64 : 128, tiles = (R + 127) / 128;
-  const uint32_t splits =
-      hop::choose_splits(tiles * batch, (C + bn - 1) / bn, device_sm_count(current_device()), min_blocks, max_splits);
-  return splits > 1 && !(hop::g_forward_fused && tiles * batch * sizeof(uint32_t) <= kWorkspaceCounterBytes) ? 2 : 1;
-}
-
-// kernel (+ sum_splits when the traversal split engages) (+ the dO conversion pass of dK/dV on large grids)
-uint32_t tcgen05_backward_launch_count(int type, uint32_t R, uint32_t C, uint32_t D, uint32_t batch, uint32_t min_blocks,
-                                       uint32_t max_splits, bool convert_dO) {
-  const bool key_value = type == 2;  // MFA_BACKWARD_KEY_VALUE
-  uint32_t threads, smem, par, trav, head;
-  tcgen05_backward_geometry(type, D, &threads, &smem, &par, &trav, &head);
-  const uint32_t tiles = ((key_value ? C : R) + par - 1) / par, total = ((key_value ? R : C) + trav - 1) / trav;
-  const uint32_t per = hop::choose_blocks_per_split(tiles * batch, total, device_sm_count(current_device()), min_blocks, max_splits);
-  return (per < total ? 2 : 1) + (key_value && convert_dO && hop::key_value_converts_dO_first(C, D, batch) ? 1 : 0);
-}
-
-void tcgen05_forward_geometry(uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
-                              uint32_t *head) {
-  const uint32_t c = hop::chunks(D);
-  *threads = hop::FwdCfg<1, 128>::kThreads;
-  *smem_bytes = c == 1 ? hop::FwdCfg<1, 128>::kSmemBytes
-                       : (c == 2 ? hop::FwdCfg<2, 128>::kSmemBytes : hop::FwdCfg<4, 64>::kSmemBytes);
-  *par = hop::FwdCfg<1, 128>::kTileM;
-  *trav = c == 4 ? 64 : 128;
-  const uint32_t padded = (D + 7) / 8 * 8;
-  *head = c * 64 < padded ? c * 64 : padded;
-}
-
-void tcgen05_backward_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par,
-                               uint32_t *trav, uint32_t *head) {
-  const uint32_t c = hop::chunks(D);
-  if (type == 1) {  // MFA_BACKWARD_QUERY
-    *threads = c == 4 ? hop::QCfg<4>::kThreads : hop::QCfg<1>::kThreads;
-    *smem_bytes = c == 1 ? hop::QCfg<1>::kSmemBytes : (c == 2 ? hop::QCfg<2>::kSmemBytes : hop::QCfg<4>::kSmemBytes);
-    *par = c == 4 ? hop::QCfg<4>::kTileM : hop::QCfg<1>::kTileM;
-    *trav = hop::QCfg<1>::BN;
-  } else {
-    *threads = hop::KVCfg<1>::kThreads;
-    *smem_bytes = c == 1 ? hop::KVCfg<1>::kSmemBytes : (c == 2 ? hop::KVCfg<2>::kSmemBytes : hop::KVCfg<4>::kSmemBytes);
-    *par = c == 4 ? hop::KVCfg<4>::kTileN : hop::KVCfg<1>::kTileN;
-    *trav = hop::KVCfg<1>::BM;
-  }
-  const uint32_t padded = (D + 7) / 8 * 8;
-  *head = c * 64 < padded ? c * 64 : padded;
+  return hop::dispatch(q, convert && !plan.convert_dO_first, [&](auto dch, auto bf16, auto cvt) {
+    return hop::launch_key_value<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value>(q, plan, stream);
+  });
 }
 
 }  // namespace mfa

@@ -41,7 +41,6 @@ struct AttentionKernelDescriptor {  // AttentionKernelDescriptor.swift:7-48
     return c.has_head_dimension ? std::optional<uint16_t>(c.head_dimension) : std::nullopt;
   }
   // library extension: the tuning columns of the parameter-table row (editable like every other field)
-  uint8_t &exp2FmaQuarters() { return c.exp2_fma_quarters; }
   uint8_t &splitMinBlocks() { return c.split_min_blocks; }
   uint8_t &splitMax() { return c.split_max; }
   bool tensorCoreFamily() const { return c.backend == MFA_BACKEND_TCGEN05; }

@@ -282,13 +282,8 @@ public struct AttentionKernelDescriptor {
     get { AttentionBackend(rawValue: c.backend) ?? .simtFP32 }
     set { c.backend = newValue.rawValue }
   }
-  /// library extension: tuning columns of the parameter-table row.  Of every 4 element pairs of P, how many take exp2 on
-  /// the FMA pipe (selects the kernel instantiation); small-grid split policy (minimum blocks per range, 0 = never;
-  /// maximum ranges).
-  public var exp2FmaQuarters: UInt8 {
-    get { c.exp2_fma_quarters }
-    set { c.exp2_fma_quarters = newValue }
-  }
+  /// library extension: tuning columns of the parameter-table row, the small-grid split policy (minimum blocks per
+  /// range, 0 = never; maximum ranges).
   public var splitPolicy: (minimumBlocks: UInt8, maximumSplits: UInt8) {
     get { (c.split_min_blocks, c.split_max) }
     set { c.split_min_blocks = newValue.minimumBlocks; c.split_max = newValue.maximumSplits }

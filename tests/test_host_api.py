@@ -1,6 +1,6 @@
 """Host-side logic of the C ABI (no GPU): descriptor -> kernel-descriptor heuristic, precision policy,
-parameter tables, validation / error behaviour, and that libmfa_b200.so exports every symbol the header
-declares.  Mirrors what the reference's Swift types do on the CPU
+parameter tables, validation / error behaviour, launch counts, and that libmfa_b200.so exports every symbol the header
+declares (plus one GPU test: the launch count is what encode() really launches).  Mirrors what the reference's Swift types do on the CPU
 (Sources/FlashAttention/Attention/AttentionDescriptor/*.swift, AttentionKernel.swift)."""
 import ctypes
 import os
@@ -171,8 +171,8 @@ def test_heuristic_selects_tensor_core_family_only_where_it_applies():
 def test_parameter_file_has_reference_format():
     text = make(4096, 4096, 128, lowIn=True, bf16=True).parameterFile(KT.forward)
     rows = [line for line in text.split("\n") if line.strip()]
-    # the reference's five segments (AttentionParameterRow.swift:46-49) + three tuning columns on the tensor-core family
-    assert rows and all(len([c for c in row.split("|") if c != ""]) == 8 for row in rows)
+    # the reference's five segments (AttentionParameterRow.swift:46-49) + two tuning columns on the tensor-core family
+    assert rows and all(len([c for c in row.split("|") if c != ""]) == 7 for row in rows)
     simt = make(64, 64, 35).parameterFile(KT.forward)
     assert all(len([c for c in row.split("|") if c != ""]) == 5 for row in simt.split("\n") if row.strip())
     maxima = [int(row.split("|")[1]) for row in rows]
@@ -192,6 +192,68 @@ def test_kernel_object_reports_launch_geometry():
     assert "tcgen05" in k.sourceName() and k.launchCount(c) >= 1
     k2 = mfa.AttentionKernel(make(10, 10, 3).kernelDescriptor(KT.backwardKeyValue))
     assert "simt" in k2.sourceName()
+
+
+def _launch_count(d, t):
+    c = mfa.FunctionConstantValues()
+    d.setFunctionConstants(c)
+    return mfa.AttentionKernel(d.kernelDescriptor(t)).launchCount(c)
+
+
+def test_launch_count_covers_every_batch_slice():
+    """encode() launches batches beyond 16384 problems in slices, each with its own kernels and staging copies: the
+    launch count sums them.  One 128 x 128 tile per problem: the first slice fills the GPU, the second (one problem)
+    has a single key block and is not split either."""
+    d = make(128, 128, 64, lowIn=True, bf16=True)
+    d.batchCount = 16385
+    assert _launch_count(d, KT.forward) == 2                     # two slices x the kernel
+    d = make(128, 128, 77, lowIn=True, bf16=True)
+    d.batchCount = 16385
+    assert _launch_count(d, KT.forward) == 10                    # two slices x (3 staged inputs + kernel + O copied back)
+    d.batchCount = 16384
+    assert _launch_count(d, KT.forward) == 5
+    d = make(128, 128, 32)                                       # FP32 family: one kernel per slice
+    d.batchCount = 40000
+    assert _launch_count(d, KT.backwardKeyValue) == 3
+
+
+LAUNCH_COUNT_CASES = [  # (R, C, D, batch, transposes, bf16, kernel type)
+    (4096, 4096, 128, 1, (False,) * 4, True, KT.forward),              # split-KV: attention + merge
+    (512, 512, 64, 1, (True,) * 4, True, KT.backwardQuery),            # staged transposed operands + split dQ
+    (512, 512, 64, 1, (True,) * 4, True, KT.backwardKeyValue),
+    (2048, 2048, 64, 16, (False,) * 4, False, KT.backwardKeyValue),    # FP16 Q/K/V + BF16 dO, large grid: dO pass
+    (128, 128, 64, 16385, (False,) * 4, True, KT.forward),             # two batch slices
+]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("R,C,D,batch,transposes,bf16,t", LAUNCH_COUNT_CASES)
+def test_launch_count_is_what_encode_launches(R, C, D, batch, transposes, bf16, t):
+    """launchCount against the CUDA kernels a torch.profiler trace of one encode() records."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    d = make(R, C, D, lowIn=True, transposes=transposes, bf16=bf16)
+    d.batchCount = batch
+    c = mfa.FunctionConstantValues()
+    d.setFunctionConstants(c)
+    kernel = mfa.AttentionKernel(d.kernelDescriptor(t))
+    assert kernel.sourceName().startswith("attention_") and "tcgen05" in kernel.sourceName()
+    bufs = {}
+    for op in (Op.Q, Op.K, Op.V, Op.O, Op.L, Op.D, Op.dO, Op.dV, Op.dK, Op.dQ):
+        n = d.operandElements(op)
+        bufs[op] = (torch.randn(n, device="cuda") if d.memoryPrecisions[op] == P.FP32 else
+                    torch.randn(n, device="cuda").to(torch.bfloat16 if d.memoryPrecisions[op] == P.BF16 else torch.float16))
+    bufs[Op.L].zero_()                     # finite statistics, as a forward pass would leave them
+    bufs[Op.D].zero_()
+    ptrs = {op: b.data_ptr() for op, b in bufs.items()}
+    kernel.encode(c, ptrs)                 # first encode: workspaces and shared-memory opt-ins
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        kernel.encode(c, ptrs)
+        torch.cuda.synchronize()
+    launched = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+                and not e.name.startswith(("Memcpy", "Memset"))]
+    assert len(launched) == kernel.launchCount(c), launched
 
 
 def test_invalid_precision_pairs_are_rejected():
@@ -311,76 +373,70 @@ int main() {
     assert out[0] == "128 128 128 256 256" and out[1] == "Descriptor was incomplete."
 
 
-FORWARD_TABLE = ("| 64  | 128 | 128 | 64  | Q, O | 2 | 8 | 4 |\n"
-                 "| 128 | 128 | 128 | 128 | Q, O | 1 | 2 | 16 |\n"
-                 "| 256 | 128 | 64  | 256 | Q, O | 0 | 0 | 1 |\n")
+FORWARD_TABLE = ("| 64  | 128 | 128 | 64  | Q, O | 8 | 4 |\n"
+                 "| 128 | 128 | 128 | 128 | Q, O | 2 | 16 |\n"
+                 "| 256 | 128 | 64  | 256 | Q, O | 0 | 1 |\n")
 
 
 def test_parameter_table_is_live_data():
     """The H100 parameter table drives the kernel (AttentionDescriptor+Parameters.swift:106-285 analogue): editing a row
-    changes the kernel descriptor, the cached kernel object and the small-grid split policy; every compiled variant is
-    accepted, anything else is rejected and leaves the current table in place."""
+    changes the kernel descriptor, the cached kernel object and the small-grid split policy; a malformed table is
+    rejected and leaves the current table in place."""
     d = make(4096, 4096, 128, lowIn=True, bf16=True)
     c = mfa.FunctionConstantValues()
     d.setFunctionConstants(c)
     try:
         kd = d.kernelDescriptor(KT.forward)
-        assert kd.exp2FmaQuarters == 0 and kd.splitPolicy == (4, 8)
+        assert kd.splitPolicy == (4, 8)
         k = mfa.AttentionKernel(kd)
-        assert "exp2" not in k.sourceName() and k.launchCount(c) == 2        # 32 blocks / 4 ranges of >= 4
+        assert k.launchCount(c) == 2                                          # 32 blocks / 4 ranges of >= 4
         cached_before = mfa.AttentionKernel.cached(d, KT.forward)._handle.value
 
         mfa.setParameterTable(KT.forward, FORWARD_TABLE)
         assert d.parameterFile(KT.forward) == FORWARD_TABLE
         kd = d.kernelDescriptor(KT.forward)
-        assert kd.exp2FmaQuarters == 1 and kd.splitPolicy == (2, 16)
+        assert kd.splitPolicy == (2, 16)
         mfa.AttentionKernel(kd)
         assert mfa.AttentionKernel.cached(d, KT.forward)._handle.value != cached_before   # the cache follows the table
         kd64 = make(2048, 2048, 64, lowIn=True).kernelDescriptor(KT.forward)
-        assert kd64.exp2FmaQuarters == 2 and kd64.splitPolicy == (8, 4)
+        assert kd64.splitPolicy == (8, 4)
 
         # a table may turn splitting off; the descriptor is plain data and may be edited field by field as well
         kd.splitPolicy = (0, 1)
         assert mfa.AttentionKernel(kd).launchCount(c) == 1
-        for q in range(mfa.maxExp2FmaQuarters(KT.forward) + 1):
-            kd.exp2FmaQuarters = q
-            mfa.AttentionKernel(kd)
-        kd.exp2FmaQuarters = mfa.maxExp2FmaQuarters(KT.forward) + 1
-        with pytest.raises(mfa.MFAError, match="no compiled sm_90a kernel"):
-            mfa.AttentionKernel(kd)
 
-        # rejected tables leave the installed one untouched
-        for bad, message in ((FORWARD_TABLE.replace("| 2 | 8 | 4 |", "| 3 | 8 | 4 |"), "no compiled kernel"),
+        # rejected tables leave the installed one untouched; a row with eight columns is malformed
+        for bad, message in ((FORWARD_TABLE.replace("| 8 | 4 |", "| 0 | 8 | 4 |"), "Number of segments was invalid: 8"),
                              (FORWARD_TABLE.replace("Q, O", "Q, dQ", 1), "Unexpected operand: dQ"),
                              ("| 64 | 256 | 128 |\n", "Number of segments was invalid"),
                              ("| 64 | 256 | 128 | 64 | Q, O |\n", "tuning columns")):
             with pytest.raises(mfa.MFAError, match=message):
                 mfa.setParameterTable(KT.forward, bad)
             assert d.parameterFile(KT.forward) == FORWARD_TABLE
-        # the backward kernels have their own tables and a wider compiled range
-        mfa.setParameterTable(KT.backwardQuery, "| 128 | 128 | 64 | 128 | Q, dO, dQ | 3 | 2 | 8 |\n")
+        # the backward kernels have their own tables
+        mfa.setParameterTable(KT.backwardQuery, "| 128 | 128 | 64 | 128 | Q, dO, dQ | 3 | 5 |\n")
         kdq = d.kernelDescriptor(KT.backwardQuery)
-        assert kdq.exp2FmaQuarters == 3 and kdq.splitPolicy == (2, 8)
+        assert kdq.splitPolicy == (3, 5)
         mfa.AttentionKernel(kdq)
     finally:
         for t in KT:
             mfa.setParameterTable(t, None)
-    assert d.kernelDescriptor(KT.forward).exp2FmaQuarters == 0
+    assert d.kernelDescriptor(KT.forward).splitPolicy == (4, 8)
 
 
 def test_parameter_file_from_the_environment(tmp_path):
     """MFA_B200_PARAMETER_FILE: tables in that file are picked up when the library is loaded."""
     path = tmp_path / "tables.txt"
     path.write_text("# comment\n[forward]\n" + FORWARD_TABLE + "[backwardKeyValue]\n"
-                    "| 64  | 128 | 64  | 64  | K, V, dV, dK | 1 | 2 | 4 |\n| 128 | 128 | 64  | 128 | K, V, dV, dK | 2 | 2 | 8 |\n")
+                    "| 64  | 128 | 64  | 64  | K, V, dV, dK | 2 | 4 |\n| 128 | 128 | 64  | 128 | K, V, dV, dK | 2 | 8 |\n")
     code = ("import mfa_b200 as mfa\n"
             "d = mfa.AttentionDescriptor(); d.lowPrecisionInputs = True\n"
             "d.matrixDimensions = (512, 512, 64); d.transposeState = (False,) * 4\n"
             "KT = mfa.AttentionKernelType\n"
-            "print([(d.kernelDescriptor(t).exp2FmaQuarters,) + d.kernelDescriptor(t).splitPolicy for t in KT])\n")
+            "print([d.kernelDescriptor(t).splitPolicy for t in KT])\n")
     out = subprocess.check_output([sys.executable, "-c", code], cwd=ROOT, text=True,
                                   env=dict(os.environ, MFA_B200_PARAMETER_FILE=str(path)))
-    assert out.strip() == "[(2, 8, 4), (0, 2, 8), (1, 2, 4)]"   # forward and dK-dV from the file, dQ built in
+    assert out.strip() == "[(8, 4), (2, 8), (2, 4)]"   # forward and dK-dV from the file, dQ built in
 
 
 def test_transposed_tables_are_separate_and_live(tmp_path):
@@ -391,16 +447,16 @@ def test_transposed_tables_are_separate_and_live(tmp_path):
     assert trans.kernelDescriptor(KT.backwardKeyValue).blockDimensions == (128, 64, 64)
     assert plain.kernelDescriptor(KT.backwardKeyValue).blockDimensions == (128, 64, 64)
     try:
-        mfa.setParameterTable(KT.backwardKeyValue, "| 256 | 128 | 64 | 256 | K, V, dV, dK | 0 | 4 | 2 |\n", transposed=True)
+        mfa.setParameterTable(KT.backwardKeyValue, "| 256 | 128 | 64 | 256 | K, V, dV, dK | 4 | 2 |\n", transposed=True)
         assert trans.kernelDescriptor(KT.backwardKeyValue).splitPolicy == (4, 2)
         assert plain.kernelDescriptor(KT.backwardKeyValue).splitPolicy == (2, 8)          # the row-major table is untouched
         with pytest.raises(mfa.MFAError, match="Unexpected operand"):
-            mfa.setParameterTable(KT.backwardQuery, "| 256 | 128 | 64 | 256 | K, V | 0 | 2 | 8 |\n", transposed=True)
+            mfa.setParameterTable(KT.backwardQuery, "| 256 | 128 | 64 | 256 | K, V | 2 | 8 |\n", transposed=True)
     finally:
         mfa.setParameterTable(KT.backwardKeyValue, None, transposed=True)
     assert trans.kernelDescriptor(KT.backwardKeyValue).splitPolicy == (2, 8)
     path = tmp_path / "tables.txt"
-    path.write_text("[backwardQuery.transposed]\n| 256 | 128 | 64 | 256 | Q, dO, dQ | 0 | 3 | 5 |\n")
+    path.write_text("[backwardQuery.transposed]\n| 256 | 128 | 64 | 256 | Q, dO, dQ | 3 | 5 |\n")
     code = ("import mfa_b200 as mfa\n"
             "KT = mfa.AttentionKernelType\n"
             "for t in ((False,) * 4, (True, False, False, False)):\n"
@@ -425,7 +481,7 @@ def test_committed_parameter_file_matches_the_builtin_tables():
             "    d.matrixDimensions = (512, 512, D); d.transposeState = (False,) * 4\n"
             "    for t in KT:\n"
             "        kd = d.kernelDescriptor(t)\n"
-            "        print(D, int(t), kd.backend.name, kd.blockDimensions, kd.exp2FmaQuarters, kd.splitPolicy)\n")
+            "        print(D, int(t), kd.backend.name, kd.blockDimensions, kd.splitPolicy)\n")
     plain = subprocess.check_output([sys.executable, "-c", code], cwd=ROOT, text=True,
                                     env={k: v for k, v in os.environ.items() if k != "MFA_B200_PARAMETER_FILE"})
     loaded = subprocess.check_output([sys.executable, "-c", code], cwd=ROOT, text=True,

@@ -71,47 +71,42 @@ SPLIT_KV_CASES = [(4096, 4096, 128, True),   # 16 items x 8 splits: the headline
                   (300, 2000, 128, True),    # ragged rows and a ragged last key block
                   (512, 1536, 96, True),     # 12 key blocks -> 3 splits
                   (1, 4096, 128, False),     # a single query row
-                  (2048, 2048, 64, True)]    # BASELINE configs[2] shape
+                  (2048, 2048, 64, True),    # BASELINE configs[2] shape
+                  (129, 1024, 64, False),    # two query tiles, the second holding one row -> 4 splits
+                  (64, 3000, 128, False),    # a ragged last key block of 56 keys -> 6 splits of 4 blocks
+                  (256, 4096, 8, True),      # the narrowest head: 8 real of 64 columns (TMA zero fill)
+                  (100, 2560, 120, True),    # 20 key blocks -> 5 splits, head dimension short of the 128 columns
+                  (384, 1024, 32, False),    # 3 query tiles x 4 splits
+                  (640, 2048, 64, True)]     # 5 query tiles x 8 splits of the minimum 2 blocks
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("fused", [True, False], ids=["fused-one-launch", "scratch-combine"])
 @pytest.mark.parametrize("R,C,D,bf16", SPLIT_KV_CASES)
-def test_split_kv_small_grids(R, C, D, bf16, fused):
-    """Few (head, query tile) items: the key axis is split across SMs.  Default form: normalised partials in the library's
-    workspace + the merge kernel (2 launches); one-launch form: the split CTA of a tile that arrives last on the tile's
-    counter merges the tile's rows inside the attention kernel.  Both must match the oracle, also when run back to back
-    (the one-launch form must leave its counters at zero)."""
+def test_split_kv_small_grids(R, C, D, bf16):
+    """Few (head, query tile) items: the key axis is split across SMs; normalised partials in the library's workspace +
+    the merge kernel (2 launches).  Must match the oracle, also when run back to back."""
     import mfa_b200 as mfa
     desc = _descriptor(R, C, D, bf16)
     kernel = mfa.AttentionKernel(desc.kernelDescriptor(mfa.AttentionKernelType.forward))
     constants = mfa.FunctionConstantValues()
     desc.setFunctionConstants(constants)
-    mfa._lib.mfa_debug_set_forward_fused(1 if fused else 0)
-    try:
-        assert kernel.launchCount(constants) == (1 if fused else 2), "split-KV should engage for this grid"
-        _run_and_check(R, C, D, bf16, seed=R + C + D)
-        _run_and_check(R, C, D, bf16, seed=R + C + D + 1)
-    finally:
-        mfa._lib.mfa_debug_set_forward_fused(0)   # library default: scratch + combine (two launches)
+    assert kernel.launchCount(constants) == 2, "split-KV should engage for this grid"
+    _run_and_check(R, C, D, bf16, seed=R + C + D)
+    _run_and_check(R, C, D, bf16, seed=R + C + D + 1)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("fused", [True, False], ids=["fused-one-launch", "scratch-combine"])
-def test_split_kv_batched_heads_and_fp16_L(fused):
-    """Split-KV with several heads in one launch (item -> (head, tile, split)) and FP16 L storage."""
+@pytest.mark.parametrize("H,N,D", [(3, 1024, 128), (2, 700, 64)])
+def test_split_kv_batched_heads_and_fp16_L(H, N, D):
+    """Split-KV with several heads in one launch (item -> (head, tile, split)) and FP16 L storage; the second shape has
+    ragged query tiles and a ragged last key block in every head."""
     import mfa_b200 as mfa
-    H, N, D = 3, 1024, 128
     desc = _descriptor(N, N, D, True, lowMid=True, batch=H)
     kernel = mfa.AttentionKernel(desc.kernelDescriptor(mfa.AttentionKernelType.forward))
     constants = mfa.FunctionConstantValues()
     desc.setFunctionConstants(constants)
-    mfa._lib.mfa_debug_set_forward_fused(1 if fused else 0)
-    try:
-        assert kernel.launchCount(constants) == (1 if fused else 2)
-        _check_batched_cluster(desc, H, N, D)
-    finally:
-        mfa._lib.mfa_debug_set_forward_fused(0)
+    assert kernel.launchCount(constants) == 2
+    _check_batched_cluster(desc, H, N, D)
 
 
 def _check_batched_cluster(desc, H, N, D):
