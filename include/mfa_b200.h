@@ -58,7 +58,7 @@ typedef enum mfa_status {
 /** Thread-local, NUL-terminated description of the last error on the calling thread. */
 MFA_API const char *mfa_last_error(void);
 
-/** Library version / build info ("mfa_b200 x.y sm_90a"). */
+/** Library version / build info ("mfa_b200 x.y sm_90a").  0.5 appended mfa_attention_kernel_descriptor_t.causal. */
 MFA_API const char *mfa_version(void);
 
 /* ------------------------------------------------------------------------------------------ */
@@ -117,7 +117,15 @@ typedef struct mfa_attention_descriptor {
                                           tensor-core kernels (with the reference policy the backward kernels rewrite
                                           the staged BF16 dO tiles as FP16 on chip: wgmma cannot mix
                                           FP16 and BF16 operands in one MMA). */
-  uint8_t reserved0;
+  uint8_t causal;                      /* 0: every query row sees every key (reference).  1: causal mask, aligned
+                                          bottom-right: with delta = column - row (signed), query row i sees key j
+                                          iff j <= i + delta.  row == column is the usual lower-triangular mask; with
+                                          row < column the queries are the last `row` positions of a `column`-long
+                                          sequence (chunked prefill, KV cache).  With row > column the rows
+                                          i < row - column see no key: their O row is 0 and L = +inf, their D and dQ
+                                          row are 0 and they add nothing to dK / dV (P = exp2(S - L) = 0).  The same
+                                          mask applies to every problem of the batch.  Other values are rejected by
+                                          kernelDescriptor(type:) with MFA_ERROR_INVALID_ARGUMENT. */
   uint32_t batch_count;                /* 0 or 1: single head (reference). N > 1: N independent
                                           single-head problems, each operand stored back to back
                                           (operand i of problem b starts at b * elements(i)). */
@@ -174,6 +182,10 @@ typedef struct mfa_attention_kernel_descriptor {
   uint8_t split_min_blocks;  /* small grids: a traversal range handed to one CTA has at least this many traversal
                                 blocks (blockDimensions.traversal rows each); 0 = never split */
   uint8_t split_max;         /* small grids: at most this many ranges per tile (forward <= 16, backward <= 8) */
+  /* ---- library extension: the causal mask of mfa_attention_descriptor_t.causal (0 off, 1 bottom-right), copied by
+     kernelDescriptor(type:); editable like the fields above.  Other values are rejected by AttentionKernel(descriptor:).
+     Causal kernels visit only the blocks of the attention matrix that hold a visible (query, key) pair. ---- */
+  uint8_t causal;
 } mfa_attention_kernel_descriptor_t;
 
 /** AttentionKernelDescriptor.init(): everything nil / empty. */

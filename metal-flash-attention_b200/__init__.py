@@ -59,7 +59,7 @@ class _CDescriptor(ctypes.Structure):
         ("transpose_V", ctypes.c_uint8),
         ("transpose_O", ctypes.c_uint8),
         ("input_precision_override", ctypes.c_uint8),
-        ("reserved0", ctypes.c_uint8),
+        ("causal", ctypes.c_uint8),
         ("batch_count", ctypes.c_uint32),
     ]
 
@@ -84,6 +84,7 @@ class _CKernelDescriptor(ctypes.Structure):
         ("backend", ctypes.c_uint8),
         ("split_min_blocks", ctypes.c_uint8),
         ("split_max", ctypes.c_uint8),
+        ("causal", ctypes.c_uint8),
     ]
 
 
@@ -258,6 +259,9 @@ class AttentionDescriptor:
         # library extensions (include/mfa_b200.h): None = reference policy (FP16 inputs).
         self.inputPrecisionOverride: Optional[GEMMOperandPrecision] = None
         self.batchCount: int = 1
+        # causal mask aligned bottom-right: query row i sees key j iff j <= i + (column - row); rows with no visible key
+        # (row > column) get O = 0, L = +inf, D = 0, dQ = 0
+        self.causal: bool = False
 
     def _c(self) -> _CDescriptor:
         d = _CDescriptor()
@@ -271,6 +275,7 @@ class AttentionDescriptor:
             d.transpose_Q, d.transpose_K, d.transpose_V, d.transpose_O = (int(bool(x)) for x in self.transposeState)
         d.input_precision_override = int(self.inputPrecisionOverride) if self.inputPrecisionOverride else 0
         d.batch_count = int(self.batchCount)
+        d.causal = int(self.causal)  # (any value other than 0 / 1 is passed on, and rejected by the library)
         return d
 
     @property
@@ -443,6 +448,15 @@ class AttentionKernelDescriptor:
     @splitPolicy.setter
     def splitPolicy(self, value):
         self._c.split_min_blocks, self._c.split_max = (int(v) for v in value)
+
+    # ---- library extension: the causal mask (AttentionDescriptor.causal), editable like the fields above
+    @property
+    def causal(self) -> bool:
+        return bool(self._c.causal)
+
+    @causal.setter
+    def causal(self, value):
+        self._c.causal = int(value)
 
 
 # -------------------------------------------------------------------------------------------------

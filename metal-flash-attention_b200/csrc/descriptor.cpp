@@ -300,6 +300,7 @@ int kernel_descriptor(const mfa_attention_descriptor_t &d, int type, mfa_attenti
   // createHeadDimension / createTransposeState guard clauses (:88-111)
   if (!d.has_matrix_dimensions || !d.has_transpose_state)
     return fail(MFA_ERROR_INCOMPLETE_DESCRIPTOR, "Descriptor was incomplete.");
+  if (d.causal > 1) return fail(MFA_ERROR_INVALID_ARGUMENT, "Unrecognized causal mask mode.");
 
   // Fetch the kernel-specific parameters (:36-39).
   std::vector<ParameterRow> table;
@@ -382,6 +383,7 @@ int kernel_descriptor(const mfa_attention_descriptor_t &d, int type, mfa_attenti
                                    (1u << MFA_dV) | (1u << MFA_dK) | (1u << MFA_dQ);
   out.transpose_state_mask = t;
   out.type = static_cast<uint8_t>(type);
+  out.causal = d.causal;
   return MFA_SUCCESS;
 }
 
@@ -436,7 +438,7 @@ using namespace mfa;
 extern "C" {
 
 const char *mfa_last_error(void) { return g_last_error.c_str(); }
-const char *mfa_version(void) { return "mfa_b200 0.4 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family)"; }
+const char *mfa_version(void) { return "mfa_b200 0.5 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family)"; }
 
 int mfa_precision_size(mfa_precision_t precision) { return precision == MFA_FP32 ? 4 : 2; }
 const char *mfa_precision_name(mfa_precision_t precision) {

@@ -121,6 +121,8 @@ static int build_params(const mfa_attention_kernel *k, const mfa_function_consta
   // the tuning columns of the parameter-table row this kernel was created from
   p.split_min_blocks = k->descriptor.split_min_blocks;
   p.split_max = k->descriptor.split_max ? k->descriptor.split_max : 1;
+  p.causal = k->descriptor.causal;
+  p.causal_offset = static_cast<int32_t>(static_cast<int64_t>(p.C) - static_cast<int64_t>(p.R));
   int n = 0;
   const int *ops = operands_of(k->type, &n);
   for (int i = 0; i < n; ++i)
@@ -144,6 +146,7 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
     return fail(MFA_ERROR_INCOMPLETE_DESCRIPTOR, "Descriptor was incomplete.");
   if (kd->type > MFA_BACKWARD_KEY_VALUE) return fail(MFA_ERROR_INVALID_ARGUMENT, "Unrecognized kernel type.");
   if (kd->head_dimension == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "Head dimension must be at least 1.");
+  if (kd->causal > 1) return fail(MFA_ERROR_INVALID_ARGUMENT, "Unrecognized causal mask mode.");
 
   int n = 0;
   const int *ops = operands_of(kd->type, &n);
@@ -216,7 +219,7 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
   static const char *typeNames[] = {"forward", "backward_query", "backward_key_value"};
   k->source_name = std::string("attention_") + typeNames[k->type] +
                    (k->backend == MFA_BACKEND_TCGEN05 ? "_tcgen05" : "_simt_fp32") + "<D=" + std::to_string(D) +
-                   ">";
+                   ">" + (kd->causal ? "_causal" : "");
   *out = k;
   return MFA_SUCCESS;
 }
@@ -379,7 +382,7 @@ bool same_descriptor(const mfa_attention_descriptor_t &a, const mfa_attention_de
          a.has_matrix_dimensions == b.has_matrix_dimensions && a.has_transpose_state == b.has_transpose_state &&
          a.head == b.head && a.transpose_Q == b.transpose_Q && a.transpose_K == b.transpose_K &&
          a.transpose_V == b.transpose_V && a.transpose_O == b.transpose_O &&
-         a.input_precision_override == b.input_precision_override &&
+         a.input_precision_override == b.input_precision_override && a.causal == b.causal &&
          // with transposed operands the kernel family depends on R % 8 / C % 8 (TMA row pitch)
          select_backend(a, MFA_FORWARD) == select_backend(b, MFA_FORWARD);
 }

@@ -26,6 +26,9 @@ struct AttentionParams {
   // tuning columns of the parameter-table row the kernel was created from (tensor-core family)
   uint8_t split_min_blocks;  // 0 = never split small grids
   uint8_t split_max;
+  // causal mask, aligned bottom-right: row i sees key j iff j <= i + causal_offset (causal_offset = C - R)
+  uint8_t causal;
+  int32_t causal_offset;
 };
 
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------

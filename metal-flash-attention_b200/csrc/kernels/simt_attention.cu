@@ -13,6 +13,8 @@
 //   backward dK/dV  loopBackwardKeyValue  AttentionKernel+Source.swift:244-293
 // Numerical conventions: log2-domain running max m, L = m + log2(l),
 // D stored pre-scaled by 1/sqrt(D), BF16 stores truncate, edge columns masked before softmax.
+// Causal (p.causal): row r sees column c iff c <= r + p.causal_offset; the loops skip the 64-blocks no row of the CTA
+// can see, the mask is applied with the edge mask, and a row that sees no column gets O = 0, L = +inf.
 //
 // Tiling: one CTA = 256 threads = a 64 x 64 block of the attention matrix; thread (tx, ty) owns
 // the 4 x 4 patch {rows ty+16i} x {cols tx+16j}.  Operands are staged through shared memory as
@@ -179,6 +181,17 @@ __device__ __forceinline__ float row_sum16(float v) {
   return v;
 }
 
+// Causal: end of the columns the rows [r0, r0 + 64) can see (all C when not causal)
+__device__ __forceinline__ uint32_t visible_columns(const AttentionParams &p, uint32_t r0) {
+  if (!p.causal) return p.C;
+  const int last = static_cast<int>(min(r0 + kBlock, p.R)) - 1 + p.causal_offset;  // last column of the last row
+  return last < 0 ? 0u : min(p.C, static_cast<uint32_t>(last) + 1);
+}
+// masked: column c is past the edge, or past the diagonal of row r
+__device__ __forceinline__ bool masked(const AttentionParams &p, uint32_t r, uint32_t c) {
+  return c >= p.C || (p.causal && static_cast<int>(c) > static_cast<int>(r) + p.causal_offset);
+}
+
 __device__ __forceinline__ Operand make_operand(const AttentionParams &p, int slot, uint32_t seq, uint32_t b) {
   Operand op;
   size_t bytes = static_cast<size_t>(seq) * p.D * (p.prec[slot] == FP32 ? 4 : 2);
@@ -237,7 +250,8 @@ __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const Attenti
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] = 0.f;
 
-  for (uint32_t c0 = 0; c0 < p.C; c0 += kBlock) {
+  const uint32_t cend = visible_columns(p, r0);
+  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
     float s[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -247,11 +261,11 @@ __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const Attenti
 
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      // edge mask (AttentionKernel+Softmax.swift:228-260), then online max / correction / sum (:267-324)
+      // edge (and causal) mask (AttentionKernel+Softmax.swift:228-260), then online max / correction / sum (:267-324)
       float mx = -FLT_MAX;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        if (c0 + tx + 16 * j >= p.C) s[i][j] = -INFINITY;
+        if (masked(p, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
         mx = fmaxf(mx, s[i][j]);
       }
       mx = row_max16(mx);
@@ -277,16 +291,21 @@ __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const Attenti
   }
 
   // O *= 1/l on the last iteration (AttentionKernel+Source.swift:169-171); L = m + log2(l) (+Caching.swift:373-377)
+  // causal: a row that sees no column (r + offset < 0) gets O = 0 and L = +inf
   float inv[4];
+  bool empty[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) inv[i] = 1.0f / l[i];
+  for (int i = 0; i < 4; ++i) {
+    empty[i] = p.causal && static_cast<int>(r0 + ty + 16 * i) + p.causal_offset < 0;
+    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
+  }
   store_acc<NCH>(acc, inv, p, sO, p.R, b, r0, 0, p.D, tx, ty);
   if (tx == 0 && p.buf[sL] != nullptr) {
     char *Lbase = static_cast<char *>(p.buf[sL]) + static_cast<size_t>(b) * p.R * (p.prec[sL] == FP32 ? 4 : 2);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       uint32_t r = r0 + ty + 16 * i;
-      if (r < p.R) store_elem(Lbase, r, p.prec[sL], m[i] + log2f(l[i]));
+      if (r < p.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
     }
   }
 }
@@ -328,7 +347,8 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const 
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] = 0.f;
 
-  for (uint32_t c0 = 0; c0 < p.C; c0 += kBlock) {
+  const uint32_t cend = visible_columns(p, r0);
+  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
     float s[4][4], dp[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -341,7 +361,7 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const 
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         // P = exp2(S * log2e/sqrt(D) - L);  dS = P * (dP/sqrt(D) - D)   (+Softmax.swift:419-427)
-        float pv = (c0 + tx + 16 * j < p.C) ? exp2f(fmaf(s[i][j], p.scale_log2, -Lrow[i])) : 0.f;
+        float pv = !masked(p, r0 + ty + 16 * i, c0 + tx + 16 * j) ? exp2f(fmaf(s[i][j], p.scale_log2, -Lrow[i])) : 0.f;
         sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv * fmaf(dp[i][j], p.scale, -Drow[i]);
       }
     accumulate<NCH>(acc, sP, K, c0, 0, p.D, sX, tid, tx, ty);  // dQ += dS K
@@ -376,7 +396,10 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(co
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) accV[q][i][jj] = accK[q][i][jj] = 0.f;
 
-  for (uint32_t r0 = 0; r0 < p.R; r0 += kBlock) {
+  // causal: start at the 64-block holding the first row that sees column c0 (r >= c0 - offset)
+  const int first = static_cast<int>(c0) - p.causal_offset;
+  const uint32_t rstart = p.causal && first > 0 ? static_cast<uint32_t>(first) / kBlock * kBlock : 0;
+  for (uint32_t r0 = rstart; r0 < p.R; r0 += kBlock) {
     float s[4][4], dp[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -395,7 +418,9 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(co
       float Dr = load_elem(Dbase, rc, p.prec[sD]);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        float e = (r < p.R) ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr)) : 0.f;
+        float e = (r < p.R && !(p.causal && static_cast<int>(c0 + tx + 16 * j) > static_cast<int>(r) + p.causal_offset))
+                      ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr))
+                      : 0.f;
         pv[i][j] = e;
         dp[i][j] = e * fmaf(dp[i][j], p.scale, -Dr);  // dS
         sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = e;  // P^T

@@ -15,6 +15,10 @@
 // padded to 64 / 128 / 256 columns by TMA's zero fill of the out-of-range box columns, rows past R / C are zero-filled
 // the same way and masked out of the softmax.  Numerical conventions as in simt_attention.cu: log2-domain running max,
 // L = m + log2(l), D pre-scaled by 1/sqrt(D).
+//
+// Causal (kCausal, bottom-right aligned: query row i sees key j iff j <= i + delta, delta = C - R): every CTA visits only
+// the traversal blocks its rows can see, and only the blocks that cross the diagonal mask elements (S -> -inf before the
+// softmax / before P = exp2(S - L)).  A row that sees no key (i < R - C) gets O = 0, L = +inf, D = 0, dQ = 0.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -103,6 +107,30 @@ __device__ __forceinline__ void store_acc(const float (&acc)[NR], float *out, ui
   }
 }
 
+// Causal: how many of the key blocks [kb0, kb0 + per_split) the rows [row_base, min(row_base + rows, R)) can see (key
+// j <= row + delta).  Signed: a split range can lie wholly past the diagonal, and with R > C a tile can see no key at all.
+template <uint32_t BN>
+__device__ __forceinline__ uint32_t visible_key_blocks(uint32_t row_base, uint32_t rows, uint32_t R, uint32_t C,
+                                                       int delta, uint32_t kb0, uint32_t per_split) {
+  const int last_key = static_cast<int>(min(row_base + rows, R)) - 1 + delta;  // seen by the tile's last row
+  const int end = last_key < 0 ? 0 : min(static_cast<int>((C + BN - 1) / BN), last_key / static_cast<int>(BN) + 1);
+  return static_cast<uint32_t>(max(0, min(end, static_cast<int>(kb0 + per_split)) - static_cast<int>(kb0)));
+}
+
+// Causal: S -> -inf for the keys past the diagonal in a 64 x BN accumulator block whose first key column is `key0`;
+// row_a is this thread's first row (the second is row_a + 8)
+template <int NR>
+__device__ __forceinline__ void mask_past_diagonal(float (&s)[NR], int key0, int row_a, int delta) {
+  const int c0 = key0 + 2 * static_cast<int>(threadIdx.x % 4), lim0 = row_a + delta, lim1 = lim0 + 8;
+#pragma unroll
+  for (int i = 0; i < NR / 4; ++i)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      if (c0 + 8 * i + e > lim0) s[4 * i + e] = -INFINITY;
+      if (c0 + 8 * i + e > lim1) s[4 * i + 2 + e] = -INFINITY;
+    }
+}
+
 // ================================================================================================ forward
 // Split-KV (few query tiles for 132 SMs): the key axis of every tile is cut into `splits` equal ranges handled by
 // separate CTAs (blockIdx.z), each leaving a normalised partial O and its log2-sum-exp in the library's workspace,
@@ -112,7 +140,9 @@ struct SplitArgs {
   float *O_part, *L_part;  // [split][head][R][D], [split][head][R]
 };
 
-// O[row][4 quad ..] and L[row] from the partials of every split (row = head * R + r): one thread per (row, 4 columns)
+// O[row][4 quad ..] and L[row] from the partials of every split (row = head * R + r): one thread per (row, 4 columns).
+// Causal: a split that saw no key of a row left L = -inf (weight 0); a row that no split saw gets O = 0, L = +inf.
+template <bool kCausal>
 __global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O, void *L, int l_prec, uint64_t rows_total,
                                                     uint32_t D) {
   const uint64_t idx = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -121,10 +151,11 @@ __global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O
   const uint32_t quad = static_cast<uint32_t>(idx % (D / 4));
   float lmax = -INFINITY;
   for (uint32_t s = 0; s < sp.splits; ++s) lmax = fmaxf(lmax, __ldcg(sp.L_part + s * rows_total + row));
+  const float lref = kCausal && lmax == -INFINITY ? 0.f : lmax;
   float denom = 0.f;
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
   for (uint32_t s = 0; s < sp.splits; ++s) {
-    const float w = exp2f(__ldcg(sp.L_part + s * rows_total + row) - lmax);
+    const float w = exp2f(__ldcg(sp.L_part + s * rows_total + row) - lref);
     const float4 v = __ldcg(reinterpret_cast<const float4 *>(sp.O_part + (s * rows_total + row) * D) + quad);
     denom += w;
     acc.x = fmaf(w, v.x, acc.x);
@@ -132,9 +163,10 @@ __global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O
     acc.z = fmaf(w, v.z, acc.z);
     acc.w = fmaf(w, v.w, acc.w);
   }
-  const float inv = 1.0f / denom;
+  const bool empty = kCausal && denom == 0.f;
+  const float inv = empty ? 0.f : 1.0f / denom;
   *reinterpret_cast<float4 *>(O + row * D + 4 * quad) = make_float4(acc.x * inv, acc.y * inv, acc.z * inv, acc.w * inv);
-  if (quad == 0) store_stat(L, row, l_prec, lmax + log2f(denom));
+  if (quad == 0) store_stat(L, row, l_prec, empty ? INFINITY : lmax + log2f(denom));
 }
 
 // kPar / kTrav: rows of the parallelization / traversal axis per CTA / per pipeline stage (every *Cfg has them)
@@ -146,11 +178,12 @@ struct FwdCfg {
   static constexpr uint32_t kSmemBytes = 1024 + kQBytes + 2 * 2 * kKVBytes + kBarBytes;
 };
 
-template <uint32_t DCH, bool kBF16>
+template <uint32_t DCH, bool kBF16, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
     attention_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                             const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                            uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp) {
+                            uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp,
+                            int delta) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -158,10 +191,12 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   uint8_t *kv = base + Cfg::kQBytes;  // stage s: K at kv + 2 s kKVBytes, V right after it
   uint64_t *bar = reinterpret_cast<uint64_t *>(kv + 4 * Cfg::kKVBytes);  // [0] Q, [1 + s] stage s
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
+  // (causal: unlike dQ, the forward gains nothing measurable from starting the tiles with the most key blocks first)
   const uint32_t head = blockIdx.y, row_base = blockIdx.x * Cfg::kTileM;
   // this CTA's key blocks: [kb0, kb0 + blocks)
   const uint32_t kb0 = blockIdx.z * sp.blocks_per_split;
-  const uint32_t blocks = min((C + BN - 1) / BN - kb0, sp.blocks_per_split);
+  const uint32_t blocks = kCausal ? visible_key_blocks<BN>(row_base, Cfg::kTileM, R, C, delta, kb0, sp.blocks_per_split)
+                                  : min((C + BN - 1) / BN - kb0, sp.blocks_per_split);
 
   auto load_kv = [&](uint32_t j, uint32_t s) {
     uint8_t *dst = kv + s * 2 * Cfg::kKVBytes;
@@ -211,6 +246,11 @@ __global__ void __launch_bounds__(2 * kWG, 1)
         for (uint32_t e = 0; e < 2; ++e)
           if (c0 + 8 * i + e >= C) sc[4 * i + e] = sc[4 * i + 2 + e] = -INFINITY;
     }
+    if constexpr (kCausal) {
+      const int key0 = static_cast<int>((kb0 + j) * BN);
+      if (key0 + static_cast<int>(BN) - 1 > static_cast<int>(row_base) + delta)  // the block crosses the diagonal
+        mask_past_diagonal(sc, key0, static_cast<int>(row_base + wg * kRows + (t / 32) * 16 + (t % 32) / 4), delta);
+    }
     float r0 = -INFINITY, r1 = -INFINITY;
 #pragma unroll
     for (uint32_t i = 0; i < BN / 8; ++i) {
@@ -222,7 +262,9 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     r1 = fmaxf(r1, __shfl_xor_sync(0xffffffffu, r1, 1));
     r1 = fmaxf(r1, __shfl_xor_sync(0xffffffffu, r1, 2));
     const float mn0 = fmaxf(m0, r0 * scale_log2), mn1 = fmaxf(m1, r1 * scale_log2);
-    const float a0 = ex2_approx(m0 - mn0), a1 = ex2_approx(m1 - mn1);  // 0 on the first block (m = -inf)
+    // causal: a row that has seen no key yet keeps m = -inf; 0 stands in for it as the reference value (else -inf - -inf)
+    const float ref0 = kCausal && mn0 == -INFINITY ? 0.f : mn0, ref1 = kCausal && mn1 == -INFINITY ? 0.f : mn1;
+    const float a0 = ex2_approx(m0 - ref0), a1 = ex2_approx(m1 - ref1);  // 0 on the first block (m = -inf)
     m0 = mn0;
     m1 = mn1;
     l0 *= a0;
@@ -236,10 +278,10 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     }
 #pragma unroll
     for (uint32_t i = 0; i < BN / 8; ++i) {
-      sc[4 * i] = ex2_approx(fmaf(sc[4 * i], scale_log2, -m0));
-      sc[4 * i + 1] = ex2_approx(fmaf(sc[4 * i + 1], scale_log2, -m0));
-      sc[4 * i + 2] = ex2_approx(fmaf(sc[4 * i + 2], scale_log2, -m1));
-      sc[4 * i + 3] = ex2_approx(fmaf(sc[4 * i + 3], scale_log2, -m1));
+      sc[4 * i] = ex2_approx(fmaf(sc[4 * i], scale_log2, -ref0));
+      sc[4 * i + 1] = ex2_approx(fmaf(sc[4 * i + 1], scale_log2, -ref0));
+      sc[4 * i + 2] = ex2_approx(fmaf(sc[4 * i + 2], scale_log2, -ref1));
+      sc[4 * i + 3] = ex2_approx(fmaf(sc[4 * i + 3], scale_log2, -ref1));
       l0 += sc[4 * i] + sc[4 * i + 1];
       l1 += sc[4 * i + 2] + sc[4 * i + 3];
     }
@@ -265,14 +307,17 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   // unsplit: O and L straight to the caller; split: the normalised partial of this key range
   const size_t slice = static_cast<size_t>(blockIdx.z) * sp.batch + head;
   float *Oout = sp.splits == 1 ? O + static_cast<size_t>(head) * R * D : sp.O_part + slice * R * D;
-  store_acc(o, Oout, row0, R, 0, D, 1.0f / l0, 1.0f / l1);
+  // causal: a row that saw no key (l = 0) gets O = 0 and L = +inf, or L = -inf (weight 0 in the merge) as a split partial
+  const bool empty0 = kCausal && l0 == 0.f, empty1 = kCausal && l1 == 0.f;
+  store_acc(o, Oout, row0, R, 0, D, empty0 ? 0.f : 1.0f / l0, empty1 ? 0.f : 1.0f / l1);
   if (t % 4 == 0) {
     const uint32_t r = row0 + (t / 32) * 16 + (t % 32) / 4;
     void *Lout = sp.splits == 1 ? L : sp.L_part;
     const int prec = sp.splits == 1 ? l_prec : FP32;
     const size_t hb = (sp.splits == 1 ? static_cast<size_t>(head) : slice) * R;
-    if (r < R) store_stat(Lout, hb + r, prec, m0 + log2f(l0));
-    if (r + 8 < R) store_stat(Lout, hb + r + 8, prec, m1 + log2f(l1));
+    const float none = sp.splits == 1 ? INFINITY : -INFINITY;
+    if (r < R) store_stat(Lout, hb + r, prec, empty0 ? none : m0 + log2f(l0));
+    if (r + 8 < R) store_stat(Lout, hb + r + 8, prec, empty1 ? none : m1 + log2f(l1));
   }
 }
 
@@ -297,9 +342,10 @@ struct BwdArgs {
   uint32_t R, C, D;
   float scale, scale_log2;
   int l_prec, d_prec, dO_bf16;
+  int delta;  // causal kernels: query row i sees key j iff j <= i + delta
 };
 
-template <uint32_t DCH, bool kBF16, bool kConvertDO>
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
 __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     attention_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
                                    const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
@@ -311,9 +357,12 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   uint8_t *kv = base + 2 * Cfg::kQBytes;
   uint64_t *bar = reinterpret_cast<uint64_t *>(kv + 4 * Cfg::kKVBytes);
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
-  const uint32_t head = blockIdx.y, row_base = blockIdx.x * Cfg::kTileM;
+  // causal: tiles in reverse order, so that the ones with the most key blocks start first and the wave tail is short
+  const uint32_t tile = kCausal ? gridDim.x - 1 - blockIdx.x : blockIdx.x;
+  const uint32_t head = blockIdx.y, row_base = tile * Cfg::kTileM;
   const uint32_t kb0 = blockIdx.z * a.blocks_per_split;
-  const uint32_t blocks = min((a.C + BN - 1) / BN - kb0, a.blocks_per_split);
+  const uint32_t blocks = kCausal ? visible_key_blocks<BN>(row_base, Cfg::kTileM, a.R, a.C, a.delta, kb0, a.blocks_per_split)
+                                  : min((a.C + BN - 1) / BN - kb0, a.blocks_per_split);
 
   auto load_kv = [&](uint32_t j, uint32_t s) {
     uint8_t *dst = kv + s * 2 * Cfg::kKVBytes;
@@ -387,6 +436,11 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     wgmma_wait<0>();
     fence_regs(sc);
     fence_regs(dp);
+    if constexpr (kCausal) {  // S -> -inf past the diagonal, so P = 0 there
+      const int key0 = static_cast<int>((kb0 + j) * BN);
+      if (key0 + static_cast<int>(BN) - 1 > static_cast<int>(row_base) + a.delta)
+        mask_past_diagonal(sc, key0, static_cast<int>(r), a.delta);
+    }
     const uint32_t c0 = (kb0 + j) * BN + 2 * (t % 4);
 #pragma unroll
     for (uint32_t i = 0; i < BN / 8; ++i)
@@ -413,6 +467,19 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
 }
 
 // ================================================================================================ backward dK/dV
+// Causal: the first query block that sees key `key` (query >= key - delta), and how many of the blocks [qs, qb0 +
+// per_split) exist (signed: a split range can end before qs)
+template <uint32_t BM>
+__device__ __forceinline__ uint32_t first_query_block(uint32_t key, int delta) {
+  const int q = static_cast<int>(key) - delta;
+  return q <= 0 ? 0u : static_cast<uint32_t>(q) / BM;
+}
+template <uint32_t BM>
+__device__ __forceinline__ uint32_t visible_query_blocks(uint32_t R, uint32_t qb0, uint32_t qs, uint32_t per_split) {
+  const int end = min(static_cast<int>((R + BM - 1) / BM), static_cast<int>(qb0 + per_split));
+  return static_cast<uint32_t>(max(0, end - static_cast<int>(qs)));
+}
+
 template <uint32_t DCH>
 struct KVCfg {
   static constexpr bool kSplitD = DCH == 4;  // both warpgroups on the same 64 keys, half of the D columns each
@@ -423,7 +490,7 @@ struct KVCfg {
   static constexpr uint32_t kSmemBytes = 1024 + 2 * kKBytes + 2 * 2 * kQBytes + kBarBytes;
 };
 
-template <uint32_t DCH, bool kBF16, bool kConvertDO>
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
     attention_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
                                        const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
@@ -437,13 +504,16 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   const uint32_t head = blockIdx.y, key_base = blockIdx.x * Cfg::kTileN;
   const uint32_t qb0 = blockIdx.z * a.blocks_per_split;
-  const uint32_t blocks = min((a.R + BM - 1) / BM - qb0, a.blocks_per_split);
+  // causal: this CTA's query blocks start at the first one that sees the tile's first key (query >= key_base - delta)
+  const uint32_t qs = kCausal ? max(qb0, first_query_block<BM>(key_base, a.delta)) : qb0;
+  const uint32_t blocks = kCausal ? visible_query_blocks<BM>(a.R, qb0, qs, a.blocks_per_split)
+                                  : min((a.R + BM - 1) / BM - qb0, a.blocks_per_split);
 
   auto load_qd = [&](uint32_t i, uint32_t s) {
     uint8_t *dst = qd + s * 2 * Cfg::kQBytes;
     mbar_arrive_expect_tx(&bar[1 + s], 2 * Cfg::kQBytes);
-    load_tile<DCH, BM>(dst, &mapQ, &bar[1 + s], (qb0 + i) * BM, head);
-    load_tile<DCH, BM>(dst + Cfg::kQBytes, &mapdO, &bar[1 + s], (qb0 + i) * BM, head);
+    load_tile<DCH, BM>(dst, &mapQ, &bar[1 + s], (qs + i) * BM, head);
+    load_tile<DCH, BM>(dst + Cfg::kQBytes, &mapdO, &bar[1 + s], (qs + i) * BM, head);
   };
   if (tid == 0) {
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
@@ -468,7 +538,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     const uint32_t s = i & 1;
     // per-query statistics of this thread's 16 columns, loaded while the tiles land
     float Lq[BM / 4], Dq[BM / 4];
-    const uint32_t q0 = (qb0 + i) * BM + 2 * (t % 4);
+    const uint32_t q0 = (qs + i) * BM + 2 * (t % 4);
 #pragma unroll
     for (uint32_t j = 0; j < BM / 8; ++j)
 #pragma unroll
@@ -501,6 +571,20 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     wgmma_wait<0>();
     fence_regs(st);
     fence_regs(dpt);
+    if constexpr (kCausal) {  // S^T -> -inf where key > query + delta, so P^T = 0 there
+      const int qlo = static_cast<int>((qs + i) * BM);
+      if (static_cast<int>(key_base + Cfg::kTileN) - 1 > qlo + a.delta) {
+        const int kr = static_cast<int>(key_base + krow + (t / 32) * 16 + (t % 32) / 4);
+        const int qc = qlo + 2 * static_cast<int>(t % 4) + a.delta;
+#pragma unroll
+        for (int j = 0; j < static_cast<int>(BM / 8); ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (kr > qc + 8 * j + e) st[4 * j + e] = -INFINITY;
+            if (kr + 8 > qc + 8 * j + e) st[4 * j + 2 + e] = -INFINITY;
+          }
+      }
+    }
 #pragma unroll
     for (uint32_t j = 0; j < BM / 8; ++j)
 #pragma unroll
@@ -598,10 +682,10 @@ static cudaError_t prepare(Kernel kernel, uint32_t smem) {
   return ensure_max_dynamic_smem(reinterpret_cast<const void *>(kernel), smem, current_device());
 }
 
-template <uint32_t DCH, bool kBF16>
+template <uint32_t DCH, bool kBF16, bool kCausal>
 cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
   using Cfg = FwdCfg<DCH>;
-  auto kernel = attention_forward_wgmma<DCH, kBF16>;
+  auto kernel = attention_forward_wgmma<DCH, kBF16, kCausal>;
   cudaError_t e;
   if ((e = prepare(kernel, Cfg::kSmemBytes)) != cudaSuccess) return e;
   CUtensorMap mapQ, mapK, mapV;
@@ -620,11 +704,12 @@ cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cuda
     sp.L_part = sp.O_part + o_elems;
   }
   kernel<<<plan.grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapK, mapV, static_cast<float *>(p.buf[sO]),
-                                                                p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp);
+                                                                p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp,
+                                                                p.causal_offset);
   if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
   const uint64_t threads = rows_total * (p.D / 4);
-  merge_splits<<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(sp, static_cast<float *>(p.buf[sO]),
-                                                                                 p.buf[sL], p.prec[sL], rows_total, p.D);
+  merge_splits<kCausal><<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(
+      sp, static_cast<float *>(p.buf[sO]), p.buf[sL], p.prec[sL], rows_total, p.D);
   return cudaGetLastError();
 }
 
@@ -666,13 +751,14 @@ static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
   a.l_prec = p.prec[sL];
   a.d_prec = p.prec[sD];
   a.dO_bf16 = p.prec[sdO] == BF16;
+  a.delta = p.causal_offset;
   return a;
 }
 
-template <uint32_t DCH, bool kBF16, bool kConvertDO>
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
 cudaError_t launch_query(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
   using Cfg = QCfg<DCH>;
-  auto kernel = attention_backward_query_wgmma<DCH, kBF16, kConvertDO>;
+  auto kernel = attention_backward_query_wgmma<DCH, kBF16, kConvertDO, kCausal>;
   cudaError_t e;
   if ((e = prepare(kernel, Cfg::kSmemBytes)) != cudaSuccess) return e;
   CUtensorMap mapQ, mapdO, mapK, mapV;
@@ -693,10 +779,10 @@ cudaError_t launch_query(const AttentionParams &p, const WgmmaPlan &plan, cudaSt
                     stream);
 }
 
-template <uint32_t DCH, bool kBF16, bool kConvertDO>
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
 cudaError_t launch_key_value(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
   using Cfg = KVCfg<DCH>;
-  auto kernel = attention_backward_key_value_wgmma<DCH, kBF16, kConvertDO>;
+  auto kernel = attention_backward_key_value_wgmma<DCH, kBF16, kConvertDO, kCausal>;
   cudaError_t e;
   if ((e = prepare(kernel, Cfg::kSmemBytes)) != cudaSuccess) return e;
   CUtensorMap mapQ, mapdO, mapK, mapV;
@@ -718,13 +804,16 @@ cudaError_t launch_key_value(const AttentionParams &p, const WgmmaPlan &plan, cu
                     a.split_stride, plan.splits, stream);
 }
 
-// Calls f(DCH, kBF16, kConvertDO), each as a std::integral_constant, for the kernel instantiation that serves p
+// Calls f(DCH, kBF16, kConvertDO, kCausal), each as a std::integral_constant, for the kernel instantiation that serves p
 template <class F>
 static cudaError_t dispatch(const AttentionParams &p, bool convert_dO, F f) {
   return with_chunks(p.D, [&](auto dch) {
-    if (convert_dO) return f(dch, std::false_type(), std::true_type());
-    if (p.prec[sQ] == BF16) return f(dch, std::true_type(), std::false_type());
-    return f(dch, std::false_type(), std::false_type());
+    auto types = [&](auto causal) {
+      if (convert_dO) return f(dch, std::false_type(), std::true_type(), causal);
+      if (p.prec[sQ] == BF16) return f(dch, std::true_type(), std::false_type(), causal);
+      return f(dch, std::false_type(), std::false_type(), causal);
+    };
+    return p.causal ? types(std::true_type()) : types(std::false_type());
   });
 }
 
@@ -788,8 +877,8 @@ cudaError_t launch_wgmma_forward(const AttentionParams &p, cudaStream_t stream) 
     return cudaErrorInvalidValue;
   }
   const WgmmaPlan plan = plan_for(MFA_FORWARD, p, false);
-  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto) {
-    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value>(p, plan, stream);
+  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
+    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, stream);
   });
 }
 
@@ -806,8 +895,9 @@ cudaError_t launch_wgmma_backward_query(const AttentionParams &p, cudaStream_t s
   }
   const bool convert = p.prec[sdO] != p.prec[sQ];
   const WgmmaPlan plan = plan_for(MFA_BACKWARD_QUERY, p, convert);
-  return hop::dispatch(p, convert, [&](auto dch, auto bf16, auto cvt) {
-    return hop::launch_query<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value>(p, plan, stream);
+  return hop::dispatch(p, convert, [&](auto dch, auto bf16, auto cvt, auto causal) {
+    return hop::launch_query<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value,
+                             decltype(causal)::value>(p, plan, stream);
   });
 }
 
@@ -828,8 +918,9 @@ cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream
     q.buf[sdO] = converted;
     q.prec[sdO] = q.prec[sQ];
   }
-  return hop::dispatch(q, convert && !plan.convert_dO_first, [&](auto dch, auto bf16, auto cvt) {
-    return hop::launch_key_value<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value>(q, plan, stream);
+  return hop::dispatch(q, convert && !plan.convert_dO_first, [&](auto dch, auto bf16, auto cvt, auto causal) {
+    return hop::launch_key_value<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value,
+                                 decltype(causal)::value>(q, plan, stream);
   });
 }
 

@@ -43,6 +43,8 @@ struct AttentionKernelDescriptor {  // AttentionKernelDescriptor.swift:7-48
   // library extension: the tuning columns of the parameter-table row (editable like every other field)
   uint8_t &splitMinBlocks() { return c.split_min_blocks; }
   uint8_t &splitMax() { return c.split_max; }
+  // library extension: the causal mask (0 off, 1 bottom-right aligned), copied from AttentionDescriptor::causal
+  uint8_t &causal() { return c.causal; }
   bool tensorCoreFamily() const { return c.backend == MFA_BACKEND_TCGEN05; }
 };
 
@@ -58,6 +60,7 @@ struct AttentionDescriptor {  // AttentionDescriptor.swift:10-27
   std::optional<TransposeState> transposeState;
   std::optional<GEMMOperandPrecision> inputPrecisionOverride;  // library extension
   uint32_t batchCount = 1;                                     // library extension
+  bool causal = false;  // library extension: query row i sees key j iff j <= i + (column - row)
 
   mfa_attention_descriptor_t c() const {
     mfa_attention_descriptor_t d;
@@ -75,6 +78,7 @@ struct AttentionDescriptor {  // AttentionDescriptor.swift:10-27
     }
     d.input_precision_override = inputPrecisionOverride ? static_cast<uint8_t>(*inputPrecisionOverride) : 0;
     d.batch_count = batchCount;
+    d.causal = causal ? 1 : 0;
     return d;
   }
   AttentionKernelDescriptor kernelDescriptor(AttentionKernelType type) const {  // AttentionDescriptor.swift:33-130

@@ -50,6 +50,9 @@ public struct AttentionDescriptor {
   public var inputPrecisionOverride: GEMMOperandPrecision?
   /// library extension: number of independent single-head problems stored back to back.
   public var batchCount: UInt32 = 1
+  /// library extension: causal mask aligned bottom-right (query row i sees key j iff j <= i + column - row); rows
+  /// with no visible key get O = 0, L = +inf, D = 0, dQ = 0.
+  public var causal: Bool = false
 
   public init() {}
 
@@ -69,6 +72,7 @@ public struct AttentionDescriptor {
     }
     d.input_precision_override = UInt8(inputPrecisionOverride?.rawValue ?? 0)
     d.batch_count = batchCount
+    d.causal = causal ? 1 : 0
     return d
   }
 
@@ -287,6 +291,12 @@ public struct AttentionKernelDescriptor {
   public var splitPolicy: (minimumBlocks: UInt8, maximumSplits: UInt8) {
     get { (c.split_min_blocks, c.split_max) }
     set { c.split_min_blocks = newValue.minimumBlocks; c.split_max = newValue.maximumSplits }
+  }
+
+  /// library extension: the causal mask copied from AttentionDescriptor.causal (editable like the fields above).
+  public var causal: Bool {
+    get { c.causal != 0 }
+    set { c.causal = newValue ? 1 : 0 }
   }
 }
 
