@@ -4,7 +4,6 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace mfa {
 namespace ptx {
@@ -58,6 +57,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
 
 // Bounded wait: a protocol bug must surface as a trapped kernel (an error the host reports), never
 // as a hung GPU.  ~4 s at 2 GHz; the check costs nothing on the fast path.
+// A trap from a kernel of this library therefore means a barrier protocol error (a wait whose phase never completes).
+// The branch holds no printf: any call in a kernel makes ptxas serialize every wgmma of that kernel (C7510).  To find
+// the barrier, block and parity that timed out, add a printf before the __trap locally.
 #ifndef MFA_MBAR_TIMEOUT_CYCLES
 #define MFA_MBAR_TIMEOUT_CYCLES (8000000000ll)
 #endif
@@ -65,13 +67,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long start = clock64();
   uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3ffu) == 0 && clock64() - start > MFA_MBAR_TIMEOUT_CYCLES) {
-      printf("mfa: mbarrier timeout block (%d,%d) thread %d bar@%u parity %u\n", blockIdx.x, blockIdx.y,
-             threadIdx.x, smem_u32(bar), parity);
-      __trap();
-    }
-  }
+  while (!mbar_try_wait(bar, parity))
+    if ((++spins & 0x3ffu) == 0 && clock64() - start > MFA_MBAR_TIMEOUT_CYCLES) __trap();
 }
 
 // ---------------------------------------------------------------- streaming global loads -----

@@ -291,6 +291,13 @@ __global__ void __launch_bounds__(2 * kWG, 1)
       uint32_t a[4];
       a_frag<kBF16>(sc, kk, a);
       Wgmma<NO, kBF16>::rs(o, a, desc_mnmajor<BN>(sV, kk, 0), 1);
+      // D <= 64: retiring each K step before packing the next A fragment keeps the kernel within 128 registers, so
+      // two CTAs share an SM (their shared memory fits twice); with every fragment in flight it takes 145 and one CTA
+      // per SM, about 12 % slower
+      if constexpr (DCH == 1) {
+        wgmma_commit();
+        wgmma_wait<0>();
+      }
     }
     wgmma_commit();
     wgmma_wait<0>();
