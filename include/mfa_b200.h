@@ -58,7 +58,8 @@ typedef enum mfa_status {
 /** Thread-local, NUL-terminated description of the last error on the calling thread. */
 MFA_API const char *mfa_last_error(void);
 
-/** Library version / build info ("mfa_b200 x.y sm_90a").  0.5 appended mfa_attention_kernel_descriptor_t.causal. */
+/** Library version / build info ("mfa_b200 x.y sm_90a").  0.5 appended mfa_attention_kernel_descriptor_t.causal and
+ *  mfa_function_constants_t.kv_group. */
 MFA_API const char *mfa_version(void);
 
 /* ------------------------------------------------------------------------------------------ */
@@ -224,11 +225,21 @@ MFA_API const char *mfa_attention_descriptor_parameter_file(const mfa_attention_
 MFA_API int mfa_set_parameter_table(mfa_kernel_type_t type, int transposed, const char *text);
 
 /** descriptor.setFunctionConstants(_:)  (AttentionDescriptor.swift:139-148): the two launch-time
- *  constants R (index 0) and C (index 1), plus the batch extension. */
+ *  constants R (index 0) and C (index 1), plus the batch and K/V-group extensions. */
 typedef struct mfa_function_constants {
   uint32_t row;         /* R, function constant 0 */
   uint32_t column;      /* C, function constant 1 */
   uint32_t batch_count; /* extension; 0/1 = single head */
+  uint32_t kv_group;    /* extension (appended in 0.5): grouped-query / multi-query attention.  The number of query
+                           problems that share one K/V problem; 0 or 1 = every problem has its own K and V.  Query
+                           problem b (Q, O, L, D, dO, dQ) reads K/V problem b / kv_group; the K, V, dK and dV buffers
+                           hold batch_count / kv_group problems back to back, and dK / dV are the sums over the
+                           kv_group query problems of a group.  For PyTorch [B, Hq, N, D] queries and [B, Hkv, N, D]
+                           keys / values: batch_count = B * Hq, kv_group = Hq / Hkv (the head mapping of
+                           scaled_dot_product_attention(enable_gqa=True)).  batch_count must be a multiple of kv_group
+                           and kv_group at most 16384, else encode / grid_size / launch_count return
+                           MFA_ERROR_INVALID_ARGUMENT.  set_function_constants writes 0 (the descriptor describes no
+                           grouping): set it afterwards.  Not part of any kernel or of the kernel cache's key. */
 } mfa_function_constants_t;
 MFA_API int mfa_attention_descriptor_set_function_constants(const mfa_attention_descriptor_t *descriptor,
                                                             mfa_function_constants_t *constants);
@@ -252,7 +263,8 @@ MFA_API int mfa_attention_kernel_threadgroup_size(const mfa_attention_kernel_t *
 MFA_API int mfa_attention_kernel_threadgroup_memory_allocation(const mfa_attention_kernel_t *kernel,
                                                                uint32_t *out);
 /** Grid size the dispatch uses: ceil(parallelization dimension / blockDimensions.parallelization)
- *  (SquareAttentionTest.swift:328-339) times batch_count. */
+ *  (SquareAttentionTest.swift:328-339) times batch_count (dK/dV: times batch_count / kv_group, one CTA per K/V tile
+ *  walks the query problems of its group). */
 MFA_API int mfa_attention_kernel_grid_size(const mfa_attention_kernel_t *kernel,
                                            const mfa_function_constants_t *constants, uint32_t *out);
 /** Name of the compiled kernel family ("attention_forward_tcgen05<128>" ...) -- stands in for
@@ -275,7 +287,8 @@ MFA_API int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel,
                                         const mfa_function_constants_t *constants,
                                         void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
 
-/** Number of CUDA kernels one encode() launches.  Per slice of at most 16384 problems of the batch: 1; +1 when a small
+/** Number of CUDA kernels one encode() launches.  Per slice of at most 16384 problems of the batch (a multiple of
+ *  kv_group, so that a group never straddles two slices): 1; +1 when a small
  *  grid is split along the traversal axis and a merge kernel follows (split-KV combine for the forward, a plain sum of
  *  partial accumulators for dQ and dK/dV); +1 per operand staged row-major (head % 8 != 0 or stored transposed) and
  *  per output copied back from such a staging buffer; +1 when dK/dV converts a BF16 dO to FP16 in a pass of its own. */
@@ -310,7 +323,8 @@ MFA_API int mfa_attention_kernel_cache_size(void);
  *  ordinal; the caller's current device is restored before the call returns.
  *  With batch_count > 1 the independent problems are processed in chunks that rotate over three
  *  streams, so uploads, kernels and downloads of neighbouring chunks overlap (pass page-locked host
- *  memory to get the overlap; pageable memory still works, serialised by the driver). */
+ *  memory to get the overlap; pageable memory still works, serialised by the driver).
+ *  Every problem has its own K and V here (kv_group = 1): grouped K/V goes through mfa_attention_kernel_encode. */
 MFA_API int mfa_attention_run_host(const mfa_attention_descriptor_t *descriptor, uint32_t run_mask,
                                    void *const host_buffers[MFA_BUFFER_COUNT], int device);
 

@@ -89,7 +89,8 @@ class _CKernelDescriptor(ctypes.Structure):
 
 
 class _CFunctionConstants(ctypes.Structure):
-    _fields_ = [("row", ctypes.c_uint32), ("column", ctypes.c_uint32), ("batch_count", ctypes.c_uint32)]
+    _fields_ = [("row", ctypes.c_uint32), ("column", ctypes.c_uint32), ("batch_count", ctypes.c_uint32),
+                ("kv_group", ctypes.c_uint32)]
 
 
 def _load():
@@ -345,6 +346,19 @@ class FunctionConstantValues:
     @property
     def batchCount(self) -> int:
         return self._c.batch_count
+
+    # ---- library extension: grouped-query / multi-query attention
+    @property
+    def kvGroup(self) -> int:
+        """Query problems per K/V problem (0 or 1: every problem has its own K and V).  Query problem b reads K/V
+        problem b // kvGroup; K, V, dK, dV hold batchCount // kvGroup problems and dK / dV are summed per group.
+        For [B, Hq, N, D] queries and [B, Hkv, N, D] keys: batchCount = B * Hq, kvGroup = Hq // Hkv.
+        setFunctionConstants writes 0; set this afterwards."""
+        return self._c.kv_group
+
+    @kvGroup.setter
+    def kvGroup(self, value: int) -> None:
+        self._c.kv_group = int(value)
 
 
 # -------------------------------------------------------------------------------------------------

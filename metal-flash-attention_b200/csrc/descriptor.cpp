@@ -438,7 +438,7 @@ using namespace mfa;
 extern "C" {
 
 const char *mfa_last_error(void) { return g_last_error.c_str(); }
-const char *mfa_version(void) { return "mfa_b200 0.5 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family)"; }
+const char *mfa_version(void) { return "mfa_b200 0.5 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family, grouped K/V)"; }
 
 int mfa_precision_size(mfa_precision_t precision) { return precision == MFA_FP32 ? 4 : 2; }
 const char *mfa_precision_name(mfa_precision_t precision) {
@@ -564,6 +564,7 @@ int mfa_attention_descriptor_set_function_constants(const mfa_attention_descript
   constants->row = descriptor->row;
   constants->column = descriptor->column;
   constants->batch_count = descriptor->batch_count;
+  constants->kv_group = 0;  // the descriptor describes no K/V grouping; the caller sets it
   return MFA_SUCCESS;
 }
 

@@ -65,17 +65,35 @@ static uint32_t staged_operands(const mfa_attention_kernel *k) {
 
 // Several kernels carry the batch in gridDim.y (limit 65535; the SIMT dK/dV kernel multiplies it by up to four head
 // slices): larger batches go out as several launches over slices of the batch -- the problems are independent and
-// stored back to back, so a slice is just a pointer offset.  Calls f(first problem, problems) per slice and stops at
-// the first status other than MFA_SUCCESS.
+// stored back to back, so a slice is just a pointer offset.  With grouped K/V every slice holds whole groups (its K/V
+// problems start at h0 / group), so a dK/dV CTA still sums over all query problems of its group.  Calls f(first
+// problem, problems) per slice and stops at the first status other than MFA_SUCCESS.
+constexpr uint32_t kMaxBatchPerLaunch = 16384;
 template <class F>
-static int for_each_batch_slice(uint32_t batch, F f) {
-  constexpr uint32_t kMaxBatchPerLaunch = 16384;
-  for (uint32_t h0 = 0; h0 < batch; h0 += kMaxBatchPerLaunch) {
-    const int status = f(h0, batch - h0 < kMaxBatchPerLaunch ? batch - h0 : kMaxBatchPerLaunch);
+static int for_each_batch_slice(uint32_t batch, uint32_t group, F f) {
+  const uint32_t step = kMaxBatchPerLaunch / group * group;
+  for (uint32_t h0 = 0; h0 < batch; h0 += step) {
+    const int status = f(h0, batch - h0 < step ? batch - h0 : step);
     if (status != MFA_SUCCESS) return status;
   }
   return MFA_SUCCESS;
 }
+
+// The query problems per K/V problem of the launch constants (kv_group 0 or 1: every problem has its own K and V)
+static int kv_group_of(const mfa_function_constants_t *c, uint32_t *group) {
+  const uint32_t batch = c->batch_count ? c->batch_count : 1, g = c->kv_group ? c->kv_group : 1;
+  if (g > kMaxBatchPerLaunch)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "kv_group " + std::to_string(g) + " exceeds " +
+                                                std::to_string(kMaxBatchPerLaunch) +
+                                                ", the query problems of one launch slice.");
+  if (batch % g != 0)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "batch_count " + std::to_string(batch) + " is not a multiple of kv_group " +
+                                                std::to_string(g) + ".");
+  *group = g;
+  return MFA_SUCCESS;
+}
+
+static bool key_value_slot(int slot) { return slot == sK || slot == sV || slot == sdK || slot == sdV; }
 
 // sm_90 check of the current device, cached per device ordinal (encode() of a microsecond-scale kernel must not pay
 // two runtime queries per call)
@@ -109,6 +127,8 @@ static int build_params(const mfa_attention_kernel *k, const mfa_function_consta
   p.C = c->column;
   p.D = k->descriptor.head_dimension;
   p.batch = c->batch_count ? c->batch_count : 1;
+  const int status = kv_group_of(c, &p.group);
+  if (status != MFA_SUCCESS) return status;
   for (int s = 0; s < kSlots; ++s) {
     p.buf[s] = buffers[s];
     uint8_t mp = k->descriptor.memory_precisions[s];
@@ -191,7 +211,7 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
                   "descriptor.");
     }
     // (only the geometry fields are used: they depend on neither the problem size nor the device)
-    const WgmmaPlan plan = wgmma_plan(k->type, Dp, 1, 1, 1, 0, 1, false, 1);
+    const WgmmaPlan plan = wgmma_plan(k->type, Dp, 1, 1, 1, 1, 0, 1, false, 1);
     k->threads = plan.threads;
     k->smem_bytes = plan.smem_bytes;
     k->par = plan.par;
@@ -251,9 +271,14 @@ int mfa_attention_kernel_grid_size(const mfa_attention_kernel_t *kernel, const m
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   // parallelization dimension: R for forward / backwardQuery, C for backwardKeyValue
   // (AttentionKernel.swift:197-204; dispatch: SquareAttentionTest.swift:328-339)
-  const uint32_t dim = kernel->type == MFA_BACKWARD_KEY_VALUE ? c->column : c->row;
+  // (dK/dV: one CTA per K/V tile, which walks the query problems of its group)
+  const bool key_value = kernel->type == MFA_BACKWARD_KEY_VALUE;
+  const uint32_t dim = key_value ? c->column : c->row;
   const uint32_t batch = c->batch_count ? c->batch_count : 1;
-  *out = ((dim + kernel->par - 1) / kernel->par) * batch;
+  uint32_t group = 1;
+  const int status = kv_group_of(c, &group);
+  if (status != MFA_SUCCESS) return status;
+  *out = ((dim + kernel->par - 1) / kernel->par) * (key_value ? batch / group : batch);
   return MFA_SUCCESS;
 }
 
@@ -266,13 +291,16 @@ int mfa_attention_kernel_launch_count(const mfa_attention_kernel_t *kernel, cons
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
   const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, staged = __builtin_popcount(staged_operands(kernel));
+  uint32_t group = 1;
+  const int status = kv_group_of(c, &group);
+  if (status != MFA_SUCCESS) return status;
   const uint32_t sm_count = kernel->backend == MFA_BACKEND_TCGEN05 ? device_sm_count(current_device()) : 0;
   *out = 0;
-  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, [&](uint32_t, uint32_t batch) -> int {
+  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t, uint32_t batch) -> int {
     *out += kernel->backend != MFA_BACKEND_TCGEN05
                 ? 1
-                : staged + wgmma_plan(kernel->type, Dp, c->row, c->column, batch, d.split_min_blocks, d.split_max,
-                                      d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q], sm_count)
+                : staged + wgmma_plan(kernel->type, Dp, c->row, c->column, batch, group, d.split_min_blocks,
+                                      d.split_max, d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q], sm_count)
                                .launches;
     return MFA_SUCCESS;
   });
@@ -293,24 +321,28 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
   // are copied back to the caller's layout without the padding.
   size_t head_bytes[kSlots];
   for (int slot = 0; slot < kSlots; ++slot) {
-    const size_t seq = (slot == sK || slot == sV || slot == sdK || slot == sdV) ? p.C : p.R;
+    const size_t seq = key_value_slot(slot) ? p.C : p.R;
     const size_t elements = (slot == sL || slot == sD) ? seq : seq * p.D;
     head_bytes[slot] = elements * (p.prec[slot] == FP32 ? 4 : 2);
   }
   const uint32_t staged = staged_operands(kernel);
   const uint32_t Dp = (p.D + 7) / 8 * 8;
   const int device = staged ? current_device() : 0;
-  auto seq_of = [&](int slot) -> uint32_t { return (slot == sK || slot == sV || slot == sdK || slot == sdV) ? p.C : p.R; };
-  return for_each_batch_slice(p.batch, [&](uint32_t h0, uint32_t batch) -> int {
+  auto seq_of = [&](int slot) -> uint32_t { return key_value_slot(slot) ? p.C : p.R; };
+  return for_each_batch_slice(p.batch, p.group, [&](uint32_t h0, uint32_t batch) -> int {
     AttentionParams q = p;
     q.batch = batch;
+    // the problems of a slot in this slice: K, V, dK and dV hold one per group
+    auto problems_of = [&](int slot) -> uint32_t { return key_value_slot(slot) ? batch / p.group : batch; };
     for (int slot = 0; slot < kSlots; ++slot)
-      if (q.buf[slot]) q.buf[slot] = static_cast<char *>(q.buf[slot]) + head_bytes[slot] * h0;
+      if (q.buf[slot])
+        q.buf[slot] = static_cast<char *>(q.buf[slot]) + head_bytes[slot] * (key_value_slot(slot) ? h0 / p.group : h0);
     cudaError_t e = cudaSuccess;
     void *user_out[kSlots] = {};  // staged outputs: where the caller's copies go
     if (staged) {
       auto bytes_of = [&](int slot) -> size_t {
-        return ((static_cast<size_t>(q.batch) * seq_of(slot) * Dp * (p.prec[slot] == FP32 ? 4 : 2)) + 255) & ~size_t(255);
+        return ((static_cast<size_t>(problems_of(slot)) * seq_of(slot) * Dp * (p.prec[slot] == FP32 ? 4 : 2)) + 255) &
+               ~size_t(255);
       };
       size_t total = 0;
       for (int slot = 0; slot < kSlots; ++slot)
@@ -324,8 +356,8 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
         if (is_output(kernel->type, slot))
           user_out[slot] = q.buf[slot];
         else
-          e = launch_stage_operand(q.buf[slot], cursor, q.batch, seq_of(slot), p.D, Dp, p.prec[slot] == FP32 ? 4 : 2,
-                                   q.transposed[slot], stream);
+          e = launch_stage_operand(q.buf[slot], cursor, problems_of(slot), seq_of(slot), p.D, Dp,
+                                   p.prec[slot] == FP32 ? 4 : 2, q.transposed[slot], stream);
         q.buf[slot] = cursor;
         cursor += bytes_of(slot);
       }
@@ -351,8 +383,8 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
                                       " " + last_launch_detail());
     for (int slot = 0; slot < kSlots && e == cudaSuccess; ++slot)
       if (user_out[slot])
-        e = launch_unstage_output(static_cast<const float *>(q.buf[slot]), static_cast<float *>(user_out[slot]), q.batch,
-                                  seq_of(slot), p.D, Dp, p.transposed[slot], stream);
+        e = launch_unstage_output(static_cast<const float *>(q.buf[slot]), static_cast<float *>(user_out[slot]),
+                                  problems_of(slot), seq_of(slot), p.D, Dp, p.transposed[slot], stream);
     if (e != cudaSuccess) return fail(MFA_ERROR_CUDA, std::string("copy-back of staged outputs failed: ") + cudaGetErrorString(e));
     return MFA_SUCCESS;
   });

@@ -18,6 +18,9 @@ struct AttentionParams {
   uint32_t C;      // columns (input sequence length)
   uint32_t D;      // head dimension
   uint32_t batch;  // independent single-head problems, >= 1
+  // query problems per K/V problem (>= 1, divides batch): query problem b reads K / V problem b / group, and the K, V,
+  // dK, dV buffers hold batch / group problems (dK / dV summed over each group)
+  uint32_t group;
   void *buf[kSlots];        // device pointers, by slot
   uint8_t prec[kSlots];     // memory precision, by slot
   uint8_t transposed[kSlots];  // 1: stored [D][seq] (leading dim = seq), 0: [seq][D]
@@ -50,12 +53,14 @@ cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream
 struct WgmmaPlan {
   uint32_t threads, smem_bytes;        // per CTA
   uint32_t par, trav, head;            // blockDimensions: rows per CTA, rows per pipeline stage, head block
-  dim3 grid;                           // (tiles, batch, splits)
+  dim3 grid;                           // (tiles, batch, splits); dK/dV: (tiles, batch / group, splits)
   uint32_t blocks_per_split, splits;   // traversal blocks per CTA; ranges of the traversal axis (1 = not split)
   bool convert_dO_first;               // dK/dV: the BF16 dO is converted to FP16 in a pass of its own
   uint32_t launches;                   // kernels the launcher issues
 };
-WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t min_blocks,
+// batch = query problems, group = query problems per K/V problem (only the dK/dV plan, whose CTAs own K/V tiles,
+// depends on it)
+WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
                      uint32_t max_splits, bool convert_dO, uint32_t sm_count);
 
 // operand staging for the tensor-core family (pad_head.cu): a [batch][seq][D] (or, transposed, [batch][D][seq]) operand

@@ -15,6 +15,8 @@
 // D stored pre-scaled by 1/sqrt(D), BF16 stores truncate, edge columns masked before softmax.
 // Causal (p.causal): row r sees column c iff c <= r + p.causal_offset; the loops skip the 64-blocks no row of the CTA
 // can see, the mask is applied with the edge mask, and a row that sees no column gets O = 0, L = +inf.
+// Grouped K/V (p.group query problems per K/V problem): query problem b reads K / V problem b / p.group, and a dK/dV
+// CTA sums over the rows of every query problem of its group.
 //
 // Tiling: one CTA = 256 threads = a 64 x 64 block of the attention matrix; thread (tx, ty) owns
 // the 4 x 4 patch {rows ty+16i} x {cols tx+16j}.  Operands are staged through shared memory as
@@ -233,7 +235,8 @@ __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const Attenti
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
 
-  const Operand Q = make_operand(p, sQ, p.R, b), K = make_operand(p, sK, p.C, b), V = make_operand(p, sV, p.C, b);
+  const Operand Q = make_operand(p, sQ, p.R, b), K = make_operand(p, sK, p.C, b / p.group),
+                V = make_operand(p, sV, p.C, b / p.group);
 
   // m = -FLT_MAX, l = denorm_min  (AttentionKernel+Caching.swift:310-311)
   float m[4], l[4];
@@ -320,7 +323,8 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const 
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
 
-  const Operand Q = make_operand(p, sQ, p.R, b), K = make_operand(p, sK, p.C, b), V = make_operand(p, sV, p.C, b);
+  const Operand Q = make_operand(p, sQ, p.R, b), K = make_operand(p, sK, p.C, b / p.group),
+                V = make_operand(p, sV, p.C, b / p.group);
   const Operand O = make_operand(p, sO, p.R, b), dO = make_operand(p, sdO, p.R, b);
   const char *Lbase = static_cast<const char *>(p.buf[sL]) + static_cast<size_t>(b) * p.R * (p.prec[sL] == FP32 ? 4 : 2);
   char *Dbase = static_cast<char *>(p.buf[sD]) + static_cast<size_t>(b) * p.R * (p.prec[sD] == FP32 ? 4 : 2);
@@ -372,6 +376,7 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const 
 
 // ------------------------------------------------------------------------------------------------
 // backward dK/dV: dV = sum_r P^T dO;  dK = sum_r dS^T Q      (one CTA per 64 columns x D-slice)
+// Grouped K/V: blockIdx.y covers K/V heads, and the sums run over the rows of every query head of the group.
 // ------------------------------------------------------------------------------------------------
 template <int NCH>
 __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(const AttentionParams p,
@@ -379,14 +384,11 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(co
   extern __shared__ __align__(16) float smem[];
   float *sA = smem, *sB = sA + kBlock * kLDA, *sPT = sB + kBlock * kLDA, *sX = sPT + kBlock * kLDP;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const uint32_t b = blockIdx.y / dSlices, slice = blockIdx.y % dSlices, c0 = blockIdx.x * kBlock;
+  const uint32_t kvb = blockIdx.y / dSlices, slice = blockIdx.y % dSlices, c0 = blockIdx.x * kBlock;
   const uint32_t dlo = slice * (NCH * kBlock);
   const uint32_t dhi = min(p.D, dlo + NCH * kBlock);
 
-  const Operand Q = make_operand(p, sQ, p.R, b), K = make_operand(p, sK, p.C, b), V = make_operand(p, sV, p.C, b);
-  const Operand dO = make_operand(p, sdO, p.R, b);
-  const char *Lbase = static_cast<const char *>(p.buf[sL]) + static_cast<size_t>(b) * p.R * (p.prec[sL] == FP32 ? 4 : 2);
-  const char *Dbase = static_cast<const char *>(p.buf[sD]) + static_cast<size_t>(b) * p.R * (p.prec[sD] == FP32 ? 4 : 2);
+  const Operand K = make_operand(p, sK, p.C, kvb), V = make_operand(p, sV, p.C, kvb);
 
   float accV[NCH][4][4], accK[NCH][4][4];
 #pragma unroll
@@ -399,43 +401,50 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(co
   // causal: start at the 64-block holding the first row that sees column c0 (r >= c0 - offset)
   const int first = static_cast<int>(c0) - p.causal_offset;
   const uint32_t rstart = p.causal && first > 0 ? static_cast<uint32_t>(first) / kBlock * kBlock : 0;
-  for (uint32_t r0 = rstart; r0 < p.R; r0 += kBlock) {
-    float s[4][4], dp[4][4];
+  for (uint32_t b = kvb * p.group; b < (kvb + 1) * p.group; ++b) {  // the query heads of the group
+    const Operand Q = make_operand(p, sQ, p.R, b), dO = make_operand(p, sdO, p.R, b);
+    const char *Lbase =
+        static_cast<const char *>(p.buf[sL]) + static_cast<size_t>(b) * p.R * (p.prec[sL] == FP32 ? 4 : 2);
+    const char *Dbase =
+        static_cast<const char *>(p.buf[sD]) + static_cast<size_t>(b) * p.R * (p.prec[sD] == FP32 ? 4 : 2);
+    for (uint32_t r0 = rstart; r0 < p.R; r0 += kBlock) {
+      float s[4][4], dp[4][4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
+      for (int i = 0; i < 4; ++i)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);    // S[r][c]
-    gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);  // dP[r][c]
+        for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
+      gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);    // S[r][c]
+      gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);  // dP[r][c]
 
-    float pv[4][4];
+      float pv[4][4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      uint32_t r = r0 + ty + 16 * i;
-      uint32_t rc = min(r, p.R - 1);
-      // L and D are read back in their memory precision (+Softmax.swift:356-404, 453-468)
-      float Lr = load_elem(Lbase, rc, p.prec[sL]);
-      float Dr = load_elem(Dbase, rc, p.prec[sD]);
+      for (int i = 0; i < 4; ++i) {
+        uint32_t r = r0 + ty + 16 * i;
+        uint32_t rc = min(r, p.R - 1);
+        // L and D are read back in their memory precision (+Softmax.swift:356-404, 453-468)
+        float Lr = load_elem(Lbase, rc, p.prec[sL]);
+        float Dr = load_elem(Dbase, rc, p.prec[sD]);
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float e = (r < p.R && !(p.causal && static_cast<int>(c0 + tx + 16 * j) > static_cast<int>(r) + p.causal_offset))
-                      ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr))
-                      : 0.f;
-        pv[i][j] = e;
-        dp[i][j] = e * fmaf(dp[i][j], p.scale, -Dr);  // dS
-        sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = e;  // P^T
+        for (int j = 0; j < 4; ++j) {
+          float e = (r < p.R && !(p.causal && static_cast<int>(c0 + tx + 16 * j) > static_cast<int>(r) + p.causal_offset))
+                        ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr))
+                        : 0.f;
+          pv[i][j] = e;
+          dp[i][j] = e * fmaf(dp[i][j], p.scale, -Dr);  // dS
+          sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = e;  // P^T
+        }
       }
+      accumulate<NCH>(accV, sPT, dO, r0, dlo, dhi, sX, tid, tx, ty);  // dV += P^T dO
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = dp[i][j];  // dS^T
+      accumulate<NCH>(accK, sPT, Q, r0, dlo, dhi, sX, tid, tx, ty);  // dK += dS^T Q
     }
-    accumulate<NCH>(accV, sPT, dO, r0, dlo, dhi, sX, tid, tx, ty);  // dV += P^T dO
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = dp[i][j];  // dS^T
-    accumulate<NCH>(accK, sPT, Q, r0, dlo, dhi, sX, tid, tx, ty);  // dK += dS^T Q
   }
   const float one[4] = {1.f, 1.f, 1.f, 1.f};
-  store_acc<NCH>(accV, one, p, sdV, p.C, b, c0, dlo, dhi, tx, ty);
-  store_acc<NCH>(accK, one, p, sdK, p.C, b, c0, dlo, dhi, tx, ty);
+  store_acc<NCH>(accV, one, p, sdV, p.C, kvb, c0, dlo, dhi, tx, ty);
+  store_acc<NCH>(accK, one, p, sdK, p.C, kvb, c0, dlo, dhi, tx, ty);
 }
 
 template <typename KernelT>
@@ -487,7 +496,7 @@ cudaError_t launch_simt_backward_key_value(const AttentionParams &p, cudaStream_
   int chunks = simt::chunks_for(p.D);
   int nch = chunks <= 1 ? 1 : chunks <= 2 ? 2 : 4;
   uint32_t dSlices = (chunks + nch - 1) / nch;
-  dim3 grid((p.C + simt::kBlock - 1) / simt::kBlock, p.batch * dSlices);
+  dim3 grid((p.C + simt::kBlock - 1) / simt::kBlock, p.batch / p.group * dSlices);  // one CTA row per K/V head
   cudaError_t e;
   if (nch == 1) {
     if ((e = simt::prepare(simt::simt_backward_key_value_kernel<1>)) != cudaSuccess) return e;

@@ -19,6 +19,10 @@
 // Causal (kCausal, bottom-right aligned: query row i sees key j iff j <= i + delta, delta = C - R): every CTA visits only
 // the traversal blocks its rows can see, and only the blocks that cross the diagonal mask elements (S -> -inf before the
 // softmax / before P = exp2(S - L)).  A row that sees no key (i < R - C) gets O = 0, L = +inf, D = 0, dQ = 0.
+//
+// Grouped K/V (`group` query heads per K/V head, a launch-time value): forward and dQ read K/V head head / group; the
+// dK/dV grid's y axis is K/V heads, and a CTA walks the query blocks of every query head of its group, so dK and dV
+// are the group sums, accumulated in registers without atomics.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -183,7 +187,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     attention_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                             const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
                             uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp,
-                            int delta) {
+                            int delta, uint32_t group) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -193,6 +197,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   // (causal: unlike dQ, the forward gains nothing measurable from starting the tiles with the most key blocks first)
   const uint32_t head = blockIdx.y, row_base = blockIdx.x * Cfg::kTileM;
+  const uint32_t kv_head = head / group;  // grouped K/V: the query heads of a group read one K/V head
   // this CTA's key blocks: [kb0, kb0 + blocks)
   const uint32_t kb0 = blockIdx.z * sp.blocks_per_split;
   const uint32_t blocks = kCausal ? visible_key_blocks<BN>(row_base, Cfg::kTileM, R, C, delta, kb0, sp.blocks_per_split)
@@ -201,8 +206,8 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   auto load_kv = [&](uint32_t j, uint32_t s) {
     uint8_t *dst = kv + s * 2 * Cfg::kKVBytes;
     mbar_arrive_expect_tx(&bar[1 + s], 2 * Cfg::kKVBytes);
-    load_tile<DCH, BN>(dst, &mapK, &bar[1 + s], (kb0 + j) * BN, head);
-    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, &bar[1 + s], (kb0 + j) * BN, head);
+    load_tile<DCH, BN>(dst, &mapK, &bar[1 + s], (kb0 + j) * BN, kv_head);
+    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, &bar[1 + s], (kb0 + j) * BN, kv_head);
   };
   if (tid == 0) {
     prefetch_tensormap(&mapQ);
@@ -350,6 +355,7 @@ struct BwdArgs {
   float scale, scale_log2;
   int l_prec, d_prec, dO_bf16;
   int delta;  // causal kernels: query row i sees key j iff j <= i + delta
+  uint32_t group;  // query heads per K/V head: query head h reads K/V head h / group
 };
 
 template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
@@ -366,7 +372,7 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   // causal: tiles in reverse order, so that the ones with the most key blocks start first and the wave tail is short
   const uint32_t tile = kCausal ? gridDim.x - 1 - blockIdx.x : blockIdx.x;
-  const uint32_t head = blockIdx.y, row_base = tile * Cfg::kTileM;
+  const uint32_t head = blockIdx.y, row_base = tile * Cfg::kTileM, kv_head = head / a.group;
   const uint32_t kb0 = blockIdx.z * a.blocks_per_split;
   const uint32_t blocks = kCausal ? visible_key_blocks<BN>(row_base, Cfg::kTileM, a.R, a.C, a.delta, kb0, a.blocks_per_split)
                                   : min((a.C + BN - 1) / BN - kb0, a.blocks_per_split);
@@ -374,8 +380,8 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   auto load_kv = [&](uint32_t j, uint32_t s) {
     uint8_t *dst = kv + s * 2 * Cfg::kKVBytes;
     mbar_arrive_expect_tx(&bar[1 + s], 2 * Cfg::kKVBytes);
-    load_tile<DCH, BN>(dst, &mapK, &bar[1 + s], (kb0 + j) * BN, head);
-    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, &bar[1 + s], (kb0 + j) * BN, head);
+    load_tile<DCH, BN>(dst, &mapK, &bar[1 + s], (kb0 + j) * BN, kv_head);
+    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, &bar[1 + s], (kb0 + j) * BN, kv_head);
   };
   if (tid == 0) {
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
@@ -509,18 +515,23 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   uint8_t *qd = base + 2 * Cfg::kKBytes;  // stage s: Q at qd + 2 s kQBytes, dO right after it
   uint64_t *bar = reinterpret_cast<uint64_t *>(qd + 4 * Cfg::kQBytes);
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
-  const uint32_t head = blockIdx.y, key_base = blockIdx.x * Cfg::kTileN;
+  // grouped K/V: blockIdx.y is a K/V head, and the CTA walks the query blocks of every query head of its group
+  const uint32_t kv_head = blockIdx.y, key_base = blockIdx.x * Cfg::kTileN;
   const uint32_t qb0 = blockIdx.z * a.blocks_per_split;
   // causal: this CTA's query blocks start at the first one that sees the tile's first key (query >= key_base - delta)
   const uint32_t qs = kCausal ? max(qb0, first_query_block<BM>(key_base, a.delta)) : qb0;
   const uint32_t blocks = kCausal ? visible_query_blocks<BM>(a.R, qb0, qs, a.blocks_per_split)
                                   : min((a.R + BM - 1) / BM - qb0, a.blocks_per_split);
+  // the same query blocks [qs, qs + blocks) of each of the group's query heads, as one flattened sequence n = g blocks
+  // + i that drives the Q / dO ring: prefetch and barrier parity carry across head boundaries
+  const uint32_t total = a.group * blocks;
 
-  auto load_qd = [&](uint32_t i, uint32_t s) {
+  auto load_qd = [&](uint32_t n, uint32_t s) {
+    const uint32_t g = n / blocks, i = n - g * blocks;
     uint8_t *dst = qd + s * 2 * Cfg::kQBytes;
     mbar_arrive_expect_tx(&bar[1 + s], 2 * Cfg::kQBytes);
-    load_tile<DCH, BM>(dst, &mapQ, &bar[1 + s], (qs + i) * BM, head);
-    load_tile<DCH, BM>(dst + Cfg::kQBytes, &mapdO, &bar[1 + s], (qs + i) * BM, head);
+    load_tile<DCH, BM>(dst, &mapQ, &bar[1 + s], (qs + i) * BM, kv_head * a.group + g);
+    load_tile<DCH, BM>(dst + Cfg::kQBytes, &mapdO, &bar[1 + s], (qs + i) * BM, kv_head * a.group + g);
   };
   if (tid == 0) {
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
@@ -529,20 +540,20 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   __syncthreads();
   if (tid == 0) {
     mbar_arrive_expect_tx(&bar[0], 2 * Cfg::kKBytes);
-    load_tile<DCH, Cfg::kTileN>(base, &mapK, &bar[0], key_base, head);
-    load_tile<DCH, Cfg::kTileN>(base + Cfg::kKBytes, &mapV, &bar[0], key_base, head);
-    for (uint32_t s = 0; s < 2 && s < blocks; ++s) load_qd(s, s);
+    load_tile<DCH, Cfg::kTileN>(base, &mapK, &bar[0], key_base, kv_head);
+    load_tile<DCH, Cfg::kTileN>(base + Cfg::kKBytes, &mapV, &bar[0], key_base, kv_head);
+    for (uint32_t s = 0; s < 2 && s < total; ++s) load_qd(s, s);
   }
   const uint32_t sK = smem_u32(base), sV = sK + Cfg::kKBytes;
   const uint32_t krow = Cfg::kSplitD ? 0 : wg * kRows;      // this warpgroup's key rows inside the tile
   const uint32_t nchunk = Cfg::kSplitD ? wg * (NA / 64) : 0;  // ... and its first accumulator column chunk
-  const size_t hb = static_cast<size_t>(head) * a.R;
+  size_t hb = static_cast<size_t>(kv_head) * a.group * a.R;  // L / D rows of the current query head
   float dv[NA / 2], dk[NA / 2];
   zero(dv);
   zero(dk);
   mbar_wait(&bar[0], 0);
-  for (uint32_t i = 0; i < blocks; ++i) {
-    const uint32_t s = i & 1;
+  for (uint32_t n = 0, i = 0; n < total; ++n) {
+    const uint32_t s = n & 1;
     // per-query statistics of this thread's 16 columns, loaded while the tiles land
     float Lq[BM / 4], Dq[BM / 4];
     const uint32_t q0 = (qs + i) * BM + 2 * (t % 4);
@@ -554,7 +565,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
         Lq[2 * j + e] = load_stat(a.L, hb + q, a.l_prec);
         Dq[2 * j + e] = load_stat(a.Dterm, hb + q, a.d_prec);
       }
-    mbar_wait(&bar[1 + s], (i >> 1) & 1);
+    mbar_wait(&bar[1 + s], (n >> 1) & 1);
     if constexpr (kConvertDO) {
       // BF16 dO beside FP16 Q/K/V on a small grid: the streamed dO tile is rewritten as FP16 in place (a grid of more
       // than one wave converts dO once, in a pass of its own, instead)
@@ -615,9 +626,13 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     fence_regs(dv);
     fence_regs(dk);
     __syncthreads();
-    if (tid == 0 && i + 2 < blocks) load_qd(i + 2, s);
+    if (tid == 0 && n + 2 < total) load_qd(n + 2, s);
+    if (++i == blocks) {  // the next query head of the group; dK and dV keep accumulating
+      i = 0;
+      hb += a.R;
+    }
   }
-  const size_t kb = static_cast<size_t>(head) * a.C * a.D;
+  const size_t kb = static_cast<size_t>(kv_head) * a.C * a.D;
   const uint32_t row0 = key_base + krow, col0 = nchunk * 64;
   store_acc(dv, a.dV + blockIdx.z * a.split_stride + kb, row0, a.C, col0, a.D, 1.f, 1.f);
   store_acc(dk, a.dK + blockIdx.z * a.split_stride + kb, row0, a.C, col0, a.D, 1.f, 1.f);
@@ -697,8 +712,8 @@ cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cuda
   if ((e = prepare(kernel, Cfg::kSmemBytes)) != cudaSuccess) return e;
   CUtensorMap mapQ, mapK, mapV;
   if ((e = make_tensor_map_16bit(&mapQ, p.buf[sQ], p.R, p.D, p.batch, Cfg::kTileM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch, Cfg::BN)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch, Cfg::BN)) != cudaSuccess) return e;
+  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) return e;
+  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) return e;
   SplitArgs sp{plan.blocks_per_split, plan.splits, p.batch, nullptr, nullptr};
   const uint64_t rows_total = static_cast<uint64_t>(p.batch) * p.R;
   if (plan.splits > 1) {
@@ -712,7 +727,7 @@ cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cuda
   }
   kernel<<<plan.grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapK, mapV, static_cast<float *>(p.buf[sO]),
                                                                 p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp,
-                                                                p.causal_offset);
+                                                                p.causal_offset, p.group);
   if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
   const uint64_t threads = rows_total * (p.D / 4);
   merge_splits<kCausal><<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(
@@ -759,6 +774,7 @@ static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
   a.d_prec = p.prec[sD];
   a.dO_bf16 = p.prec[sdO] == BF16;
   a.delta = p.causal_offset;
+  a.group = p.group;
   return a;
 }
 
@@ -771,8 +787,8 @@ cudaError_t launch_query(const AttentionParams &p, const WgmmaPlan &plan, cudaSt
   CUtensorMap mapQ, mapdO, mapK, mapV;
   if ((e = make_tensor_map_16bit(&mapQ, p.buf[sQ], p.R, p.D, p.batch, Cfg::kTileM)) != cudaSuccess) return e;
   if ((e = make_tensor_map_16bit(&mapdO, p.buf[sdO], p.R, p.D, p.batch, Cfg::kTileM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch, Cfg::BN)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch, Cfg::BN)) != cudaSuccess) return e;
+  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) return e;
+  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) return e;
   BwdArgs a = backward_args(p, plan);
   const size_t tensor_elems = static_cast<size_t>(p.batch) * p.R * p.D;
   float *scratch = nullptr;
@@ -795,10 +811,10 @@ cudaError_t launch_key_value(const AttentionParams &p, const WgmmaPlan &plan, cu
   CUtensorMap mapQ, mapdO, mapK, mapV;
   if ((e = make_tensor_map_16bit(&mapQ, p.buf[sQ], p.R, p.D, p.batch, Cfg::BM)) != cudaSuccess) return e;
   if ((e = make_tensor_map_16bit(&mapdO, p.buf[sdO], p.R, p.D, p.batch, Cfg::BM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch, Cfg::kTileN)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch, Cfg::kTileN)) != cudaSuccess) return e;
+  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch / p.group, Cfg::kTileN)) != cudaSuccess) return e;
+  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch / p.group, Cfg::kTileN)) != cudaSuccess) return e;
   BwdArgs a = backward_args(p, plan);
-  const size_t tensor_elems = static_cast<size_t>(p.batch) * p.C * p.D;
+  const size_t tensor_elems = static_cast<size_t>(p.batch / p.group) * p.C * p.D;  // dK / dV: one per K/V head
   float *scratch = nullptr;
   if (plan.splits > 1) {
     if ((e = split_scratch(a, plan.splits, 2, tensor_elems, stream, &scratch)) != cudaSuccess) return e;
@@ -826,7 +842,7 @@ static cudaError_t dispatch(const AttentionParams &p, bool convert_dO, F f) {
 
 }  // namespace hop
 
-WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t min_blocks,
+WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
                      uint32_t max_splits, bool convert_dO, uint32_t sm_count) {
   WgmmaPlan p{};
   auto geometry = [&](auto cfg) {
@@ -850,17 +866,20 @@ WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batc
 
   const bool key_value = type == MFA_BACKWARD_KEY_VALUE;
   const uint32_t tiles = ((key_value ? C : R) + p.par - 1) / p.par, total = ((key_value ? R : C) + p.trav - 1) / p.trav;
+  // CTAs per tile row: one per query head, or for dK/dV one per K/V head (it walks the query heads of its group; the
+  // split cuts each head's query blocks the same way)
+  const uint32_t heads = key_value ? batch / group : batch;
   if (type == MFA_FORWARD) {
-    p.splits = hop::choose_splits(tiles * batch, total, sm_count, min_blocks, max_splits);
+    p.splits = hop::choose_splits(tiles * heads, total, sm_count, min_blocks, max_splits);
     p.blocks_per_split = total / p.splits;
   } else {
-    p.blocks_per_split = hop::choose_blocks_per_split(tiles * batch, total, sm_count, min_blocks, max_splits);
+    p.blocks_per_split = hop::choose_blocks_per_split(tiles * heads, total, sm_count, min_blocks, max_splits);
     p.splits = (total + p.blocks_per_split - 1) / p.blocks_per_split;
   }
-  p.grid = dim3(tiles, batch, p.splits);
+  p.grid = dim3(tiles, heads, p.splits);
   // dK/dV with BF16 dO beside FP16 Q/K/V: a grid of more than one wave converts dO once, in a pass of its own (a
   // smaller one converts each streamed dO tile in shared memory)
-  p.convert_dO_first = key_value && convert_dO && static_cast<uint64_t>(tiles) * batch > sm_count;
+  p.convert_dO_first = key_value && convert_dO && static_cast<uint64_t>(tiles) * heads > sm_count;
   // the kernel, + merge_splits / sum_splits when split, + the dO conversion pass
   p.launches = 1 + (p.splits > 1 ? 1 : 0) + (p.convert_dO_first ? 1 : 0);
   return p;
@@ -874,7 +893,7 @@ static bool row_major_16bit(const AttentionParams &p) {
 }
 
 static WgmmaPlan plan_for(int type, const AttentionParams &p, bool convert_dO) {
-  return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.split_min_blocks, p.split_max, convert_dO,
+  return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, convert_dO,
                     device_sm_count(current_device()));
 }
 

@@ -27,6 +27,11 @@ inline void check(int status) {
   if (status != MFA_SUCCESS) throw std::runtime_error(mfa_last_error());
 }
 
+// library extension: grouped-query / multi-query attention, a launch-time constant like R, C and the batch.  The query
+// problems per K/V problem (0 or 1: none shared); query problem b reads K/V problem b / kvGroup, and dK / dV are summed
+// per group.  AttentionDescriptor::setFunctionConstants writes 0: set it afterwards, kvGroup(constants) = Hq / Hkv.
+inline uint32_t &kvGroup(mfa_function_constants_t &constants) { return constants.kv_group; }
+
 struct MatrixDimensions { uint32_t row, column; uint16_t head; };
 struct TransposeState { bool Q, K, V, O; };
 

@@ -110,7 +110,7 @@ public struct AttentionDescriptor {
     return output
   }
 
-  /// AttentionDescriptor.swift:139-148 (R at index 0, C at index 1).
+  /// AttentionDescriptor.swift:139-148 (R at index 0, C at index 1).  Writes kvGroup = 0 (no grouping).
   public func setFunctionConstants(_ constants: inout mfa_function_constants_t) {
     var descriptor = c
     check(mfa_attention_descriptor_set_function_constants(&descriptor, &constants))
@@ -381,5 +381,15 @@ public final class AttentionKernel {
     }
     var constants = constants
     check(mfa_attention_kernel_encode(handle, &constants, &table, stream))
+  }
+}
+
+/// library extension: grouped-query / multi-query attention, a launch-time constant like R, C and the batch.  The
+/// query problems per K/V problem (0 or 1: none shared); query problem b reads K/V problem b / kvGroup, and dK / dV
+/// are summed per group.  `setFunctionConstants` writes 0: set it afterwards (Hq / Hkv).
+extension mfa_function_constants_t {
+  public var kvGroup: UInt32 {
+    get { kv_group }
+    set { kv_group = newValue }
   }
 }
