@@ -27,7 +27,10 @@
 #include <float.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "attention_params.h"
+#include "device_state.h"
 
 namespace mfa {
 namespace simt {
@@ -205,6 +208,11 @@ __device__ __forceinline__ Operand make_operand(const AttentionParams &p, int sl
   return op;
 }
 
+// the R statistics (L or D) of problem b in `slot`
+__device__ __forceinline__ char *stat_row(const AttentionParams &p, int slot, uint32_t b) {
+  return static_cast<char *>(p.buf[slot]) + static_cast<size_t>(b) * p.R * (p.prec[slot] == FP32 ? 4 : 2);
+}
+
 // store a [64 x (NCH*64)] register accumulator block to a matrix operand (FP32/FP16/BF16, maybe transposed)
 template <int NCH>
 __device__ __forceinline__ void store_acc(const float (&acc)[NCH][4][4], const float (&rowScale)[4],
@@ -304,7 +312,7 @@ __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const Attenti
   }
   store_acc<NCH>(acc, inv, p, sO, p.R, b, r0, 0, p.D, tx, ty);
   if (tx == 0 && p.buf[sL] != nullptr) {
-    char *Lbase = static_cast<char *>(p.buf[sL]) + static_cast<size_t>(b) * p.R * (p.prec[sL] == FP32 ? 4 : 2);
+    char *Lbase = stat_row(p, sL, b);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       uint32_t r = r0 + ty + 16 * i;
@@ -326,8 +334,8 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const 
   const Operand Q = make_operand(p, sQ, p.R, b), K = make_operand(p, sK, p.C, b / p.group),
                 V = make_operand(p, sV, p.C, b / p.group);
   const Operand O = make_operand(p, sO, p.R, b), dO = make_operand(p, sdO, p.R, b);
-  const char *Lbase = static_cast<const char *>(p.buf[sL]) + static_cast<size_t>(b) * p.R * (p.prec[sL] == FP32 ? 4 : 2);
-  char *Dbase = static_cast<char *>(p.buf[sD]) + static_cast<size_t>(b) * p.R * (p.prec[sD] == FP32 ? 4 : 2);
+  const char *Lbase = stat_row(p, sL, b);
+  char *Dbase = stat_row(p, sD, b);
 
   // computeD (AttentionKernel+Softmax.swift:32-221): D = (sum_d dO * O) * 1/sqrt(D), kept in FP32
   // registers for this kernel and stored (possibly as BF16) for the dK/dV kernel.
@@ -403,10 +411,7 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(co
   const uint32_t rstart = p.causal && first > 0 ? static_cast<uint32_t>(first) / kBlock * kBlock : 0;
   for (uint32_t b = kvb * p.group; b < (kvb + 1) * p.group; ++b) {  // the query heads of the group
     const Operand Q = make_operand(p, sQ, p.R, b), dO = make_operand(p, sdO, p.R, b);
-    const char *Lbase =
-        static_cast<const char *>(p.buf[sL]) + static_cast<size_t>(b) * p.R * (p.prec[sL] == FP32 ? 4 : 2);
-    const char *Dbase =
-        static_cast<const char *>(p.buf[sD]) + static_cast<size_t>(b) * p.R * (p.prec[sD] == FP32 ? 4 : 2);
+    const char *Lbase = stat_row(p, sL, b), *Dbase = stat_row(p, sD, b);
     for (uint32_t r0 = rstart; r0 < p.R; r0 += kBlock) {
       float s[4][4], dp[4][4];
 #pragma unroll
@@ -447,68 +452,58 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(co
   store_acc<NCH>(accK, one, p, sdK, p.C, kvb, c0, dlo, dhi, tx, ty);
 }
 
-template <typename KernelT>
-cudaError_t prepare(KernelT kernel) {
-  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+inline int chunks_for(uint32_t D) { return (D + kBlock - 1) / kBlock; }
+
+// Calls f(std::integral_constant<int, NCH>()) for the fewest of 1 / 2 / 4 / 8 (at most kMax) column chunks per CTA
+// that cover `chunks`
+template <int kMax, class F>
+cudaError_t with_chunks(int chunks, F f) {
+  static_assert(kMax == 4 || kMax == 8, "the kernels are instantiated for 1 / 2 / 4 / 8 chunks");
+  if (chunks <= 1) return f(std::integral_constant<int, 1>());
+  if (chunks <= 2) return f(std::integral_constant<int, 2>());
+  if constexpr (kMax == 4) {
+    return f(std::integral_constant<int, 4>());
+  } else {
+    if (chunks <= 4) return f(std::integral_constant<int, 4>());
+    return f(std::integral_constant<int, 8>());
+  }
 }
 
-inline int chunks_for(uint32_t D) { return (D + kBlock - 1) / kBlock; }
+// kernel<<<grid>>>(args...) after the opt-in to kSmemBytes of dynamic shared memory (once per kernel and device)
+template <typename Kernel, typename... Args>
+cudaError_t launch(Kernel kernel, dim3 grid, cudaStream_t stream, const Args &...args) {
+  cudaError_t e = ensure_max_dynamic_smem(reinterpret_cast<const void *>(kernel), kSmemBytes, current_device());
+  if (e != cudaSuccess) return e;
+  kernel<<<grid, kThreads, kSmemBytes, stream>>>(args...);
+  return cudaGetLastError();
+}
 
 }  // namespace simt
 
-#define MFA_SIMT_DISPATCH(NCHUNKS, KERNEL, GRID, ...)                                     \
-  do {                                                                                    \
-    cudaError_t e_;                                                                       \
-    if ((NCHUNKS) <= 1) {                                                                 \
-      e_ = simt::prepare(simt::KERNEL<1>);                                                \
-      if (e_ != cudaSuccess) return e_;                                                   \
-      simt::KERNEL<1><<<GRID, simt::kThreads, simt::kSmemBytes, stream>>>(__VA_ARGS__);   \
-    } else if ((NCHUNKS) <= 2) {                                                          \
-      e_ = simt::prepare(simt::KERNEL<2>);                                                \
-      if (e_ != cudaSuccess) return e_;                                                   \
-      simt::KERNEL<2><<<GRID, simt::kThreads, simt::kSmemBytes, stream>>>(__VA_ARGS__);   \
-    } else if ((NCHUNKS) <= 4) {                                                          \
-      e_ = simt::prepare(simt::KERNEL<4>);                                                \
-      if (e_ != cudaSuccess) return e_;                                                   \
-      simt::KERNEL<4><<<GRID, simt::kThreads, simt::kSmemBytes, stream>>>(__VA_ARGS__);   \
-    } else {                                                                              \
-      e_ = simt::prepare(simt::KERNEL<8>);                                                \
-      if (e_ != cudaSuccess) return e_;                                                   \
-      simt::KERNEL<8><<<GRID, simt::kThreads, simt::kSmemBytes, stream>>>(__VA_ARGS__);   \
-    }                                                                                     \
-  } while (0)
-
 cudaError_t launch_simt_forward(const AttentionParams &p, cudaStream_t stream) {
   dim3 grid((p.R + simt::kBlock - 1) / simt::kBlock, p.batch);
-  MFA_SIMT_DISPATCH(simt::chunks_for(p.D), simt_forward_kernel, grid, p);
-  return cudaGetLastError();
+  return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
+    return simt::launch(simt::simt_forward_kernel<decltype(nch)::value>, grid, stream, p);
+  });
 }
 
 cudaError_t launch_simt_backward_query(const AttentionParams &p, cudaStream_t stream) {
   dim3 grid((p.R + simt::kBlock - 1) / simt::kBlock, p.batch);
-  MFA_SIMT_DISPATCH(simt::chunks_for(p.D), simt_backward_query_kernel, grid, p);
-  return cudaGetLastError();
+  return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
+    return simt::launch(simt::simt_backward_query_kernel<decltype(nch)::value>, grid, stream, p);
+  });
 }
 
 cudaError_t launch_simt_backward_key_value(const AttentionParams &p, cudaStream_t stream) {
   // two accumulators (dV, dK) per thread: keep at most 4 chunks (256 columns) of each in registers and
   // slice larger head dimensions over blockIdx.y (each slice recomputes S and dP).
-  int chunks = simt::chunks_for(p.D);
-  int nch = chunks <= 1 ? 1 : chunks <= 2 ? 2 : 4;
-  uint32_t dSlices = (chunks + nch - 1) / nch;
-  dim3 grid((p.C + simt::kBlock - 1) / simt::kBlock, p.batch / p.group * dSlices);  // one CTA row per K/V head
-  cudaError_t e;
-  if (nch == 1) {
-    if ((e = simt::prepare(simt::simt_backward_key_value_kernel<1>)) != cudaSuccess) return e;
-    simt::simt_backward_key_value_kernel<1><<<grid, simt::kThreads, simt::kSmemBytes, stream>>>(p, dSlices);
-  } else if (nch == 2) {
-    if ((e = simt::prepare(simt::simt_backward_key_value_kernel<2>)) != cudaSuccess) return e;
-    simt::simt_backward_key_value_kernel<2><<<grid, simt::kThreads, simt::kSmemBytes, stream>>>(p, dSlices);
-  } else {
-    if ((e = simt::prepare(simt::simt_backward_key_value_kernel<4>)) != cudaSuccess) return e;
-    simt::simt_backward_key_value_kernel<4><<<grid, simt::kThreads, simt::kSmemBytes, stream>>>(p, dSlices);
-  }
-  return cudaGetLastError();
+  const int chunks = simt::chunks_for(p.D);
+  return simt::with_chunks<4>(chunks, [&](auto nch) {
+    constexpr int NCH = decltype(nch)::value;
+    const uint32_t dSlices = (chunks + NCH - 1) / NCH;
+    dim3 grid((p.C + simt::kBlock - 1) / simt::kBlock, p.batch / p.group * dSlices);  // one CTA row per K/V head
+    return simt::launch(simt::simt_backward_key_value_kernel<NCH>, grid, stream, p, dSlices);
+  });
 }
 
 // Launch geometry reported through AttentionKernel.threadgroupSize / threadgroupMemoryAllocation /

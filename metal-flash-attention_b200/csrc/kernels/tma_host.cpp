@@ -106,16 +106,4 @@ cudaError_t make_tensor_map_16bit(CUtensorMap *map, const void *base, uint32_t s
   return encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, seq, D, batch, 64, box_rows);
 }
 
-// Transposed operand: [batch][D][seq] (leading dimension = seq), tiled as boxes of 64 (seq) x box_d_rows (D) x 1.
-cudaError_t make_tensor_map_16bit_transposed(CUtensorMap *map, const void *base, uint32_t seq, uint32_t D, uint32_t batch,
-                                             uint32_t box_d_rows) {
-  // same encoder with the roles of the two inner dimensions swapped: inner extent = seq, rows = D
-  return encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, D, seq, batch, 64, box_d_rows);
-}
-
-cudaError_t make_tensor_map_f32(CUtensorMap *map, const void *base, uint32_t seq, uint32_t D, uint32_t batch,
-                                uint32_t box_rows) {
-  return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, base, seq, D, batch, 32, box_rows);
-}
-
 }  // namespace mfa

@@ -13,15 +13,6 @@ namespace mfa {
 cudaError_t make_tensor_map_16bit(CUtensorMap *map, const void *base, uint32_t seq, uint32_t D, uint32_t batch,
                                   uint32_t box_rows);
 
-// The same operand stored transposed, [batch][D][seq] (leading dimension = seq; AttentionKernel.swift:189-195): boxes of
-// 64 (seq) x box_d_rows (D) x 1.  Needs seq % 8 == 0 (16-byte row pitch).
-cudaError_t make_tensor_map_16bit_transposed(CUtensorMap *map, const void *base, uint32_t seq, uint32_t D, uint32_t batch,
-                                             uint32_t box_d_rows);
-
-// Row-major [batch][seq][D] matrix of FP32 elements, boxes of 32 (D) x box_rows x 1, 128-byte swizzle.
-cudaError_t make_tensor_map_f32(CUtensorMap *map, const void *base, uint32_t seq, uint32_t D, uint32_t batch,
-                                uint32_t box_rows);
-
 void set_launch_detail(const char *fmt, ...);
 
 }  // namespace mfa

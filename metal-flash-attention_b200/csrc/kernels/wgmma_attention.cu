@@ -50,6 +50,9 @@ constexpr uint32_t kWG = 128;    // threads per warpgroup
 constexpr uint32_t kRows = 64;   // rows of one wgmma M tile (one warpgroup)
 constexpr uint32_t kBarBytes = 64;
 
+// The first of the two accumulator rows that thread t of a warpgroup holds (the second is 8 below it; wgmma.cuh)
+__device__ __forceinline__ uint32_t frag_row(uint32_t t) { return (t / 32) * 16 + (t % 32) / 4; }
+
 // Shared-memory tiles are [column chunk][rows][64 16-bit elements], 128-byte swizzled, one TMA box per chunk.
 // K-major descriptor of K step kk (16 elements) for the 64-row M / N tile starting at row `row0` of a ROWS-row tile
 template <uint32_t ROWS>
@@ -60,6 +63,15 @@ __device__ __forceinline__ uint64_t desc_kmajor(uint32_t tile, uint32_t row0, ui
 template <uint32_t ROWS>
 __device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile, uint32_t kk, uint32_t c0) {
   return make_smem_desc_sw128(tile + c0 * ROWS * 128 + kk * 16 * 128, ROWS * 128, 1024);
+}
+
+// acc = A B^T over the DCH * 64 head columns: A = rows [a0, a0 + 64) of the ROWS_A-row tile at sA, B = the N-row tile
+// at sB, both K-major.  Issues the wgmmas only; the caller fences, commits and waits.
+template <uint32_t DCH, uint32_t N, bool kBF16, uint32_t ROWS_A>
+__device__ __forceinline__ void mma_ss(float (&acc)[N / 2], uint32_t sA, uint32_t a0, uint32_t sB) {
+#pragma unroll
+  for (uint32_t kk = 0; kk < DCH * 4; ++kk)
+    Wgmma<N, kBF16>::ss(acc, desc_kmajor<ROWS_A>(sA, a0, kk), desc_kmajor<N>(sB, 0, kk), kk > 0);
 }
 
 template <bool kBF16>
@@ -78,6 +90,62 @@ __device__ __forceinline__ void a_frag(const float (&s)[NR], uint32_t kk, uint32
 __device__ __forceinline__ uint8_t *align1024(uint8_t *p) {
   return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
 }
+
+// Shared memory of a kernel from its 1024-byte-aligned base: the resident tiles, two ring stages of two streamed tiles
+// each, then the barriers.  kSmemBytes adds the slack for aligning the base.
+template <uint32_t RESIDENT, uint32_t TILE>
+struct SmemLayout {
+  static constexpr uint32_t kResidentBytes = RESIDENT, kStageBytes = 2 * TILE;
+  static constexpr uint32_t kBarOffset = RESIDENT + 2 * kStageBytes;
+  static constexpr uint32_t kSmemBytes = 1024 + kBarOffset + kBarBytes;
+};
+
+// The two-stage ring of the streamed tiles.  Traversal step n goes to stage n & 1, which completes on bar[1 + (n & 1)]
+// with parity (n >> 1) & 1; bar[0] tracks the resident tiles.  Thread 0 issues every load; a load callback
+// load(n, dst, bar) issues the TMA loads of step n's two tiles into dst.  The callbacks are taken by reference: copying
+// the closures into these calls made ptxas schedule the dK/dV kernels differently (1-2 registers, more instructions).
+template <class Smem>
+struct Ring {
+  uint8_t *base;
+  uint64_t *bar;
+
+  __device__ __forceinline__ explicit Ring(uint8_t *smem)
+      : base(align1024(smem)), bar(reinterpret_cast<uint64_t *>(base + Smem::kBarOffset)) {}
+  // stage s starts kResidentBytes + s kStageBytes into the base
+  __device__ __forceinline__ uint8_t *stage(uint32_t n) const {
+    return base + Smem::kResidentBytes + (n & 1) * Smem::kStageBytes;
+  }
+
+  __device__ __forceinline__ void init() const {
+    if (threadIdx.x == 0) {
+      for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
+      fence_barrier_init();
+    }
+    __syncthreads();
+  }
+  // step n into stage s = n & 1
+  template <class Load>
+  __device__ __forceinline__ void load(uint32_t n, uint32_t s, const Load &issue) const {
+    mbar_arrive_expect_tx(&bar[1 + s], Smem::kStageBytes);
+    issue(n, stage(s), &bar[1 + s]);
+  }
+  // thread 0: the resident tiles (load_resident(base, bar)) and the first two steps
+  template <class Resident, class Load>
+  __device__ __forceinline__ void start(const Resident &load_resident, uint32_t total, const Load &load) const {
+    if (threadIdx.x != 0) return;
+    mbar_arrive_expect_tx(&bar[0], Smem::kResidentBytes);
+    load_resident(base, &bar[0]);
+    for (uint32_t n = 0; n < 2 && n < total; ++n) this->load(n, n, load);
+  }
+  __device__ __forceinline__ void wait_resident() const { mbar_wait(&bar[0], 0); }
+  __device__ __forceinline__ void wait(uint32_t n) const { mbar_wait(&bar[1 + (n & 1)], (n >> 1) & 1); }
+  // every thread is done with step n: its stage takes step n + 2
+  template <class Load>
+  __device__ __forceinline__ void release_and_refill(uint32_t n, uint32_t total, const Load &load) const {
+    __syncthreads();
+    if (threadIdx.x == 0 && n + 2 < total) this->load(n + 2, n & 1, load);
+  }
+};
 
 // DCH column chunks of a `rows`-row tile at (column 0, row0, head) -> smem, completion on bar
 template <uint32_t DCH, uint32_t ROWS>
@@ -98,7 +166,7 @@ template <int NR>
 __device__ __forceinline__ void store_acc(const float (&acc)[NR], float *out, uint32_t row0, uint32_t limit, uint32_t col0,
                                           uint32_t D, float inv0, float inv1) {
   const uint32_t t = threadIdx.x % kWG;
-  const uint32_t r = row0 + (t / 32) * 16 + (t % 32) / 4;
+  const uint32_t r = row0 + frag_row(t);
 #pragma unroll
   for (int i = 0; i < NR / 4; ++i) {
     const uint32_t col = col0 + 8 * i + 2 * (t % 4);
@@ -111,28 +179,68 @@ __device__ __forceinline__ void store_acc(const float (&acc)[NR], float *out, ui
   }
 }
 
-// Causal: how many of the key blocks [kb0, kb0 + per_split) the rows [row_base, min(row_base + rows, R)) can see (key
-// j <= row + delta).  Signed: a split range can lie wholly past the diagonal, and with R > C a tile can see no key at all.
-template <uint32_t BN>
-__device__ __forceinline__ uint32_t visible_key_blocks(uint32_t row_base, uint32_t rows, uint32_t R, uint32_t C,
-                                                       int delta, uint32_t kb0, uint32_t per_split) {
-  const int last_key = static_cast<int>(min(row_base + rows, R)) - 1 + delta;  // seen by the tile's last row
-  const int end = last_key < 0 ? 0 : min(static_cast<int>((C + BN - 1) / BN), last_key / static_cast<int>(BN) + 1);
-  return static_cast<uint32_t>(max(0, min(end, static_cast<int>(kb0 + per_split)) - static_cast<int>(kb0)));
+// ================================================================================================ traversal ranges
+// The key blocks of a forward / dQ CTA: [kb0, kb0 + result) of the split range [kb0, kb0 + per_split).  Causal: only
+// those the rows [row_base, min(row_base + rows, R)) can see (key j <= row + delta).  Signed: a split range can lie
+// wholly past the diagonal, and with R > C a tile can see no key at all.
+template <uint32_t BN, bool kCausal>
+__device__ __forceinline__ uint32_t key_blocks(uint32_t row_base, uint32_t rows, uint32_t R, uint32_t C, int delta,
+                                               uint32_t kb0, uint32_t per_split) {
+  if constexpr (!kCausal) {
+    return min((C + BN - 1) / BN - kb0, per_split);
+  } else {
+    const int last_key = static_cast<int>(min(row_base + rows, R)) - 1 + delta;  // seen by the tile's last row
+    const int end = last_key < 0 ? 0 : min(static_cast<int>((C + BN - 1) / BN), last_key / static_cast<int>(BN) + 1);
+    return static_cast<uint32_t>(max(0, min(end, static_cast<int>(kb0 + per_split)) - static_cast<int>(kb0)));
+  }
 }
 
-// Causal: S -> -inf for the keys past the diagonal in a 64 x BN accumulator block whose first key column is `key0`;
-// row_a is this thread's first row (the second is row_a + 8)
-template <int NR>
-__device__ __forceinline__ void mask_past_diagonal(float (&s)[NR], int key0, int row_a, int delta) {
-  const int c0 = key0 + 2 * static_cast<int>(threadIdx.x % 4), lim0 = row_a + delta, lim1 = lim0 + 8;
+// Causal dK/dV: the first query block that sees key `key` (query >= key - delta), and how many of the blocks [qs, qb0 +
+// per_split) exist (signed: a split range can end before qs)
+template <uint32_t BM>
+__device__ __forceinline__ uint32_t first_query_block(uint32_t key, int delta) {
+  const int q = static_cast<int>(key) - delta;
+  return q <= 0 ? 0u : static_cast<uint32_t>(q) / BM;
+}
+template <uint32_t BM>
+__device__ __forceinline__ uint32_t visible_query_blocks(uint32_t R, uint32_t qb0, uint32_t qs, uint32_t per_split) {
+  const int end = min(static_cast<int>((R + BM - 1) / BM), static_cast<int>(qb0 + per_split));
+  return static_cast<uint32_t>(max(0, end - static_cast<int>(qs)));
+}
+
+// ================================================================================================ masks
+// Causal: a block whose last key is `last_key` has elements past the diagonal for some row from `first_query` on
+__device__ __forceinline__ bool crosses_diagonal(int last_key, int first_query, int delta) {
+  return last_key > first_query + delta;
+}
+
+// Causal: -inf for the elements past the diagonal (key > query + delta) of a 64 x N accumulator block, S (rows are
+// queries, columns keys) or, kKeyRows, S^T (rows are keys, columns queries).  row: this thread's first row (the second
+// is row + 8); col0: the block's first column.
+template <bool kKeyRows, int NR>
+__device__ __forceinline__ void mask_past_diagonal(float (&s)[NR], int row, int col0, int delta) {
+  // masked: key > query + delta, with delta added to the query side (the columns of S^T, the row of S)
+  const int c0 = col0 + 2 * static_cast<int>(threadIdx.x % 4) + (kKeyRows ? delta : 0);
+  const int r0 = row + (kKeyRows ? 0 : delta);
 #pragma unroll
   for (int i = 0; i < NR / 4; ++i)
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      if (c0 + 8 * i + e > lim0) s[4 * i + e] = -INFINITY;
-      if (c0 + 8 * i + e > lim1) s[4 * i + 2 + e] = -INFINITY;
+      const int c = c0 + 8 * i + e;
+      if (kKeyRows ? r0 > c : c > r0) s[4 * i + e] = -INFINITY;
+      if (kKeyRows ? r0 + 8 > c : c > r0 + 8) s[4 * i + 2 + e] = -INFINITY;
     }
+}
+
+// Keys past C: -inf in both rows of a 64 x N accumulator block of S whose first key column is key0
+template <int NR>
+__device__ __forceinline__ void mask_past_edge(float (&s)[NR], uint32_t key0, uint32_t C) {
+  const uint32_t c0 = key0 + 2 * (threadIdx.x % 4);
+#pragma unroll
+  for (uint32_t i = 0; i < NR / 4; ++i)
+#pragma unroll
+    for (uint32_t e = 0; e < 2; ++e)
+      if (c0 + 8 * i + e >= C) s[4 * i + e] = s[4 * i + 2 + e] = -INFINITY;
 }
 
 // ================================================================================================ forward
@@ -173,13 +281,14 @@ __global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O
   if (quad == 0) store_stat(L, row, l_prec, empty ? INFINITY : lmax + log2f(denom));
 }
 
-// kPar / kTrav: rows of the parallelization / traversal axis per CTA / per pipeline stage (every *Cfg has them)
+// kPar / kTrav: rows of the parallelization / traversal axis per CTA / per pipeline stage; kQueryBoxRows /
+// kKeyBoxRows: rows of the TMA boxes of Q and dO / of K and V; Smem: the shared-memory layout (every *Cfg has them)
 template <uint32_t DCH>
 struct FwdCfg {
   static constexpr uint32_t kThreads = 2 * kWG, kTileM = 2 * kRows, BN = DCH == 4 ? 64 : 128;
-  static constexpr uint32_t kPar = kTileM, kTrav = BN;
+  static constexpr uint32_t kPar = kTileM, kTrav = BN, kQueryBoxRows = kTileM, kKeyBoxRows = BN;
   static constexpr uint32_t kQBytes = DCH * kTileM * 128, kKVBytes = DCH * BN * 128;
-  static constexpr uint32_t kSmemBytes = 1024 + kQBytes + 2 * 2 * kKVBytes + kBarBytes;
+  using Smem = SmemLayout<kQBytes, kKVBytes>;  // resident Q; stage: K, V
 };
 
 template <uint32_t DCH, bool kBF16, bool kCausal>
@@ -191,70 +300,49 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t *base = align1024(smem_raw);
-  uint8_t *kv = base + Cfg::kQBytes;  // stage s: K at kv + 2 s kKVBytes, V right after it
-  uint64_t *bar = reinterpret_cast<uint64_t *>(kv + 4 * Cfg::kKVBytes);  // [0] Q, [1 + s] stage s
+  const Ring<typename Cfg::Smem> ring(smem_raw);  // resident Q; step j: K and V of key block kb0 + j
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   // (causal: unlike dQ, the forward gains nothing measurable from starting the tiles with the most key blocks first)
   const uint32_t head = blockIdx.y, row_base = blockIdx.x * Cfg::kTileM;
   const uint32_t kv_head = head / group;  // grouped K/V: the query heads of a group read one K/V head
-  // this CTA's key blocks: [kb0, kb0 + blocks)
   const uint32_t kb0 = blockIdx.z * sp.blocks_per_split;
-  const uint32_t blocks = kCausal ? visible_key_blocks<BN>(row_base, Cfg::kTileM, R, C, delta, kb0, sp.blocks_per_split)
-                                  : min((C + BN - 1) / BN - kb0, sp.blocks_per_split);
+  const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, R, C, delta, kb0, sp.blocks_per_split);
 
-  auto load_kv = [&](uint32_t j, uint32_t s) {
-    uint8_t *dst = kv + s * 2 * Cfg::kKVBytes;
-    mbar_arrive_expect_tx(&bar[1 + s], 2 * Cfg::kKVBytes);
-    load_tile<DCH, BN>(dst, &mapK, &bar[1 + s], (kb0 + j) * BN, kv_head);
-    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, &bar[1 + s], (kb0 + j) * BN, kv_head);
+  auto load_kv = [&](uint32_t j, uint8_t *dst, uint64_t *bar) {
+    load_tile<DCH, BN>(dst, &mapK, bar, (kb0 + j) * BN, kv_head);
+    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, bar, (kb0 + j) * BN, kv_head);
   };
   if (tid == 0) {
     prefetch_tensormap(&mapQ);
     prefetch_tensormap(&mapK);
     prefetch_tensormap(&mapV);
-    for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
-    fence_barrier_init();
   }
-  __syncthreads();
-  if (tid == 0) {
-    mbar_arrive_expect_tx(&bar[0], Cfg::kQBytes);
-    load_tile<DCH, Cfg::kTileM>(base, &mapQ, &bar[0], row_base, head);
-    for (uint32_t s = 0; s < 2 && s < blocks; ++s) load_kv(s, s);
-  }
+  ring.init();
+  ring.start([&](uint8_t *dst, uint64_t *bar) { load_tile<DCH, Cfg::kTileM>(dst, &mapQ, bar, row_base, head); }, blocks,
+             load_kv);
 
-  const uint32_t sQ = smem_u32(base);
+  const uint32_t sQ = smem_u32(ring.base);
   float o[NO / 2];
   zero(o);
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-  mbar_wait(&bar[0], 0);
+  ring.wait_resident();
   for (uint32_t j = 0; j < blocks; ++j) {
-    const uint32_t s = j & 1;
-    mbar_wait(&bar[1 + s], (j >> 1) & 1);
-    const uint32_t sK = smem_u32(kv + s * 2 * Cfg::kKVBytes), sV = sK + Cfg::kKVBytes;
+    ring.wait(j);
+    const uint32_t sK = smem_u32(ring.stage(j)), sV = sK + Cfg::kKVBytes;
     float sc[BN / 2];
     zero(sc);
     wgmma_fence();
-#pragma unroll
-    for (uint32_t kk = 0; kk < DCH * 4; ++kk)
-      Wgmma<BN, kBF16>::ss(sc, desc_kmajor<Cfg::kTileM>(sQ, wg * kRows, kk), desc_kmajor<BN>(sK, 0, kk), kk > 0);
+    mma_ss<DCH, BN, kBF16, Cfg::kTileM>(sc, sQ, wg * kRows, sK);
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(sc);
 
     // keys past C: -inf before the row max
-    if ((kb0 + j + 1) * BN > C) {
-      const uint32_t c0 = (kb0 + j) * BN + 2 * (t % 4);
-#pragma unroll
-      for (uint32_t i = 0; i < BN / 8; ++i)
-#pragma unroll
-        for (uint32_t e = 0; e < 2; ++e)
-          if (c0 + 8 * i + e >= C) sc[4 * i + e] = sc[4 * i + 2 + e] = -INFINITY;
-    }
+    if ((kb0 + j + 1) * BN > C) mask_past_edge(sc, (kb0 + j) * BN, C);
     if constexpr (kCausal) {
       const int key0 = static_cast<int>((kb0 + j) * BN);
-      if (key0 + static_cast<int>(BN) - 1 > static_cast<int>(row_base) + delta)  // the block crosses the diagonal
-        mask_past_diagonal(sc, key0, static_cast<int>(row_base + wg * kRows + (t / 32) * 16 + (t % 32) / 4), delta);
+      if (crosses_diagonal(key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base), delta))
+        mask_past_diagonal<false>(sc, static_cast<int>(row_base + wg * kRows + frag_row(t)), key0, delta);
     }
     float r0 = -INFINITY, r1 = -INFINITY;
 #pragma unroll
@@ -307,8 +395,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(o);
-    __syncthreads();  // every warpgroup is done with stage s
-    if (tid == 0 && j + 2 < blocks) load_kv(j + 2, s);
+    ring.release_and_refill(j, blocks, load_kv);
   }
 
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
@@ -323,7 +410,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   const bool empty0 = kCausal && l0 == 0.f, empty1 = kCausal && l1 == 0.f;
   store_acc(o, Oout, row0, R, 0, D, empty0 ? 0.f : 1.0f / l0, empty1 ? 0.f : 1.0f / l1);
   if (t % 4 == 0) {
-    const uint32_t r = row0 + (t / 32) * 16 + (t % 32) / 4;
+    const uint32_t r = row0 + frag_row(t);
     void *Lout = sp.splits == 1 ? L : sp.L_part;
     const int prec = sp.splits == 1 ? l_prec : FP32;
     const size_t hb = (sp.splits == 1 ? static_cast<size_t>(head) : slice) * R;
@@ -338,9 +425,9 @@ template <uint32_t DCH>
 struct QCfg {
   static constexpr uint32_t kWarpgroups = DCH == 4 ? 1 : 2;
   static constexpr uint32_t kThreads = kWarpgroups * kWG, kTileM = kWarpgroups * kRows, BN = 64;
-  static constexpr uint32_t kPar = kTileM, kTrav = BN;
+  static constexpr uint32_t kPar = kTileM, kTrav = BN, kQueryBoxRows = kTileM, kKeyBoxRows = BN;
   static constexpr uint32_t kQBytes = DCH * kTileM * 128, kKVBytes = DCH * BN * 128;
-  static constexpr uint32_t kSmemBytes = 1024 + 2 * kQBytes + 2 * 2 * kKVBytes + kBarBytes;
+  using Smem = SmemLayout<2 * kQBytes, kKVBytes>;  // resident Q, dO; stage: K, V
 };
 
 struct BwdArgs {
@@ -366,39 +453,30 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   using Cfg = QCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t *base = align1024(smem_raw);
-  uint8_t *kv = base + 2 * Cfg::kQBytes;
-  uint64_t *bar = reinterpret_cast<uint64_t *>(kv + 4 * Cfg::kKVBytes);
+  const Ring<typename Cfg::Smem> ring(smem_raw);  // resident Q, dO; step j: K and V of key block kb0 + j
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   // causal: tiles in reverse order, so that the ones with the most key blocks start first and the wave tail is short
   const uint32_t tile = kCausal ? gridDim.x - 1 - blockIdx.x : blockIdx.x;
   const uint32_t head = blockIdx.y, row_base = tile * Cfg::kTileM, kv_head = head / a.group;
   const uint32_t kb0 = blockIdx.z * a.blocks_per_split;
-  const uint32_t blocks = kCausal ? visible_key_blocks<BN>(row_base, Cfg::kTileM, a.R, a.C, a.delta, kb0, a.blocks_per_split)
-                                  : min((a.C + BN - 1) / BN - kb0, a.blocks_per_split);
+  const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, a.R, a.C, a.delta, kb0, a.blocks_per_split);
 
-  auto load_kv = [&](uint32_t j, uint32_t s) {
-    uint8_t *dst = kv + s * 2 * Cfg::kKVBytes;
-    mbar_arrive_expect_tx(&bar[1 + s], 2 * Cfg::kKVBytes);
-    load_tile<DCH, BN>(dst, &mapK, &bar[1 + s], (kb0 + j) * BN, kv_head);
-    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, &bar[1 + s], (kb0 + j) * BN, kv_head);
+  auto load_kv = [&](uint32_t j, uint8_t *dst, uint64_t *bar) {
+    load_tile<DCH, BN>(dst, &mapK, bar, (kb0 + j) * BN, kv_head);
+    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, bar, (kb0 + j) * BN, kv_head);
   };
-  if (tid == 0) {
-    for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  if (tid == 0) {
-    mbar_arrive_expect_tx(&bar[0], 2 * Cfg::kQBytes);
-    load_tile<DCH, Cfg::kTileM>(base, &mapQ, &bar[0], row_base, head);
-    load_tile<DCH, Cfg::kTileM>(base + Cfg::kQBytes, &mapdO, &bar[0], row_base, head);
-    for (uint32_t s = 0; s < 2 && s < blocks; ++s) load_kv(s, s);
-  }
+  ring.init();
+  ring.start(
+      [&](uint8_t *dst, uint64_t *bar) {
+        load_tile<DCH, Cfg::kTileM>(dst, &mapQ, bar, row_base, head);
+        load_tile<DCH, Cfg::kTileM>(dst + Cfg::kQBytes, &mapdO, bar, row_base, head);
+      },
+      blocks, load_kv);
 
   // D = rowsum(dO * O) / sqrt(D) for this thread's two rows (the four threads of a row split the columns), while the
   // tiles are in flight; stored for the dK/dV kernel, kept in FP32 here
   const uint32_t row0 = row_base + wg * kRows;
-  const uint32_t r = row0 + (t / 32) * 16 + (t % 32) / 4;
+  const uint32_t r = row0 + frag_row(t);
   const size_t hb = static_cast<size_t>(head) * a.R;
   float Dr[2], Lr[2];
 #pragma unroll
@@ -419,12 +497,12 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     if (t % 4 == 0 && r + 8 * h < a.R && blockIdx.z == 0) store_stat(a.Dterm, hb + r + 8 * h, a.d_prec, Dr[h]);
   }
 
-  const uint32_t sQ = smem_u32(base), sdO = sQ + Cfg::kQBytes;
-  mbar_wait(&bar[0], 0);
+  const uint32_t sQ = smem_u32(ring.base), sdO = sQ + Cfg::kQBytes;
+  ring.wait_resident();
   if constexpr (kConvertDO) {
     // BF16 dO beside FP16 Q/K/V: wgmma takes one element type for A and B, so the resident dO tile is rewritten as
     // FP16 in place (exact for 2^-14 <= |x| < 65504)
-    uint4 *tile = reinterpret_cast<uint4 *>(base + Cfg::kQBytes);
+    uint4 *tile = reinterpret_cast<uint4 *>(ring.base + Cfg::kQBytes);
     for (uint32_t i = tid; i < Cfg::kQBytes / 16; i += Cfg::kThreads) tile[i] = bwd::bf16x8_to_f16x8(tile[i]);
     fence_proxy_async_smem();
     __syncthreads();
@@ -432,27 +510,22 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   float dq[NO / 2];
   zero(dq);
   for (uint32_t j = 0; j < blocks; ++j) {
-    const uint32_t s = j & 1;
-    mbar_wait(&bar[1 + s], (j >> 1) & 1);
-    const uint32_t sK = smem_u32(kv + s * 2 * Cfg::kKVBytes), sV = sK + Cfg::kKVBytes;
+    ring.wait(j);
+    const uint32_t sK = smem_u32(ring.stage(j)), sV = sK + Cfg::kKVBytes;
     float sc[BN / 2], dp[BN / 2];
     zero(sc);
     zero(dp);
     wgmma_fence();
-#pragma unroll
-    for (uint32_t kk = 0; kk < DCH * 4; ++kk)
-      Wgmma<BN, kBF16>::ss(sc, desc_kmajor<Cfg::kTileM>(sQ, wg * kRows, kk), desc_kmajor<BN>(sK, 0, kk), kk > 0);
-#pragma unroll
-    for (uint32_t kk = 0; kk < DCH * 4; ++kk)
-      Wgmma<BN, kBF16>::ss(dp, desc_kmajor<Cfg::kTileM>(sdO, wg * kRows, kk), desc_kmajor<BN>(sV, 0, kk), kk > 0);
+    mma_ss<DCH, BN, kBF16, Cfg::kTileM>(sc, sQ, wg * kRows, sK);
+    mma_ss<DCH, BN, kBF16, Cfg::kTileM>(dp, sdO, wg * kRows, sV);
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(sc);
     fence_regs(dp);
     if constexpr (kCausal) {  // S -> -inf past the diagonal, so P = 0 there
       const int key0 = static_cast<int>((kb0 + j) * BN);
-      if (key0 + static_cast<int>(BN) - 1 > static_cast<int>(row_base) + a.delta)
-        mask_past_diagonal(sc, key0, static_cast<int>(r), a.delta);
+      if (crosses_diagonal(key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base), a.delta))
+        mask_past_diagonal<false>(sc, static_cast<int>(r), key0, a.delta);
     }
     const uint32_t c0 = (kb0 + j) * BN + 2 * (t % 4);
 #pragma unroll
@@ -473,34 +546,20 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(dq);
-    __syncthreads();
-    if (tid == 0 && j + 2 < blocks) load_kv(j + 2, s);
+    ring.release_and_refill(j, blocks, load_kv);
   }
   store_acc(dq, a.dQ + blockIdx.z * a.split_stride + hb * a.D, row0, a.R, 0, a.D, 1.f, 1.f);
 }
 
 // ================================================================================================ backward dK/dV
-// Causal: the first query block that sees key `key` (query >= key - delta), and how many of the blocks [qs, qb0 +
-// per_split) exist (signed: a split range can end before qs)
-template <uint32_t BM>
-__device__ __forceinline__ uint32_t first_query_block(uint32_t key, int delta) {
-  const int q = static_cast<int>(key) - delta;
-  return q <= 0 ? 0u : static_cast<uint32_t>(q) / BM;
-}
-template <uint32_t BM>
-__device__ __forceinline__ uint32_t visible_query_blocks(uint32_t R, uint32_t qb0, uint32_t qs, uint32_t per_split) {
-  const int end = min(static_cast<int>((R + BM - 1) / BM), static_cast<int>(qb0 + per_split));
-  return static_cast<uint32_t>(max(0, end - static_cast<int>(qs)));
-}
-
 template <uint32_t DCH>
 struct KVCfg {
   static constexpr bool kSplitD = DCH == 4;  // both warpgroups on the same 64 keys, half of the D columns each
   static constexpr uint32_t kThreads = 2 * kWG, kTileN = kSplitD ? kRows : 2 * kRows, BM = 64;
-  static constexpr uint32_t kPar = kTileN, kTrav = BM;
+  static constexpr uint32_t kPar = kTileN, kTrav = BM, kQueryBoxRows = BM, kKeyBoxRows = kTileN;
   static constexpr uint32_t kAcc = kSplitD ? 128 : DCH * 64;  // accumulator columns per warpgroup
   static constexpr uint32_t kKBytes = DCH * kTileN * 128, kQBytes = DCH * BM * 128;
-  static constexpr uint32_t kSmemBytes = 1024 + 2 * kKBytes + 2 * 2 * kQBytes + kBarBytes;
+  using Smem = SmemLayout<2 * kKBytes, kQBytes>;  // resident K, V; stage: Q, dO
 };
 
 template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
@@ -511,9 +570,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   using Cfg = KVCfg<DCH>;
   constexpr uint32_t BM = Cfg::BM, NA = Cfg::kAcc;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t *base = align1024(smem_raw);
-  uint8_t *qd = base + 2 * Cfg::kKBytes;  // stage s: Q at qd + 2 s kQBytes, dO right after it
-  uint64_t *bar = reinterpret_cast<uint64_t *>(qd + 4 * Cfg::kQBytes);
+  const Ring<typename Cfg::Smem> ring(smem_raw);  // resident K, V; step n: Q and dO of one query block
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   // grouped K/V: blockIdx.y is a K/V head, and the CTA walks the query blocks of every query head of its group
   const uint32_t kv_head = blockIdx.y, key_base = blockIdx.x * Cfg::kTileN;
@@ -526,34 +583,27 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   // + i that drives the Q / dO ring: prefetch and barrier parity carry across head boundaries
   const uint32_t total = a.group * blocks;
 
-  auto load_qd = [&](uint32_t n, uint32_t s) {
+  auto load_qd = [&](uint32_t n, uint8_t *dst, uint64_t *bar) {
     const uint32_t g = n / blocks, i = n - g * blocks;
-    uint8_t *dst = qd + s * 2 * Cfg::kQBytes;
-    mbar_arrive_expect_tx(&bar[1 + s], 2 * Cfg::kQBytes);
-    load_tile<DCH, BM>(dst, &mapQ, &bar[1 + s], (qs + i) * BM, kv_head * a.group + g);
-    load_tile<DCH, BM>(dst + Cfg::kQBytes, &mapdO, &bar[1 + s], (qs + i) * BM, kv_head * a.group + g);
+    load_tile<DCH, BM>(dst, &mapQ, bar, (qs + i) * BM, kv_head * a.group + g);
+    load_tile<DCH, BM>(dst + Cfg::kQBytes, &mapdO, bar, (qs + i) * BM, kv_head * a.group + g);
   };
-  if (tid == 0) {
-    for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  if (tid == 0) {
-    mbar_arrive_expect_tx(&bar[0], 2 * Cfg::kKBytes);
-    load_tile<DCH, Cfg::kTileN>(base, &mapK, &bar[0], key_base, kv_head);
-    load_tile<DCH, Cfg::kTileN>(base + Cfg::kKBytes, &mapV, &bar[0], key_base, kv_head);
-    for (uint32_t s = 0; s < 2 && s < total; ++s) load_qd(s, s);
-  }
-  const uint32_t sK = smem_u32(base), sV = sK + Cfg::kKBytes;
+  ring.init();
+  ring.start(
+      [&](uint8_t *dst, uint64_t *bar) {
+        load_tile<DCH, Cfg::kTileN>(dst, &mapK, bar, key_base, kv_head);
+        load_tile<DCH, Cfg::kTileN>(dst + Cfg::kKBytes, &mapV, bar, key_base, kv_head);
+      },
+      total, load_qd);
+  const uint32_t sK = smem_u32(ring.base), sV = sK + Cfg::kKBytes;
   const uint32_t krow = Cfg::kSplitD ? 0 : wg * kRows;      // this warpgroup's key rows inside the tile
   const uint32_t nchunk = Cfg::kSplitD ? wg * (NA / 64) : 0;  // ... and its first accumulator column chunk
   size_t hb = static_cast<size_t>(kv_head) * a.group * a.R;  // L / D rows of the current query head
   float dv[NA / 2], dk[NA / 2];
   zero(dv);
   zero(dk);
-  mbar_wait(&bar[0], 0);
+  ring.wait_resident();
   for (uint32_t n = 0, i = 0; n < total; ++n) {
-    const uint32_t s = n & 1;
     // per-query statistics of this thread's 16 columns, loaded while the tiles land
     float Lq[BM / 4], Dq[BM / 4];
     const uint32_t q0 = (qs + i) * BM + 2 * (t % 4);
@@ -565,43 +615,30 @@ __global__ void __launch_bounds__(2 * kWG, 1)
         Lq[2 * j + e] = load_stat(a.L, hb + q, a.l_prec);
         Dq[2 * j + e] = load_stat(a.Dterm, hb + q, a.d_prec);
       }
-    mbar_wait(&bar[1 + s], (n >> 1) & 1);
+    ring.wait(n);
     if constexpr (kConvertDO) {
       // BF16 dO beside FP16 Q/K/V on a small grid: the streamed dO tile is rewritten as FP16 in place (a grid of more
       // than one wave converts dO once, in a pass of its own, instead)
-      uint4 *tile = reinterpret_cast<uint4 *>(qd + s * 2 * Cfg::kQBytes + Cfg::kQBytes);
+      uint4 *tile = reinterpret_cast<uint4 *>(ring.stage(n) + Cfg::kQBytes);
       for (uint32_t k = tid; k < Cfg::kQBytes / 16; k += Cfg::kThreads) tile[k] = bwd::bf16x8_to_f16x8(tile[k]);
       fence_proxy_async_smem();
       __syncthreads();
     }
-    const uint32_t sQ = smem_u32(qd + s * 2 * Cfg::kQBytes), sdO = sQ + Cfg::kQBytes;
+    const uint32_t sQ = smem_u32(ring.stage(n)), sdO = sQ + Cfg::kQBytes;
     float st[BM / 2], dpt[BM / 2];
     zero(st);
     zero(dpt);
     wgmma_fence();
-#pragma unroll
-    for (uint32_t kk = 0; kk < DCH * 4; ++kk)
-      Wgmma<BM, kBF16>::ss(st, desc_kmajor<Cfg::kTileN>(sK, krow, kk), desc_kmajor<BM>(sQ, 0, kk), kk > 0);
-#pragma unroll
-    for (uint32_t kk = 0; kk < DCH * 4; ++kk)
-      Wgmma<BM, kBF16>::ss(dpt, desc_kmajor<Cfg::kTileN>(sV, krow, kk), desc_kmajor<BM>(sdO, 0, kk), kk > 0);
+    mma_ss<DCH, BM, kBF16, Cfg::kTileN>(st, sK, krow, sQ);
+    mma_ss<DCH, BM, kBF16, Cfg::kTileN>(dpt, sV, krow, sdO);
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(st);
     fence_regs(dpt);
     if constexpr (kCausal) {  // S^T -> -inf where key > query + delta, so P^T = 0 there
       const int qlo = static_cast<int>((qs + i) * BM);
-      if (static_cast<int>(key_base + Cfg::kTileN) - 1 > qlo + a.delta) {
-        const int kr = static_cast<int>(key_base + krow + (t / 32) * 16 + (t % 32) / 4);
-        const int qc = qlo + 2 * static_cast<int>(t % 4) + a.delta;
-#pragma unroll
-        for (int j = 0; j < static_cast<int>(BM / 8); ++j)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            if (kr > qc + 8 * j + e) st[4 * j + e] = -INFINITY;
-            if (kr + 8 > qc + 8 * j + e) st[4 * j + 2 + e] = -INFINITY;
-          }
-      }
+      if (crosses_diagonal(static_cast<int>(key_base + Cfg::kTileN) - 1, qlo, a.delta))
+        mask_past_diagonal<true>(st, static_cast<int>(key_base + krow + frag_row(t)), qlo, a.delta);
     }
 #pragma unroll
     for (uint32_t j = 0; j < BM / 8; ++j)
@@ -625,8 +662,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     wgmma_wait<0>();
     fence_regs(dv);
     fence_regs(dk);
-    __syncthreads();
-    if (tid == 0 && n + 2 < total) load_qd(n + 2, s);
+    ring.release_and_refill(n, total, load_qd);
     if (++i == blocks) {  // the next query head of the group; dK and dV keep accumulating
       i = 0;
       hb += a.R;
@@ -704,16 +740,31 @@ static cudaError_t prepare(Kernel kernel, uint32_t smem) {
   return ensure_max_dynamic_smem(reinterpret_cast<const void *>(kernel), smem, current_device());
 }
 
+// The tensor maps of a kernel: Q and (with_dO) dO in boxes of Cfg::kQueryBoxRows rows, K and V in boxes of
+// Cfg::kKeyBoxRows.  Grouped K/V: K and V hold batch / group heads.
+struct TensorMaps {
+  CUtensorMap Q, dO, K, V;
+};
+template <class Cfg>
+static cudaError_t make_maps(const AttentionParams &p, bool with_dO, TensorMaps *m) {
+  cudaError_t e;
+  if ((e = make_tensor_map_16bit(&m->Q, p.buf[sQ], p.R, p.D, p.batch, Cfg::kQueryBoxRows)) != cudaSuccess) return e;
+  if (with_dO &&
+      (e = make_tensor_map_16bit(&m->dO, p.buf[sdO], p.R, p.D, p.batch, Cfg::kQueryBoxRows)) != cudaSuccess)
+    return e;
+  const uint32_t kv_heads = p.batch / p.group;
+  if ((e = make_tensor_map_16bit(&m->K, p.buf[sK], p.C, p.D, kv_heads, Cfg::kKeyBoxRows)) != cudaSuccess) return e;
+  return make_tensor_map_16bit(&m->V, p.buf[sV], p.C, p.D, kv_heads, Cfg::kKeyBoxRows);
+}
+
 template <uint32_t DCH, bool kBF16, bool kCausal>
 cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
   using Cfg = FwdCfg<DCH>;
+  constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
   auto kernel = attention_forward_wgmma<DCH, kBF16, kCausal>;
+  TensorMaps m;
   cudaError_t e;
-  if ((e = prepare(kernel, Cfg::kSmemBytes)) != cudaSuccess) return e;
-  CUtensorMap mapQ, mapK, mapV;
-  if ((e = make_tensor_map_16bit(&mapQ, p.buf[sQ], p.R, p.D, p.batch, Cfg::kTileM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) return e;
+  if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess) return e;
   SplitArgs sp{plan.blocks_per_split, plan.splits, p.batch, nullptr, nullptr};
   const uint64_t rows_total = static_cast<uint64_t>(p.batch) * p.R;
   if (plan.splits > 1) {
@@ -725,33 +776,13 @@ cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cuda
     sp.O_part = static_cast<float *>(ws);
     sp.L_part = sp.O_part + o_elems;
   }
-  kernel<<<plan.grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapK, mapV, static_cast<float *>(p.buf[sO]),
-                                                                p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp,
-                                                                p.causal_offset, p.group);
+  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL],
+                                                           p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp, p.causal_offset,
+                                                           p.group);
   if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
   const uint64_t threads = rows_total * (p.D / 4);
   merge_splits<kCausal><<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(
       sp, static_cast<float *>(p.buf[sO]), p.buf[sL], p.prec[sL], rows_total, p.D);
-  return cudaGetLastError();
-}
-
-// partial accumulators of a traversal split in the workspace: [split][tensor][batch][rows][D] FP32
-static cudaError_t split_scratch(BwdArgs &a, uint32_t splits, uint32_t tensors, size_t tensor_elems, cudaStream_t stream,
-                                 float **scratch) {
-  void *ws = nullptr;
-  cudaError_t e = workspace_for(current_device(), stream, splits * tensors * tensor_elems * sizeof(float), &ws);
-  if (e != cudaSuccess) return e;
-  *scratch = static_cast<float *>(ws);
-  a.split_stride = tensors * tensor_elems;
-  return cudaSuccess;
-}
-
-static cudaError_t launch_sum(const float *scratch, float *out0, float *out1, size_t tensor_elems, uint32_t tensors,
-                              size_t split_stride, uint32_t splits, cudaStream_t stream) {
-  const size_t quads = tensor_elems / 4;  // D % 8 == 0
-  sum_splits<<<dim3(static_cast<uint32_t>((quads + 255) / 256), tensors), 256, 0, stream>>>(
-      reinterpret_cast<const float4 *>(scratch), reinterpret_cast<float4 *>(out0), reinterpret_cast<float4 *>(out1), quads,
-      split_stride / 4, splits);
   return cudaGetLastError();
 }
 
@@ -778,53 +809,37 @@ static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
   return a;
 }
 
-template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
-cudaError_t launch_query(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
-  using Cfg = QCfg<DCH>;
-  auto kernel = attention_backward_query_wgmma<DCH, kBF16, kConvertDO, kCausal>;
+// A backward kernel whose outputs are the BwdArgs fields out0 and, unless null, out1: FP32 tensors of `elems` elements
+// each.  Split: each split writes partial sums to the workspace, [split][output][elems], and sum_splits adds them into
+// the outputs.
+using OutputSlot = float *BwdArgs::*;
+template <class Cfg, class Kernel>
+static cudaError_t launch_backward(Kernel kernel, const AttentionParams &p, const WgmmaPlan &plan, OutputSlot out0,
+                                   OutputSlot out1, size_t elems, cudaStream_t stream) {
+  constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
+  const uint32_t outputs = out1 ? 2 : 1;
+  TensorMaps m;
   cudaError_t e;
-  if ((e = prepare(kernel, Cfg::kSmemBytes)) != cudaSuccess) return e;
-  CUtensorMap mapQ, mapdO, mapK, mapV;
-  if ((e = make_tensor_map_16bit(&mapQ, p.buf[sQ], p.R, p.D, p.batch, Cfg::kTileM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapdO, p.buf[sdO], p.R, p.D, p.batch, Cfg::kTileM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) return e;
+  if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, true, &m)) != cudaSuccess) return e;
   BwdArgs a = backward_args(p, plan);
-  const size_t tensor_elems = static_cast<size_t>(p.batch) * p.R * p.D;
+  float *const dst0 = a.*out0, *const dst1 = out1 ? a.*out1 : nullptr;
   float *scratch = nullptr;
   if (plan.splits > 1) {
-    if ((e = split_scratch(a, plan.splits, 1, tensor_elems, stream, &scratch)) != cudaSuccess) return e;
-    a.dQ = scratch;
+    void *ws = nullptr;
+    if ((e = workspace_for(current_device(), stream, plan.splits * outputs * elems * sizeof(float), &ws)) != cudaSuccess)
+      return e;
+    scratch = static_cast<float *>(ws);
+    a.split_stride = outputs * elems;
+    a.*out0 = scratch;
+    if (out1) a.*out1 = scratch + elems;
   }
-  kernel<<<plan.grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapdO, mapK, mapV, a);
+  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.dO, m.K, m.V, a);
   if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
-  return launch_sum(scratch, static_cast<float *>(p.buf[sdQ]), nullptr, tensor_elems, 1, a.split_stride, plan.splits,
-                    stream);
-}
-
-template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
-cudaError_t launch_key_value(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
-  using Cfg = KVCfg<DCH>;
-  auto kernel = attention_backward_key_value_wgmma<DCH, kBF16, kConvertDO, kCausal>;
-  cudaError_t e;
-  if ((e = prepare(kernel, Cfg::kSmemBytes)) != cudaSuccess) return e;
-  CUtensorMap mapQ, mapdO, mapK, mapV;
-  if ((e = make_tensor_map_16bit(&mapQ, p.buf[sQ], p.R, p.D, p.batch, Cfg::BM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapdO, p.buf[sdO], p.R, p.D, p.batch, Cfg::BM)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch / p.group, Cfg::kTileN)) != cudaSuccess) return e;
-  if ((e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch / p.group, Cfg::kTileN)) != cudaSuccess) return e;
-  BwdArgs a = backward_args(p, plan);
-  const size_t tensor_elems = static_cast<size_t>(p.batch / p.group) * p.C * p.D;  // dK / dV: one per K/V head
-  float *scratch = nullptr;
-  if (plan.splits > 1) {
-    if ((e = split_scratch(a, plan.splits, 2, tensor_elems, stream, &scratch)) != cudaSuccess) return e;
-    a.dV = scratch;
-    a.dK = scratch + tensor_elems;
-  }
-  kernel<<<plan.grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(mapQ, mapdO, mapK, mapV, a);
-  if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
-  return launch_sum(scratch, static_cast<float *>(p.buf[sdV]), static_cast<float *>(p.buf[sdK]), tensor_elems, 2,
-                    a.split_stride, plan.splits, stream);
+  const size_t quads = elems / 4;  // D % 8 == 0
+  sum_splits<<<dim3(static_cast<uint32_t>((quads + 255) / 256), outputs), 256, 0, stream>>>(
+      reinterpret_cast<const float4 *>(scratch), reinterpret_cast<float4 *>(dst0), reinterpret_cast<float4 *>(dst1), quads,
+      a.split_stride / 4, plan.splits);
+  return cudaGetLastError();
 }
 
 // Calls f(DCH, kBF16, kConvertDO, kCausal), each as a std::integral_constant, for the kernel instantiation that serves p
@@ -848,7 +863,7 @@ WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batc
   auto geometry = [&](auto cfg) {
     using Cfg = decltype(cfg);
     p.threads = Cfg::kThreads;
-    p.smem_bytes = Cfg::kSmemBytes;
+    p.smem_bytes = Cfg::Smem::kSmemBytes;
     p.par = Cfg::kPar;
     p.trav = Cfg::kTrav;
   };
@@ -908,30 +923,29 @@ cudaError_t launch_wgmma_forward(const AttentionParams &p, cudaStream_t stream) 
   });
 }
 
-static bool backward_ok(const AttentionParams &p) {
+static cudaError_t check_backward(const AttentionParams &p) {
   const bool dO_ok = p.prec[sdO] == p.prec[sQ] || (p.prec[sQ] == FP16 && p.prec[sdO] == BF16);
-  return row_major_16bit(p) && dO_ok && p.prec[sO] == FP32 && p.prec[sdQ] == FP32 && p.prec[sdK] == FP32 &&
-         p.prec[sdV] == FP32;
+  if (row_major_16bit(p) && dO_ok && p.prec[sO] == FP32 && p.prec[sdQ] == FP32 && p.prec[sdK] == FP32 &&
+      p.prec[sdV] == FP32)
+    return cudaSuccess;
+  set_launch_detail("descriptor is outside the wgmma backward kernels' domain");
+  return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_wgmma_backward_query(const AttentionParams &p, cudaStream_t stream) {
-  if (!backward_ok(p)) {
-    set_launch_detail("descriptor is outside the wgmma backward kernels' domain");
-    return cudaErrorInvalidValue;
-  }
+  if (cudaError_t e = check_backward(p)) return e;
   const bool convert = p.prec[sdO] != p.prec[sQ];
   const WgmmaPlan plan = plan_for(MFA_BACKWARD_QUERY, p, convert);
   return hop::dispatch(p, convert, [&](auto dch, auto bf16, auto cvt, auto causal) {
-    return hop::launch_query<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value,
-                             decltype(causal)::value>(p, plan, stream);
+    constexpr uint32_t DCH = decltype(dch)::value;
+    return hop::launch_backward<hop::QCfg<DCH>>(
+        hop::attention_backward_query_wgmma<DCH, decltype(bf16)::value, decltype(cvt)::value, decltype(causal)::value>, p,
+        plan, &hop::BwdArgs::dQ, nullptr, static_cast<size_t>(p.batch) * p.R * p.D, stream);
   });
 }
 
 cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream_t stream) {
-  if (!backward_ok(p)) {
-    set_launch_detail("descriptor is outside the wgmma backward kernels' domain");
-    return cudaErrorInvalidValue;
-  }
+  if (cudaError_t e = check_backward(p)) return e;
   const bool convert = p.prec[sdO] != p.prec[sQ];
   const WgmmaPlan plan = plan_for(MFA_BACKWARD_KEY_VALUE, p, convert);
   AttentionParams q = p;
@@ -945,8 +959,11 @@ cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream
     q.prec[sdO] = q.prec[sQ];
   }
   return hop::dispatch(q, convert && !plan.convert_dO_first, [&](auto dch, auto bf16, auto cvt, auto causal) {
-    return hop::launch_key_value<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value,
-                                 decltype(causal)::value>(q, plan, stream);
+    constexpr uint32_t DCH = decltype(dch)::value;
+    return hop::launch_backward<hop::KVCfg<DCH>>(
+        hop::attention_backward_key_value_wgmma<DCH, decltype(bf16)::value, decltype(cvt)::value, decltype(causal)::value>,
+        q, plan, &hop::BwdArgs::dV, &hop::BwdArgs::dK, static_cast<size_t>(q.batch / q.group) * q.C * q.D,  // per K/V head
+        stream);
   });
 }
 
