@@ -296,6 +296,50 @@ MFA_API int mfa_attention_kernel_launch_count(const mfa_attention_kernel_t *kern
                                               const mfa_function_constants_t *constants, uint32_t *out);
 
 /* ------------------------------------------------------------------------------------------ */
+/* Variable-length (packed) sequences (library extension)                                      */
+/* ------------------------------------------------------------------------------------------ */
+/** One call over `count` sequences of different lengths: FlashAttention's cu_seqlens.  Sequence s owns query rows
+ *  [row_offsets[s], row_offsets[s + 1]) and key rows [column_offsets[s], column_offsets[s + 1]) of every problem.  The
+ *  buffers keep the layout of mfa_attention_kernel_encode, each problem contiguous: Q, O, dO, dQ are [batch_count][row]
+ *  [D], L and D [batch_count][row], K, V, dK, dV [batch_count / kv_group][column][D], with row / column / batch_count /
+ *  kv_group from the function constants (a packed [T, H, D] tensor is x.transpose(0, 1).contiguous(), row = T).
+ *
+ *  Within a sequence every output is exactly attention on that sequence: O, L, D, dQ of its Rs query rows over its Cs
+ *  keys, and dK / dV summed over the query problems of each K/V group (deterministic, no atomics).  Causal is
+ *  bottom-right aligned per sequence (delta = Cs - Rs).  A row that sees no key, including every row of a sequence
+ *  with Cs = 0, gets O = 0, L = +inf, D = 0, dQ = 0; the keys of a sequence with Rs = 0 get dK = dV = 0.  Rows past
+ *  row_offsets[count] / column_offsets[count] are never written, and the attention kernels do not read them (the
+ *  staging copies of operands with head % 8 != 0 or a transposed layout, and the separate FP16 conversion of a BF16 dO,
+ *  copy whole input buffers).  Packed calls never split a tile's traversal across CTAs.  MFA_BACKEND_SIMT_FP32 takes
+ *  packed sequences with row-major operands only (MFA_ERROR_INVALID_ARGUMENT otherwise).
+ *
+ *  The offset tables are DEVICE memory, read by the kernels only (no host synchronisation; a packed encode can be
+ *  captured into a CUDA graph and replayed with new table contents).  The host checks what it can see:
+ *  MFA_ERROR_INVALID_ARGUMENT for a NULL table or offset pointer, count of 0 or above 65535 (the grid's z limit), and
+ *  max_row / max_column of 0 or above row / column.  The kernels clamp every range into [0, row] / [0, column] (an end
+ *  below its start counts as empty), so malformed contents never reach outside the caller's buffers; but a sequence
+ *  longer than max_row / max_column breaks the contract: its rows past the maximum may be left unwritten. */
+typedef struct mfa_sequence_table {
+  uint32_t count;               /* S >= 1 */
+  uint32_t max_row, max_column; /* host values >= every Rs / Cs: they size the grid */
+  const int32_t *row_offsets;   /* device, S + 1 non-decreasing entries, last <= constants.row */
+  const int32_t *column_offsets; /* device, S + 1 entries, last <= constants.column */
+} mfa_sequence_table_t;
+/** mfa_attention_kernel_encode over packed sequences. */
+MFA_API int mfa_attention_kernel_encode_sequences(const mfa_attention_kernel_t *kernel,
+                                                  const mfa_function_constants_t *constants,
+                                                  const mfa_sequence_table_t *sequences,
+                                                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
+/** Grid size of a packed call: ceil(max_row (dK/dV: max_column) / parallelization) x problems x count. */
+MFA_API int mfa_attention_kernel_grid_size_sequences(const mfa_attention_kernel_t *kernel,
+                                                     const mfa_function_constants_t *constants,
+                                                     const mfa_sequence_table_t *sequences, uint32_t *out);
+/** Kernels one packed encode launches: as mfa_attention_kernel_launch_count, never with a split merge. */
+MFA_API int mfa_attention_kernel_launch_count_sequences(const mfa_attention_kernel_t *kernel,
+                                                        const mfa_function_constants_t *constants,
+                                                        const mfa_sequence_table_t *sequences, uint32_t *out);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Kernel cache keyed by descriptor                                                            */
 /* ------------------------------------------------------------------------------------------ */
 /** The analogue of the reference's pipeline cache (GEMMKernel.register(descriptor:) / pipelineCache[descriptor],

@@ -93,6 +93,17 @@ class _CFunctionConstants(ctypes.Structure):
                 ("kv_group", ctypes.c_uint32)]
 
 
+class SequenceTable(ctypes.Structure):
+    """mfa_sequence_table_t: packed variable-length sequences (FlashAttention's cu_seqlens).  Sequence s owns query rows
+    [row_offsets[s], row_offsets[s + 1]) and key rows [column_offsets[s], column_offsets[s + 1]) of every problem; the
+    offsets are int32 DEVICE pointers with count + 1 entries, max_row / max_column bound every sequence's lengths."""
+    _fields_ = [("count", ctypes.c_uint32), ("max_row", ctypes.c_uint32), ("max_column", ctypes.c_uint32),
+                ("row_offsets", ctypes.c_void_p), ("column_offsets", ctypes.c_void_p)]
+
+    def __init__(self, count=0, max_row=0, max_column=0, row_offsets=0, column_offsets=0):
+        super().__init__(int(count), int(max_row), int(max_column), row_offsets or None, column_offsets or None)
+
+
 def _load():
     if not os.path.exists(_LIB_PATH):
         raise ImportError(
@@ -128,6 +139,13 @@ def _load():
                                                       c.POINTER(c.c_uint32)]
     lib.mfa_attention_kernel_encode.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
                                                 c.POINTER(c.c_void_p * MFA_BUFFER_COUNT), c.c_void_p]
+    lib.mfa_attention_kernel_encode_sequences.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                          c.POINTER(SequenceTable),
+                                                          c.POINTER(c.c_void_p * MFA_BUFFER_COUNT), c.c_void_p]
+    lib.mfa_attention_kernel_grid_size_sequences.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                             c.POINTER(SequenceTable), c.POINTER(c.c_uint32)]
+    lib.mfa_attention_kernel_launch_count_sequences.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                                c.POINTER(SequenceTable), c.POINTER(c.c_uint32)]
     lib.mfa_attention_kernel_cache_fetch.argtypes = [c.POINTER(_CDescriptor), c.c_int, c.POINTER(c.c_void_p)]
     lib.mfa_attention_kernel_cache_size.restype = c.c_int
     lib.mfa_attention_run_host.argtypes = [c.POINTER(_CDescriptor), c.c_uint32,
@@ -525,14 +543,23 @@ class AttentionKernel:
         _check(_lib.mfa_attention_kernel_threadgroup_memory_allocation(self._handle, ctypes.byref(out)))
         return out.value
 
-    def gridSize(self, constants: FunctionConstantValues) -> int:
+    def gridSize(self, constants: FunctionConstantValues, sequences: Optional[SequenceTable] = None) -> int:
+        """sequences: packed variable-length sequences (mfa_attention_kernel_grid_size_sequences)."""
         out = ctypes.c_uint32()
-        _check(_lib.mfa_attention_kernel_grid_size(self._handle, ctypes.byref(constants._c), ctypes.byref(out)))
+        if sequences is None:
+            _check(_lib.mfa_attention_kernel_grid_size(self._handle, ctypes.byref(constants._c), ctypes.byref(out)))
+        else:
+            _check(_lib.mfa_attention_kernel_grid_size_sequences(self._handle, ctypes.byref(constants._c),
+                                                                 ctypes.byref(sequences), ctypes.byref(out)))
         return out.value
 
-    def launchCount(self, constants: FunctionConstantValues) -> int:
+    def launchCount(self, constants: FunctionConstantValues, sequences: Optional[SequenceTable] = None) -> int:
         out = ctypes.c_uint32()
-        _check(_lib.mfa_attention_kernel_launch_count(self._handle, ctypes.byref(constants._c), ctypes.byref(out)))
+        if sequences is None:
+            _check(_lib.mfa_attention_kernel_launch_count(self._handle, ctypes.byref(constants._c), ctypes.byref(out)))
+        else:
+            _check(_lib.mfa_attention_kernel_launch_count_sequences(self._handle, ctypes.byref(constants._c),
+                                                                    ctypes.byref(sequences), ctypes.byref(out)))
         return out.value
 
     def sourceName(self) -> str:
@@ -540,20 +567,26 @@ class AttentionKernel:
         return _lib.mfa_attention_kernel_source_name(self._handle).decode()
 
     def encode(self, constants: FunctionConstantValues, buffers: Dict[AttentionOperand, int],
-               stream: int = 0) -> None:
-        """buffers: {AttentionOperand: device pointer}; stream: cudaStream_t as int (0 = default)."""
+               stream: int = 0, sequences: Optional[SequenceTable] = None) -> None:
+        """buffers: {AttentionOperand: device pointer}; stream: cudaStream_t as int (0 = default).  sequences: packed
+        variable-length sequences over the rows of every problem (mfa_attention_kernel_encode_sequences)."""
         arr = (ctypes.c_void_p * MFA_BUFFER_COUNT)()
         for op, ptr in buffers.items():
             binding = AttentionOperand(op).bufferBinding
             if binding is None:
                 raise MFAError(-2, f"Operand {AttentionOperand(op).name} has no buffer binding.")
             arr[binding] = ptr
-        _check(_lib.mfa_attention_kernel_encode(self._handle, ctypes.byref(constants._c), ctypes.byref(arr),
-                                                ctypes.c_void_p(stream)))
+        if sequences is None:
+            _check(_lib.mfa_attention_kernel_encode(self._handle, ctypes.byref(constants._c), ctypes.byref(arr),
+                                                    ctypes.c_void_p(stream)))
+        else:
+            _check(_lib.mfa_attention_kernel_encode_sequences(self._handle, ctypes.byref(constants._c),
+                                                              ctypes.byref(sequences), ctypes.byref(arr),
+                                                              ctypes.c_void_p(stream)))
 
 
 __all__ = [
     "AttentionDescriptor", "AttentionKernelDescriptor", "AttentionKernel", "AttentionKernelType",
-    "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError",
+    "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError", "SequenceTable",
     "library_path", "version", "setParameterTable", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
 ]

@@ -152,6 +152,40 @@ static int build_params(const mfa_attention_kernel *k, const mfa_function_consta
   return MFA_SUCCESS;
 }
 
+// The launch form of a packed-sequence table, after the checks the host can make without reading device memory
+constexpr uint32_t kMaxSequences = 65535;  // the grid's z limit
+static int sequences_of(const mfa_attention_kernel *k, const mfa_function_constants_t *c, const mfa_sequence_table_t *t,
+                        Sequences *out) {
+  if (!t) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL sequence table.");
+  // (the tensor-core family stages transposed operands row-major; the SIMT packed kernels read row-major operands only)
+  if (k->backend == MFA_BACKEND_SIMT_FP32) {
+    int n = 0;
+    const int *ops = operands_of(k->type, &n);
+    for (int i = 0; i < n; ++i)
+      if ((k->descriptor.transpose_state_mask >> ops[i]) & 1)
+        return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Packed sequences on MFA_BACKEND_SIMT_FP32 need row-major "
+                                                            "operands; ") +
+                                                    mfa_operand_name((mfa_operand_t)ops[i]) + " is transposed.");
+  }
+  if (!t->row_offsets || !t->column_offsets)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Sequence table: row_offsets and column_offsets must not be NULL.");
+  if (t->count == 0 || t->count > kMaxSequences)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Sequence table: count " + std::to_string(t->count) +
+                                                " is outside [1, " + std::to_string(kMaxSequences) + "].");
+  if (t->max_row == 0 || t->max_row > c->row)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Sequence table: max_row " + std::to_string(t->max_row) +
+                                                " is outside [1, row = " + std::to_string(c->row) + "].");
+  if (t->max_column == 0 || t->max_column > c->column)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Sequence table: max_column " + std::to_string(t->max_column) +
+                                                " is outside [1, column = " + std::to_string(c->column) + "].");
+  *out = Sequences{t->row_offsets, t->column_offsets, c->row, c->column, t->count, t->max_row, t->max_column};
+  return MFA_SUCCESS;
+}
+
+// encode() of problems of the full R x C shape (seq == nullptr) or of packed sequences
+static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, const Sequences *seq,
+                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
+
 }  // namespace mfa
 
 using namespace mfa;
@@ -266,20 +300,61 @@ int mfa_attention_kernel_threadgroup_memory_allocation(const mfa_attention_kerne
   return MFA_SUCCESS;
 }
 
-int mfa_attention_kernel_grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
-                                   uint32_t *out) {
-  if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+namespace mfa {
+static int grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
+                     uint32_t *out) {
   // parallelization dimension: R for forward / backwardQuery, C for backwardKeyValue
   // (AttentionKernel.swift:197-204; dispatch: SquareAttentionTest.swift:328-339)
-  // (dK/dV: one CTA per K/V tile, which walks the query problems of its group)
+  // (dK/dV: one CTA per K/V tile, which walks the query problems of its group; packed sequences: the tiles of the
+  // longest sequence, once per sequence)
   const bool key_value = kernel->type == MFA_BACKWARD_KEY_VALUE;
-  const uint32_t dim = key_value ? c->column : c->row;
+  const uint32_t dim = key_value ? (seq ? seq->max_column : c->column) : (seq ? seq->max_row : c->row);
   const uint32_t batch = c->batch_count ? c->batch_count : 1;
   uint32_t group = 1;
   const int status = kv_group_of(c, &group);
   if (status != MFA_SUCCESS) return status;
-  *out = ((dim + kernel->par - 1) / kernel->par) * (key_value ? batch / group : batch);
+  *out = ((dim + kernel->par - 1) / kernel->par) * (key_value ? batch / group : batch) * (seq ? seq->count : 1);
   return MFA_SUCCESS;
+}
+
+static int launch_count(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
+                        uint32_t *out) {
+  const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
+  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, staged = __builtin_popcount(staged_operands(kernel));
+  uint32_t group = 1;
+  const int status = kv_group_of(c, &group);
+  if (status != MFA_SUCCESS) return status;
+  const uint32_t sm_count = kernel->backend == MFA_BACKEND_TCGEN05 ? device_sm_count(current_device()) : 0;
+  const bool convert_dO = d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q];
+  *out = 0;
+  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t, uint32_t batch) -> int {
+    if (kernel->backend != MFA_BACKEND_TCGEN05)
+      *out += 1;
+    else if (seq)
+      *out += staged + wgmma_plan_sequences(kernel->type, Dp, seq->max_row, seq->max_column, seq->count, batch, group,
+                                            convert_dO, sm_count)
+                           .launches;
+    else
+      *out += staged + wgmma_plan(kernel->type, Dp, c->row, c->column, batch, group, d.split_min_blocks, d.split_max,
+                                  convert_dO, sm_count)
+                           .launches;
+    return MFA_SUCCESS;
+  });
+}
+}  // namespace mfa
+
+int mfa_attention_kernel_grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                                   uint32_t *out) {
+  if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  return grid_size(kernel, c, nullptr, out);
+}
+
+int mfa_attention_kernel_grid_size_sequences(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                                             const mfa_sequence_table_t *table, uint32_t *out) {
+  if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  Sequences seq;
+  const int status = sequences_of(kernel, c, table, &seq);
+  return status != MFA_SUCCESS ? status : grid_size(kernel, c, &seq, out);
 }
 
 const char *mfa_attention_kernel_source_name(const mfa_attention_kernel_t *kernel) {
@@ -289,26 +364,38 @@ const char *mfa_attention_kernel_source_name(const mfa_attention_kernel_t *kerne
 int mfa_attention_kernel_launch_count(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                       uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
-  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, staged = __builtin_popcount(staged_operands(kernel));
-  uint32_t group = 1;
-  const int status = kv_group_of(c, &group);
-  if (status != MFA_SUCCESS) return status;
-  const uint32_t sm_count = kernel->backend == MFA_BACKEND_TCGEN05 ? device_sm_count(current_device()) : 0;
-  *out = 0;
-  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t, uint32_t batch) -> int {
-    *out += kernel->backend != MFA_BACKEND_TCGEN05
-                ? 1
-                : staged + wgmma_plan(kernel->type, Dp, c->row, c->column, batch, group, d.split_min_blocks,
-                                      d.split_max, d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q], sm_count)
-                               .launches;
-    return MFA_SUCCESS;
-  });
+  return launch_count(kernel, c, nullptr, out);
+}
+
+int mfa_attention_kernel_launch_count_sequences(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                                                const mfa_sequence_table_t *table, uint32_t *out) {
+  if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  Sequences seq;
+  const int status = sequences_of(kernel, c, table, &seq);
+  return status != MFA_SUCCESS ? status : launch_count(kernel, c, &seq, out);
 }
 
 int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
                                 void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  return encode(kernel, constants, nullptr, buffers, cuda_stream);
+}
+
+int mfa_attention_kernel_encode_sequences(const mfa_attention_kernel_t *kernel,
+                                          const mfa_function_constants_t *constants, const mfa_sequence_table_t *table,
+                                          void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
+  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
+  Sequences seq;
+  const int status = sequences_of(kernel, constants, table, &seq);
+  return status != MFA_SUCCESS ? status : encode(kernel, constants, &seq, buffers, cuda_stream);
+}
+
+}  // extern "C"
+
+namespace mfa {
+static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, const Sequences *seq,
+                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   int status = check_device();
   if (status != MFA_SUCCESS) return status;
   AttentionParams p;
@@ -367,28 +454,38 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
     }
     if (kernel->backend == MFA_BACKEND_TCGEN05) {
       switch (kernel->type) {
-        case MFA_FORWARD: e = launch_wgmma_forward(q, stream); break;
-        case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, stream); break;
-        default: e = launch_wgmma_backward_key_value(q, stream); break;
+        case MFA_FORWARD: e = launch_wgmma_forward(q, seq, stream); break;
+        case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, seq, stream); break;
+        default: e = launch_wgmma_backward_key_value(q, seq, stream); break;
       }
     } else {
       switch (kernel->type) {
-        case MFA_FORWARD: e = launch_simt_forward(q, stream); break;
-        case MFA_BACKWARD_QUERY: e = launch_simt_backward_query(q, stream); break;
-        default: e = launch_simt_backward_key_value(q, stream); break;
+        case MFA_FORWARD: e = launch_simt_forward(q, seq, stream); break;
+        case MFA_BACKWARD_QUERY: e = launch_simt_backward_query(q, seq, stream); break;
+        default: e = launch_simt_backward_key_value(q, seq, stream); break;
       }
     }
     if (e != cudaSuccess)
       return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " failed: " + cudaGetErrorString(e) +
                                       " " + last_launch_detail());
+    // (packed sequences: only the sequences' rows, which the kernels wrote; the caller's other rows stay as they are)
     for (int slot = 0; slot < kSlots && e == cudaSuccess; ++slot)
-      if (user_out[slot])
+      if (user_out[slot] && seq)
+        e = launch_unstage_sequences(static_cast<const float *>(q.buf[slot]), static_cast<float *>(user_out[slot]),
+                                     problems_of(slot), seq_of(slot),
+                                     key_value_slot(slot) ? seq->column_offsets : seq->row_offsets, seq->count,
+                                     key_value_slot(slot) ? seq->max_column : seq->max_row, p.D, Dp,
+                                     p.transposed[slot], stream);
+      else if (user_out[slot])
         e = launch_unstage_output(static_cast<const float *>(q.buf[slot]), static_cast<float *>(user_out[slot]),
                                   problems_of(slot), seq_of(slot), p.D, Dp, p.transposed[slot], stream);
     if (e != cudaSuccess) return fail(MFA_ERROR_CUDA, std::string("copy-back of staged outputs failed: ") + cudaGetErrorString(e));
     return MFA_SUCCESS;
   });
 }
+}  // namespace mfa
+
+extern "C" {
 
 // ------------------------------------------------------------------------------------------------
 // Kernel cache keyed by descriptor -- the useful half of the reference's pipeline cache

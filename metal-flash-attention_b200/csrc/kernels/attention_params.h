@@ -34,19 +34,50 @@ struct AttentionParams {
   int32_t causal_offset;
 };
 
+// Packed variable-length sequences (mfa_sequence_table_t), a kernel argument of their own so that the fixed-length
+// kernels keep their parameter lists: sequence s owns query rows [row_offsets[s], row_offsets[s + 1]) and key rows
+// [column_offsets[s], column_offsets[s + 1]) of every problem, each range clamped into [0, rows] / [0, columns] (the
+// rows each problem's buffer holds, AttentionParams R / C).  The grid's z axis is the sequence.
+struct Sequences {
+  const int32_t *row_offsets, *column_offsets;  // device memory, count + 1 entries each
+  uint32_t rows, columns;
+  uint32_t count, max_row, max_column;  // host values: they size the grid
+};
+
+// The rows of sequence s that a kernel works on, read from the tables and clamped (kernels only)
+struct SequenceSpan {
+  uint32_t q0, R, k0, C;  // first query row and query count; first key row and key count
+};
+#ifdef __CUDACC__
+// Sequence i's rows in a table: [offsets[i], offsets[i + 1]) clamped into [0, limit], an end below its start empty
+__device__ __forceinline__ uint32_t sequence_rows(const int32_t *offsets, uint32_t i, uint32_t limit, uint32_t *first) {
+  const int lo = min(max(__ldg(offsets + i), 0), static_cast<int>(limit));
+  const int hi = min(max(__ldg(offsets + i + 1), lo), static_cast<int>(limit));
+  *first = static_cast<uint32_t>(lo);
+  return static_cast<uint32_t>(hi - lo);
+}
+__device__ __forceinline__ SequenceSpan sequence_span(const Sequences &s, uint32_t i) {
+  SequenceSpan r;
+  r.R = sequence_rows(s.row_offsets, i, s.rows, &r.q0);
+  r.C = sequence_rows(s.column_offsets, i, s.columns, &r.k0);
+  return r;
+}
+#endif
+
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
-cudaError_t launch_simt_forward(const AttentionParams &p, cudaStream_t stream);
-cudaError_t launch_simt_backward_query(const AttentionParams &p, cudaStream_t stream);
-cudaError_t launch_simt_backward_key_value(const AttentionParams &p, cudaStream_t stream);
+// seq: packed sequences, or nullptr for problems of the full R x C shape
+cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
+cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
+cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
 void simt_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
                    uint32_t *head);
 
 // ---- tensor-core family (wgmma_attention.cu; the backend keeps its historical name "tcgen05" in the ABI) --------
 // 16-bit row-major operands with D % 8 == 0 and D <= kWgmmaMaxHead; kernel.cpp stages every other layout into that form.
 constexpr uint32_t kWgmmaMaxHead = 256;
-cudaError_t launch_wgmma_forward(const AttentionParams &p, cudaStream_t stream);
-cudaError_t launch_wgmma_backward_query(const AttentionParams &p, cudaStream_t stream);
-cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream_t stream);
+cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
+cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
+cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
 
 // How the launcher of kernel `type` (mfa_kernel_type_t) runs one problem of padded head dimension D; every field is
 // derived from the kernels' compile-time configurations.  R, C and batch do not affect the geometry fields.
@@ -62,6 +93,10 @@ struct WgmmaPlan {
 // depends on it)
 WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
                      uint32_t max_splits, bool convert_dO, uint32_t sm_count);
+// The plan of a packed call over `count` sequences of at most max_row x max_column: never split, grid (tiles of the
+// longest sequence, heads, count); the dO-conversion choice counts every CTA of that grid
+WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t max_column, uint32_t count,
+                               uint32_t batch, uint32_t group, bool convert_dO, uint32_t sm_count);
 
 // operand staging for the tensor-core family (pad_head.cu): a [batch][seq][D] (or, transposed, [batch][D][seq]) operand
 // is copied to row-major [batch][seq][Dp] with zero padding columns, and an FP32 output computed in that form is copied
@@ -70,6 +105,11 @@ cudaError_t launch_stage_operand(const void *src, void *dst, uint32_t batch, uin
                                  uint32_t element_bytes, bool transposed, cudaStream_t stream);
 cudaError_t launch_unstage_output(const float *src, float *dst, uint32_t batch, uint32_t seq, uint32_t D, uint32_t Dp,
                                   bool transposed, cudaStream_t stream);
+// packed sequences: only rows [0, min(length, limit)) of each of the `count` sequences of `offsets` (the rows the
+// attention kernels wrote), so that rows outside every sequence keep the caller's contents
+cudaError_t launch_unstage_sequences(const float *src, float *dst, uint32_t batch, uint32_t seq, const int32_t *offsets,
+                                     uint32_t count, uint32_t limit, uint32_t D, uint32_t Dp, bool transposed,
+                                     cudaStream_t stream);
 cudaError_t launch_bf16_to_f16(const void *src, void *dst, uint64_t elements, cudaStream_t stream);
 const char *last_launch_detail();  // thread-local detail string for MFA_ERROR_CUDA messages
 

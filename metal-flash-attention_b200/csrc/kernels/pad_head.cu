@@ -46,6 +46,19 @@ __global__ void __launch_bounds__(256) unstage_output(const float *__restrict__ 
   dst[i] = src[(b * seq + s) * Dp + c];
 }
 
+// Packed sequences: unstage_output of only the rows the attention kernels wrote, rows [0, min(length, limit)) of
+// sequence blockIdx.z (its range in `offsets`, clamped into [0, seq] as the kernels clamp it) of problem blockIdx.y
+__global__ void __launch_bounds__(256) unstage_sequences(const float *__restrict__ src, float *__restrict__ dst,
+                                                         const int32_t *__restrict__ offsets, uint32_t seq,
+                                                         uint32_t limit, uint32_t D, uint32_t Dp, bool transposed) {
+  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  uint32_t first;
+  const uint32_t rows = min(sequence_rows(offsets, blockIdx.z, seq, &first), limit);
+  if (i >= static_cast<uint64_t>(rows) * D) return;
+  const uint64_t b = blockIdx.y, s = first + i / D, c = i % D;
+  dst[transposed ? (b * D + c) * seq + s : (b * seq + s) * D + c] = src[(b * seq + s) * Dp + c];
+}
+
 // dO (BF16) -> FP16, eight elements per thread; exact for 2^-14 <= |x| < 65504 (backward_common.cuh)
 __global__ void __launch_bounds__(256) bf16_to_f16(const uint4 *__restrict__ src, uint4 *__restrict__ dst, uint64_t vectors) {
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -78,6 +91,15 @@ cudaError_t launch_unstage_output(const float *src, float *dst, uint32_t batch, 
                                   bool transposed, cudaStream_t stream) {
   const uint64_t n = static_cast<uint64_t>(batch) * seq * D;
   unstage_output<<<static_cast<uint32_t>((n + 255) / 256), 256, 0, stream>>>(src, dst, seq, D, Dp, n, transposed);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_unstage_sequences(const float *src, float *dst, uint32_t batch, uint32_t seq, const int32_t *offsets,
+                                     uint32_t count, uint32_t limit, uint32_t D, uint32_t Dp, bool transposed,
+                                     cudaStream_t stream) {
+  const uint64_t n = static_cast<uint64_t>(limit) * D;
+  unstage_sequences<<<dim3(static_cast<uint32_t>((n + 255) / 256), batch, count), 256, 0, stream>>>(
+      src, dst, offsets, seq, limit, D, Dp, transposed);
   return cudaGetLastError();
 }
 

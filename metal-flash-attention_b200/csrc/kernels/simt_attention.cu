@@ -236,6 +236,7 @@ __device__ __forceinline__ void store_acc(const float (&acc)[NCH][4][4], const f
 // ------------------------------------------------------------------------------------------------
 // forward: O = softmax(Q K^T / sqrt(D)) V,  L = log2(e) * logsumexp          (one CTA per 64 rows)
 // ------------------------------------------------------------------------------------------------
+// (packed sequences: simt_forward_kernel_varlen, below, is this kernel's twin)
 template <int NCH>
 __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const AttentionParams p) {
   extern __shared__ __align__(16) float smem[];
@@ -324,6 +325,7 @@ __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const Attenti
 // ------------------------------------------------------------------------------------------------
 // backward dQ: D = rowsum(dO * O)/sqrt(D);  dQ = sum_c P (dP/sqrt(D) - D) K     (one CTA per 64 rows)
 // ------------------------------------------------------------------------------------------------
+// (packed sequences: simt_backward_query_kernel_varlen, below, is this kernel's twin)
 template <int NCH>
 __global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const AttentionParams p) {
   extern __shared__ __align__(16) float smem[];
@@ -386,6 +388,7 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const 
 // backward dK/dV: dV = sum_r P^T dO;  dK = sum_r dS^T Q      (one CTA per 64 columns x D-slice)
 // Grouped K/V: blockIdx.y covers K/V heads, and the sums run over the rows of every query head of the group.
 // ------------------------------------------------------------------------------------------------
+// (packed sequences: simt_backward_key_value_kernel_varlen, below, is this kernel's twin)
 template <int NCH>
 __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(const AttentionParams p,
                                                                                uint32_t dSlices) {
@@ -452,6 +455,248 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(co
   store_acc<NCH>(accK, one, p, sdK, p.C, kvb, c0, dlo, dhi, tx, ty);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Packed sequences (Sequences): the same three kernels on sequence blockIdx.z of every problem, with its span in place
+// of R, C and the causal offset.  Kernels of their own rather than a template flag on the ones above, which keeps those
+// instruction for instruction as they were.  Row-major operands only (a transposed operand's leading dimension is the
+// whole buffer, which Operand does not carry; kernel.cpp rejects them).  A change to a kernel above needs the same
+// change in its twin here.  Rows past a sequence's end read as zeros (Operand::seq).
+// ------------------------------------------------------------------------------------------------
+struct Span {
+  SequenceSpan s;
+  int offset;  // causal: row r sees column c iff c <= r + offset (Cs - Rs)
+};
+__device__ __forceinline__ Span span_of(const Sequences &seq) {
+  Span sp;
+  sp.s = sequence_span(seq, blockIdx.z);
+  sp.offset = static_cast<int>(sp.s.C) - static_cast<int>(sp.s.R);
+  return sp;
+}
+// rows [first, first + len) of problem b of `slot`, whose buffer holds `rows` rows per problem
+__device__ __forceinline__ Operand span_operand(const AttentionParams &p, int slot, uint32_t rows, uint32_t b,
+                                                uint32_t first, uint32_t len) {
+  Operand op = make_operand(p, slot, rows, b);
+  op.ptr = static_cast<const char *>(op.ptr) + static_cast<size_t>(first) * p.D * (p.prec[slot] == FP32 ? 4 : 2);
+  op.seq = len;
+  return op;
+}
+__device__ __forceinline__ Operand span_query(const AttentionParams &p, int slot, uint32_t b, const Span &sp) {
+  return span_operand(p, slot, p.R, b, sp.s.q0, sp.s.R);
+}
+__device__ __forceinline__ Operand span_key(const AttentionParams &p, int slot, uint32_t kv, const Span &sp) {
+  return span_operand(p, slot, p.C, kv, sp.s.k0, sp.s.C);
+}
+__device__ __forceinline__ char *span_stats(const AttentionParams &p, int slot, uint32_t b, const Span &sp) {
+  return stat_row(p, slot, b) + static_cast<size_t>(sp.s.q0) * (p.prec[slot] == FP32 ? 4 : 2);
+}
+__device__ __forceinline__ uint32_t span_visible_columns(const AttentionParams &p, const Span &sp, uint32_t r0) {
+  if (!p.causal) return sp.s.C;
+  const int last = static_cast<int>(min(r0 + kBlock, sp.s.R)) - 1 + sp.offset;
+  return last < 0 ? 0u : min(sp.s.C, static_cast<uint32_t>(last) + 1);
+}
+__device__ __forceinline__ bool span_masked(const AttentionParams &p, const Span &sp, uint32_t r, uint32_t c) {
+  return c >= sp.s.C || (p.causal && static_cast<int>(c) > static_cast<int>(r) + sp.offset);
+}
+// store_acc to the rows [0, op.seq) of `op`
+template <int NCH>
+__device__ __forceinline__ void span_store(const float (&acc)[NCH][4][4], const float (&rowScale)[4], const Operand &op,
+                                           uint32_t s0, uint32_t dlo, uint32_t dhi, int tx, int ty) {
+  void *dst = const_cast<void *>(op.ptr);
+#pragma unroll
+  for (int q = 0; q < NCH; ++q)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint32_t s = s0 + ty + 16 * i;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const uint32_t d = dlo + q * kBlock + 4 * tx + jj;
+        if (s < op.seq && d < dhi) store_elem(dst, elem_index(op, s, d), op.prec, acc[q][i][jj] * rowScale[i]);
+      }
+    }
+}
+template <int NCH>
+__device__ __forceinline__ void zero_acc(float (&acc)[NCH][4][4]) {
+#pragma unroll
+  for (int q = 0; q < NCH; ++q)
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] = 0.f;
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel_varlen(const AttentionParams p, const Sequences seq) {
+  extern __shared__ __align__(16) float smem[];
+  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
+  const Span sp = span_of(seq);
+  if (r0 >= sp.s.R) return;  // a tile past the sequence's end
+  const Operand Q = span_query(p, sQ, b, sp), K = span_key(p, sK, b / p.group, sp), V = span_key(p, sV, b / p.group, sp);
+  float m[4], l[4], acc[NCH][4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    m[i] = -FLT_MAX;
+    l[i] = FLT_TRUE_MIN;
+  }
+  zero_acc(acc);
+  const uint32_t cend = span_visible_columns(p, sp, r0);
+  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
+    float s[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
+    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float mx = -FLT_MAX;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (span_masked(p, sp, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
+        mx = fmaxf(mx, s[i][j]);
+      }
+      mx = row_max16(mx);
+      const float m_new = fmaxf(m[i], mx * p.scale_log2), correction = exp2f(m[i] - m_new);
+      float sum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float pv = exp2f(fmaf(s[i][j], p.scale_log2, -m_new));
+        sum += pv;
+        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv;
+      }
+      l[i] = fmaf(l[i], correction, row_sum16(sum));
+      m[i] = m_new;
+#pragma unroll
+      for (int q = 0; q < NCH; ++q)
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] *= correction;
+    }
+    accumulate<NCH>(acc, sP, V, c0, 0, p.D, sX, tid, tx, ty);
+  }
+  // a row that sees no key (causal, or a sequence without keys) gets O = 0 and L = +inf
+  float inv[4];
+  bool empty[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    empty[i] = sp.s.C == 0 || (p.causal && static_cast<int>(r0 + ty + 16 * i) + sp.offset < 0);
+    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
+  }
+  span_store<NCH>(acc, inv, span_query(p, sO, b, sp), r0, 0, p.D, tx, ty);
+  if (tx == 0 && p.buf[sL] != nullptr) {
+    char *Lbase = span_stats(p, sL, b, sp);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint32_t r = r0 + ty + 16 * i;
+      if (r < sp.s.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
+    }
+  }
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel_varlen(const AttentionParams p,
+                                                                                 const Sequences seq) {
+  extern __shared__ __align__(16) float smem[];
+  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
+  const Span sp = span_of(seq);
+  if (r0 >= sp.s.R) return;
+  const Operand Q = span_query(p, sQ, b, sp), K = span_key(p, sK, b / p.group, sp), V = span_key(p, sV, b / p.group, sp);
+  const Operand O = span_query(p, sO, b, sp), dO = span_query(p, sdO, b, sp);
+  const char *Lbase = span_stats(p, sL, b, sp);
+  char *Dbase = span_stats(p, sD, b, sp);
+  float Lrow[4], Drow[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t r = min(r0 + ty + 16 * i, sp.s.R - 1);
+    float part = 0.f;
+    for (uint32_t d = tx; d < p.D; d += 16)
+      part = fmaf(load_elem(dO.ptr, elem_index(dO, r, d), dO.prec), load_elem(O.ptr, elem_index(O, r, d), O.prec), part);
+    Drow[i] = row_sum16(part) * p.scale;
+    Lrow[i] = load_elem(Lbase, r, p.prec[sL]);
+    if (tx == 0 && r0 + ty + 16 * i < sp.s.R) store_elem(Dbase, r, p.prec[sD], Drow[i]);
+  }
+  float acc[NCH][4][4];
+  zero_acc(acc);
+  const uint32_t cend = span_visible_columns(p, sp, r0);
+  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
+    float s[4][4], dp[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
+    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
+    gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float pv = !span_masked(p, sp, r0 + ty + 16 * i, c0 + tx + 16 * j)
+                             ? exp2f(fmaf(s[i][j], p.scale_log2, -Lrow[i]))
+                             : 0.f;
+        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv * fmaf(dp[i][j], p.scale, -Drow[i]);
+      }
+    accumulate<NCH>(acc, sP, K, c0, 0, p.D, sX, tid, tx, ty);
+  }
+  const float one[4] = {1.f, 1.f, 1.f, 1.f};
+  span_store<NCH>(acc, one, span_query(p, sdQ, b, sp), r0, 0, p.D, tx, ty);
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel_varlen(const AttentionParams p,
+                                                                                      uint32_t dSlices,
+                                                                                      const Sequences seq) {
+  extern __shared__ __align__(16) float smem[];
+  float *sA = smem, *sB = sA + kBlock * kLDA, *sPT = sB + kBlock * kLDA, *sX = sPT + kBlock * kLDP;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const uint32_t kvb = blockIdx.y / dSlices, slice = blockIdx.y % dSlices, c0 = blockIdx.x * kBlock;
+  const uint32_t dlo = slice * (NCH * kBlock), dhi = min(p.D, dlo + NCH * kBlock);
+  const Span sp = span_of(seq);
+  if (c0 >= sp.s.C) return;  // (keys of a sequence without queries still store their zeros)
+  const Operand K = span_key(p, sK, kvb, sp), V = span_key(p, sV, kvb, sp);
+  float accV[NCH][4][4], accK[NCH][4][4];
+  zero_acc(accV);
+  zero_acc(accK);
+  const int first = static_cast<int>(c0) - sp.offset;
+  const uint32_t rstart = p.causal && first > 0 ? static_cast<uint32_t>(first) / kBlock * kBlock : 0;
+  for (uint32_t b = kvb * p.group; b < (kvb + 1) * p.group; ++b) {
+    const Operand Q = span_query(p, sQ, b, sp), dO = span_query(p, sdO, b, sp);
+    const char *Lbase = span_stats(p, sL, b, sp), *Dbase = span_stats(p, sD, b, sp);
+    for (uint32_t r0 = rstart; r0 < sp.s.R; r0 += kBlock) {
+      float s[4][4], dp[4][4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
+      gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
+      gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint32_t r = r0 + ty + 16 * i, rc = min(r, sp.s.R - 1);
+        const float Lr = load_elem(Lbase, rc, p.prec[sL]), Dr = load_elem(Dbase, rc, p.prec[sD]);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float e = r < sp.s.R && !span_masked(p, sp, r, c0 + tx + 16 * j)
+                              ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr))
+                              : 0.f;
+          dp[i][j] = e * fmaf(dp[i][j], p.scale, -Dr);  // dS
+          sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = e;  // P^T
+        }
+      }
+      accumulate<NCH>(accV, sPT, dO, r0, dlo, dhi, sX, tid, tx, ty);  // dV += P^T dO
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = dp[i][j];  // dS^T
+      accumulate<NCH>(accK, sPT, Q, r0, dlo, dhi, sX, tid, tx, ty);  // dK += dS^T Q
+    }
+  }
+  const float one[4] = {1.f, 1.f, 1.f, 1.f};
+  span_store<NCH>(accV, one, span_key(p, sdV, kvb, sp), c0, dlo, dhi, tx, ty);
+  span_store<NCH>(accK, one, span_key(p, sdK, kvb, sp), c0, dlo, dhi, tx, ty);
+}
+
 inline int chunks_for(uint32_t D) { return (D + kBlock - 1) / kBlock; }
 
 // Calls f(std::integral_constant<int, NCH>()) for the fewest of 1 / 2 / 4 / 8 (at most kMax) column chunks per CTA
@@ -480,28 +725,40 @@ cudaError_t launch(Kernel kernel, dim3 grid, cudaStream_t stream, const Args &..
 
 }  // namespace simt
 
-cudaError_t launch_simt_forward(const AttentionParams &p, cudaStream_t stream) {
-  dim3 grid((p.R + simt::kBlock - 1) / simt::kBlock, p.batch);
+// Packed sequences (seq): the grid's x axis covers the longest sequence and its z axis the sequences (row-major
+// operands: kernel.cpp rejects transposed ones)
+static dim3 simt_grid(uint32_t rows, uint32_t y, const Sequences *seq) {
+  return dim3((rows + simt::kBlock - 1) / simt::kBlock, y, seq ? seq->count : 1);
+}
+
+cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
+  const dim3 grid = simt_grid(seq ? seq->max_row : p.R, p.batch, seq);
   return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
-    return simt::launch(simt::simt_forward_kernel<decltype(nch)::value>, grid, stream, p);
+    constexpr int NCH = decltype(nch)::value;
+    if (seq) return simt::launch(simt::simt_forward_kernel_varlen<NCH>, grid, stream, p, *seq);
+    return simt::launch(simt::simt_forward_kernel<NCH>, grid, stream, p);
   });
 }
 
-cudaError_t launch_simt_backward_query(const AttentionParams &p, cudaStream_t stream) {
-  dim3 grid((p.R + simt::kBlock - 1) / simt::kBlock, p.batch);
+cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
+  const dim3 grid = simt_grid(seq ? seq->max_row : p.R, p.batch, seq);
   return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
-    return simt::launch(simt::simt_backward_query_kernel<decltype(nch)::value>, grid, stream, p);
+    constexpr int NCH = decltype(nch)::value;
+    if (seq) return simt::launch(simt::simt_backward_query_kernel_varlen<NCH>, grid, stream, p, *seq);
+    return simt::launch(simt::simt_backward_query_kernel<NCH>, grid, stream, p);
   });
 }
 
-cudaError_t launch_simt_backward_key_value(const AttentionParams &p, cudaStream_t stream) {
+cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
   // two accumulators (dV, dK) per thread: keep at most 4 chunks (256 columns) of each in registers and
   // slice larger head dimensions over blockIdx.y (each slice recomputes S and dP).
   const int chunks = simt::chunks_for(p.D);
   return simt::with_chunks<4>(chunks, [&](auto nch) {
     constexpr int NCH = decltype(nch)::value;
     const uint32_t dSlices = (chunks + NCH - 1) / NCH;
-    dim3 grid((p.C + simt::kBlock - 1) / simt::kBlock, p.batch / p.group * dSlices);  // one CTA row per K/V head
+    // one CTA row per K/V head
+    const dim3 grid = simt_grid(seq ? seq->max_column : p.C, p.batch / p.group * dSlices, seq);
+    if (seq) return simt::launch(simt::simt_backward_key_value_kernel_varlen<NCH>, grid, stream, p, dSlices, *seq);
     return simt::launch(simt::simt_backward_key_value_kernel<NCH>, grid, stream, p, dSlices);
   });
 }

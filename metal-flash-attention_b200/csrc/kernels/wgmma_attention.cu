@@ -23,6 +23,10 @@
 // Grouped K/V (`group` query heads per K/V head, a launch-time value): forward and dQ read K/V head head / group; the
 // dK/dV grid's y axis is K/V heads, and a CTA walks the query blocks of every query head of its group, so dK and dV
 // are the group sums, accumulated in registers without atomics.
+//
+// Packed sequences (the packed_* entry points, kVarlen in the shared bodies): grid.z is the sequence; a CTA takes its
+// sequence's rows from the offset tables, leaves when its tile starts past the sequence's end, works on the sequence's
+// R, C and delta, and zeroes the rows of its last streamed block that belong to the next sequence.  Never split.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -161,6 +165,18 @@ __device__ __forceinline__ void zero(float (&d)[N]) {
   for (int i = 0; i < N; ++i) d[i] = 0.f;
 }
 
+// Packed sequences: rows [first, ROWS) of a streamed DCH-chunk tile lie past the sequence's end, so TMA filled them with
+// the next sequence's rows.  Zeroes them (each row is one 128-byte line of every chunk, whatever the swizzle): a masked
+// product is 0 x x, which is NaN when x is not finite.  The caller fences and synchronises, as for the dO conversion.
+template <uint32_t DCH, uint32_t ROWS, uint32_t kThreads>
+__device__ __forceinline__ void zero_rows(uint8_t *tile, uint32_t first) {
+  const uint32_t units = (ROWS - first) * 8;  // 16-byte units per chunk
+  for (uint32_t i = threadIdx.x; i < DCH * units; i += kThreads) {
+    const uint32_t c = i / units;
+    reinterpret_cast<uint4 *>(tile + c * ROWS * 128 + first * 128)[i - c * units] = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
 // FP32 accumulator rows -> global [rows][D] (row-major), columns < D, rows < limit
 template <int NR>
 __device__ __forceinline__ void store_acc(const float (&acc)[NR], float *out, uint32_t row0, uint32_t limit, uint32_t col0,
@@ -291,12 +307,13 @@ struct FwdCfg {
   using Smem = SmemLayout<kQBytes, kKVBytes>;  // resident Q; stage: K, V
 };
 
-template <uint32_t DCH, bool kBF16, bool kCausal>
-__global__ void __launch_bounds__(2 * kWG, 1)
-    attention_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                            const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                            uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp,
-                            int delta, uint32_t group) {
+// The body of the forward kernels.  R, C: the rows of each problem's buffers.  kVarlen (packed sequences): the CTA works
+// on sequence blockIdx.z, whose span replaces R, C and delta in the ranges and masks and offsets every row; never split.
+template <uint32_t DCH, bool kBF16, bool kCausal, bool kVarlen>
+__device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUtensorMap &mapK, const CUtensorMap &mapV,
+                                             float *__restrict__ O, void *__restrict__ L, uint32_t R, uint32_t C,
+                                             uint32_t D, float scale_log2, int l_prec, const SplitArgs &sp, int delta,
+                                             uint32_t group, const Sequences &seq) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -305,12 +322,23 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   // (causal: unlike dQ, the forward gains nothing measurable from starting the tiles with the most key blocks first)
   const uint32_t head = blockIdx.y, row_base = blockIdx.x * Cfg::kTileM;
   const uint32_t kv_head = head / group;  // grouped K/V: the query heads of a group read one K/V head
-  const uint32_t kb0 = blockIdx.z * sp.blocks_per_split;
-  const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, R, C, delta, kb0, sp.blocks_per_split);
+  SequenceSpan span{0, R, 0, C};
+  uint32_t kb0, per_split;
+  if constexpr (kVarlen) {
+    span = sequence_span(seq, blockIdx.z);
+    if (row_base >= span.R) return;  // a tile past the sequence's end
+    delta = static_cast<int>(span.C) - static_cast<int>(span.R);
+    kb0 = 0;
+    per_split = (span.C + BN - 1) / BN;
+  } else {
+    kb0 = blockIdx.z * sp.blocks_per_split;
+    per_split = sp.blocks_per_split;
+  }
+  const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, span.R, span.C, delta, kb0, per_split);
 
   auto load_kv = [&](uint32_t j, uint8_t *dst, uint64_t *bar) {
-    load_tile<DCH, BN>(dst, &mapK, bar, (kb0 + j) * BN, kv_head);
-    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, bar, (kb0 + j) * BN, kv_head);
+    load_tile<DCH, BN>(dst, &mapK, bar, span.k0 + (kb0 + j) * BN, kv_head);
+    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, bar, span.k0 + (kb0 + j) * BN, kv_head);
   };
   if (tid == 0) {
     prefetch_tensormap(&mapQ);
@@ -318,8 +346,9 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     prefetch_tensormap(&mapV);
   }
   ring.init();
-  ring.start([&](uint8_t *dst, uint64_t *bar) { load_tile<DCH, Cfg::kTileM>(dst, &mapQ, bar, row_base, head); }, blocks,
-             load_kv);
+  ring.start(
+      [&](uint8_t *dst, uint64_t *bar) { load_tile<DCH, Cfg::kTileM>(dst, &mapQ, bar, span.q0 + row_base, head); },
+      blocks, load_kv);
 
   const uint32_t sQ = smem_u32(ring.base);
   float o[NO / 2];
@@ -328,6 +357,12 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   ring.wait_resident();
   for (uint32_t j = 0; j < blocks; ++j) {
     ring.wait(j);
+    if (kVarlen && (j + 1) * BN > span.C) {  // the sequence's last key block: the next sequence's keys and values
+      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j), span.C - j * BN);
+      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, span.C - j * BN);
+      fence_proxy_async_smem();
+      __syncthreads();
+    }
     const uint32_t sK = smem_u32(ring.stage(j)), sV = sK + Cfg::kKVBytes;
     float sc[BN / 2];
     zero(sc);
@@ -338,7 +373,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     fence_regs(sc);
 
     // keys past C: -inf before the row max
-    if ((kb0 + j + 1) * BN > C) mask_past_edge(sc, (kb0 + j) * BN, C);
+    if ((kb0 + j + 1) * BN > span.C) mask_past_edge(sc, (kb0 + j) * BN, span.C);
     if constexpr (kCausal) {
       const int key0 = static_cast<int>((kb0 + j) * BN);
       if (crosses_diagonal(key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base), delta))
@@ -405,19 +440,41 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   const uint32_t row0 = row_base + wg * kRows;
   // unsplit: O and L straight to the caller; split: the normalised partial of this key range
   const size_t slice = static_cast<size_t>(blockIdx.z) * sp.batch + head;
-  float *Oout = sp.splits == 1 ? O + static_cast<size_t>(head) * R * D : sp.O_part + slice * R * D;
-  // causal: a row that saw no key (l = 0) gets O = 0 and L = +inf, or L = -inf (weight 0 in the merge) as a split partial
-  const bool empty0 = kCausal && l0 == 0.f, empty1 = kCausal && l1 == 0.f;
-  store_acc(o, Oout, row0, R, 0, D, empty0 ? 0.f : 1.0f / l0, empty1 ? 0.f : 1.0f / l1);
+  float *Oout = sp.splits == 1 ? O + (static_cast<size_t>(head) * R + span.q0) * D : sp.O_part + slice * R * D;
+  // causal, or a sequence without keys: a row that saw no key (l = 0) gets O = 0 and L = +inf, or L = -inf (weight 0 in
+  // the merge) as a split partial
+  const bool empty0 = (kCausal || kVarlen) && l0 == 0.f, empty1 = (kCausal || kVarlen) && l1 == 0.f;
+  store_acc(o, Oout, row0, span.R, 0, D, empty0 ? 0.f : 1.0f / l0, empty1 ? 0.f : 1.0f / l1);
   if (t % 4 == 0) {
     const uint32_t r = row0 + frag_row(t);
     void *Lout = sp.splits == 1 ? L : sp.L_part;
     const int prec = sp.splits == 1 ? l_prec : FP32;
-    const size_t hb = (sp.splits == 1 ? static_cast<size_t>(head) : slice) * R;
+    const size_t hb = (sp.splits == 1 ? static_cast<size_t>(head) : slice) * R + span.q0;
     const float none = sp.splits == 1 ? INFINITY : -INFINITY;
-    if (r < R) store_stat(Lout, hb + r, prec, empty0 ? none : m0 + log2f(l0));
-    if (r + 8 < R) store_stat(Lout, hb + r + 8, prec, empty1 ? none : m1 + log2f(l1));
+    if (r < span.R) store_stat(Lout, hb + r, prec, empty0 ? none : m0 + log2f(l0));
+    if (r + 8 < span.R) store_stat(Lout, hb + r + 8, prec, empty1 ? none : m1 + log2f(l1));
   }
+}
+
+template <uint32_t DCH, bool kBF16, bool kCausal>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    attention_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                            const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
+                            uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp,
+                            int delta, uint32_t group) {
+  forward_body<DCH, kBF16, kCausal, false>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, sp, delta, group,
+                                           Sequences{});
+}
+
+// Packed sequences: grid (tiles of the longest sequence, heads, sequences)
+template <uint32_t DCH, bool kBF16, bool kCausal>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    packed_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                   const __grid_constant__ CUtensorMap mapV, float *__restrict__ O,
+                                   void *__restrict__ L, uint32_t R, uint32_t C, uint32_t D, float scale_log2,
+                                   int l_prec, uint32_t group, const Sequences seq) {
+  const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
+  forward_body<DCH, kBF16, kCausal, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, unsplit, 0, group, seq);
 }
 
 // ================================================================================================ backward dQ
@@ -445,11 +502,11 @@ struct BwdArgs {
   uint32_t group;  // query heads per K/V head: query head h reads K/V head h / group
 };
 
-template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
-__global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
-    attention_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
-                                   const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
-                                   const BwdArgs a) {
+// The body of the dQ kernels; kVarlen as in forward_body
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal, bool kVarlen>
+__device__ __forceinline__ void backward_query_body(const CUtensorMap &mapQ, const CUtensorMap &mapdO,
+                                                    const CUtensorMap &mapK, const CUtensorMap &mapV, const BwdArgs &a,
+                                                    const Sequences &seq) {
   using Cfg = QCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -458,18 +515,30 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   // causal: tiles in reverse order, so that the ones with the most key blocks start first and the wave tail is short
   const uint32_t tile = kCausal ? gridDim.x - 1 - blockIdx.x : blockIdx.x;
   const uint32_t head = blockIdx.y, row_base = tile * Cfg::kTileM, kv_head = head / a.group;
-  const uint32_t kb0 = blockIdx.z * a.blocks_per_split;
-  const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, a.R, a.C, a.delta, kb0, a.blocks_per_split);
+  SequenceSpan span{0, a.R, 0, a.C};
+  int delta = a.delta;
+  uint32_t kb0, per_split;
+  if constexpr (kVarlen) {
+    span = sequence_span(seq, blockIdx.z);
+    if (row_base >= span.R) return;
+    delta = static_cast<int>(span.C) - static_cast<int>(span.R);
+    kb0 = 0;
+    per_split = (span.C + BN - 1) / BN;
+  } else {
+    kb0 = blockIdx.z * a.blocks_per_split;
+    per_split = a.blocks_per_split;
+  }
+  const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, span.R, span.C, delta, kb0, per_split);
 
   auto load_kv = [&](uint32_t j, uint8_t *dst, uint64_t *bar) {
-    load_tile<DCH, BN>(dst, &mapK, bar, (kb0 + j) * BN, kv_head);
-    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, bar, (kb0 + j) * BN, kv_head);
+    load_tile<DCH, BN>(dst, &mapK, bar, span.k0 + (kb0 + j) * BN, kv_head);
+    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, bar, span.k0 + (kb0 + j) * BN, kv_head);
   };
   ring.init();
   ring.start(
       [&](uint8_t *dst, uint64_t *bar) {
-        load_tile<DCH, Cfg::kTileM>(dst, &mapQ, bar, row_base, head);
-        load_tile<DCH, Cfg::kTileM>(dst + Cfg::kQBytes, &mapdO, bar, row_base, head);
+        load_tile<DCH, Cfg::kTileM>(dst, &mapQ, bar, span.q0 + row_base, head);
+        load_tile<DCH, Cfg::kTileM>(dst + Cfg::kQBytes, &mapdO, bar, span.q0 + row_base, head);
       },
       blocks, load_kv);
 
@@ -477,11 +546,11 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   // tiles are in flight; stored for the dK/dV kernel, kept in FP32 here
   const uint32_t row0 = row_base + wg * kRows;
   const uint32_t r = row0 + frag_row(t);
-  const size_t hb = static_cast<size_t>(head) * a.R;
+  const size_t hb = static_cast<size_t>(head) * a.R + span.q0;
   float Dr[2], Lr[2];
 #pragma unroll
   for (uint32_t h = 0; h < 2; ++h) {
-    const uint32_t rc = min(r + 8 * h, a.R - 1);
+    const uint32_t rc = min(r + 8 * h, span.R - 1);
     const float *Orow = a.O + (hb + rc) * a.D;
     const size_t drow = (hb + rc) * a.D;
     float part = 0.f;
@@ -494,7 +563,8 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     part += __shfl_xor_sync(0xffffffffu, part, 2);
     Dr[h] = part * a.scale;
     Lr[h] = load_stat(a.L, hb + rc, a.l_prec);
-    if (t % 4 == 0 && r + 8 * h < a.R && blockIdx.z == 0) store_stat(a.Dterm, hb + r + 8 * h, a.d_prec, Dr[h]);
+    if (t % 4 == 0 && r + 8 * h < span.R && (kVarlen || blockIdx.z == 0))
+      store_stat(a.Dterm, hb + r + 8 * h, a.d_prec, Dr[h]);
   }
 
   const uint32_t sQ = smem_u32(ring.base), sdO = sQ + Cfg::kQBytes;
@@ -511,6 +581,12 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   zero(dq);
   for (uint32_t j = 0; j < blocks; ++j) {
     ring.wait(j);
+    if (kVarlen && (j + 1) * BN > span.C) {  // the sequence's last key block: the next sequence's keys and values
+      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j), span.C - j * BN);
+      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, span.C - j * BN);
+      fence_proxy_async_smem();
+      __syncthreads();
+    }
     const uint32_t sK = smem_u32(ring.stage(j)), sV = sK + Cfg::kKVBytes;
     float sc[BN / 2], dp[BN / 2];
     zero(sc);
@@ -524,8 +600,8 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     fence_regs(dp);
     if constexpr (kCausal) {  // S -> -inf past the diagonal, so P = 0 there
       const int key0 = static_cast<int>((kb0 + j) * BN);
-      if (crosses_diagonal(key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base), a.delta))
-        mask_past_diagonal<false>(sc, static_cast<int>(r), key0, a.delta);
+      if (crosses_diagonal(key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base), delta))
+        mask_past_diagonal<false>(sc, static_cast<int>(r), key0, delta);
     }
     const uint32_t c0 = (kb0 + j) * BN + 2 * (t % 4);
 #pragma unroll
@@ -533,7 +609,7 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
 #pragma unroll
       for (uint32_t e = 0; e < 4; ++e) {
         const uint32_t h = e >> 1, k = 4 * i + e;
-        const float p = c0 + 8 * i + (e & 1) < a.C ? ex2_approx(fmaf(sc[k], a.scale_log2, -Lr[h])) : 0.f;
+        const float p = c0 + 8 * i + (e & 1) < span.C ? ex2_approx(fmaf(sc[k], a.scale_log2, -Lr[h])) : 0.f;
         sc[k] = p * fmaf(dp[k], a.scale, -Dr[h]);  // dS
       }
     wgmma_fence();
@@ -548,7 +624,25 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     fence_regs(dq);
     ring.release_and_refill(j, blocks, load_kv);
   }
-  store_acc(dq, a.dQ + blockIdx.z * a.split_stride + hb * a.D, row0, a.R, 0, a.D, 1.f, 1.f);
+  store_acc(dq, a.dQ + (kVarlen ? 0 : blockIdx.z * a.split_stride) + hb * a.D, row0, span.R, 0, a.D, 1.f, 1.f);
+}
+
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
+__global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
+    attention_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
+                                   const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
+                                   const BwdArgs a) {
+  backward_query_body<DCH, kBF16, kConvertDO, kCausal, false>(mapQ, mapdO, mapK, mapV, a, Sequences{});
+}
+
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
+__global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
+    packed_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ,
+                                          const __grid_constant__ CUtensorMap mapdO,
+                                          const __grid_constant__ CUtensorMap mapK,
+                                          const __grid_constant__ CUtensorMap mapV, const BwdArgs a,
+                                          const Sequences seq) {
+  backward_query_body<DCH, kBF16, kConvertDO, kCausal, true>(mapQ, mapdO, mapK, mapV, a, seq);
 }
 
 // ================================================================================================ backward dK/dV
@@ -562,11 +656,11 @@ struct KVCfg {
   using Smem = SmemLayout<2 * kKBytes, kQBytes>;  // resident K, V; stage: Q, dO
 };
 
-template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
-__global__ void __launch_bounds__(2 * kWG, 1)
-    attention_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
-                                       const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
-                                       const BwdArgs a) {
+// The body of the dK/dV kernels; kVarlen as in forward_body (a tile of keys whose sequence has no query stores zeros)
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal, bool kVarlen>
+__device__ __forceinline__ void backward_key_value_body(const CUtensorMap &mapQ, const CUtensorMap &mapdO,
+                                                        const CUtensorMap &mapK, const CUtensorMap &mapV,
+                                                        const BwdArgs &a, const Sequences &seq) {
   using Cfg = KVCfg<DCH>;
   constexpr uint32_t BM = Cfg::BM, NA = Cfg::kAcc;
   extern __shared__ uint8_t smem_raw[];
@@ -574,31 +668,43 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   // grouped K/V: blockIdx.y is a K/V head, and the CTA walks the query blocks of every query head of its group
   const uint32_t kv_head = blockIdx.y, key_base = blockIdx.x * Cfg::kTileN;
-  const uint32_t qb0 = blockIdx.z * a.blocks_per_split;
+  SequenceSpan span{0, a.R, 0, a.C};
+  int delta = a.delta;
+  uint32_t qb0, per_split;
+  if constexpr (kVarlen) {
+    span = sequence_span(seq, blockIdx.z);
+    if (key_base >= span.C) return;
+    delta = static_cast<int>(span.C) - static_cast<int>(span.R);
+    qb0 = 0;
+    per_split = (span.R + BM - 1) / BM;
+  } else {
+    qb0 = blockIdx.z * a.blocks_per_split;
+    per_split = a.blocks_per_split;
+  }
   // causal: this CTA's query blocks start at the first one that sees the tile's first key (query >= key_base - delta)
-  const uint32_t qs = kCausal ? max(qb0, first_query_block<BM>(key_base, a.delta)) : qb0;
-  const uint32_t blocks = kCausal ? visible_query_blocks<BM>(a.R, qb0, qs, a.blocks_per_split)
-                                  : min((a.R + BM - 1) / BM - qb0, a.blocks_per_split);
+  const uint32_t qs = kCausal ? max(qb0, first_query_block<BM>(key_base, delta)) : qb0;
+  const uint32_t blocks = kCausal ? visible_query_blocks<BM>(span.R, qb0, qs, per_split)
+                                  : min((span.R + BM - 1) / BM - qb0, per_split);
   // the same query blocks [qs, qs + blocks) of each of the group's query heads, as one flattened sequence n = g blocks
   // + i that drives the Q / dO ring: prefetch and barrier parity carry across head boundaries
   const uint32_t total = a.group * blocks;
 
   auto load_qd = [&](uint32_t n, uint8_t *dst, uint64_t *bar) {
     const uint32_t g = n / blocks, i = n - g * blocks;
-    load_tile<DCH, BM>(dst, &mapQ, bar, (qs + i) * BM, kv_head * a.group + g);
-    load_tile<DCH, BM>(dst + Cfg::kQBytes, &mapdO, bar, (qs + i) * BM, kv_head * a.group + g);
+    load_tile<DCH, BM>(dst, &mapQ, bar, span.q0 + (qs + i) * BM, kv_head * a.group + g);
+    load_tile<DCH, BM>(dst + Cfg::kQBytes, &mapdO, bar, span.q0 + (qs + i) * BM, kv_head * a.group + g);
   };
   ring.init();
   ring.start(
       [&](uint8_t *dst, uint64_t *bar) {
-        load_tile<DCH, Cfg::kTileN>(dst, &mapK, bar, key_base, kv_head);
-        load_tile<DCH, Cfg::kTileN>(dst + Cfg::kKBytes, &mapV, bar, key_base, kv_head);
+        load_tile<DCH, Cfg::kTileN>(dst, &mapK, bar, span.k0 + key_base, kv_head);
+        load_tile<DCH, Cfg::kTileN>(dst + Cfg::kKBytes, &mapV, bar, span.k0 + key_base, kv_head);
       },
       total, load_qd);
   const uint32_t sK = smem_u32(ring.base), sV = sK + Cfg::kKBytes;
   const uint32_t krow = Cfg::kSplitD ? 0 : wg * kRows;      // this warpgroup's key rows inside the tile
   const uint32_t nchunk = Cfg::kSplitD ? wg * (NA / 64) : 0;  // ... and its first accumulator column chunk
-  size_t hb = static_cast<size_t>(kv_head) * a.group * a.R;  // L / D rows of the current query head
+  size_t hb = static_cast<size_t>(kv_head) * a.group * a.R + span.q0;  // L / D rows of the current query head
   float dv[NA / 2], dk[NA / 2];
   zero(dv);
   zero(dk);
@@ -611,7 +717,7 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     for (uint32_t j = 0; j < BM / 8; ++j)
 #pragma unroll
       for (uint32_t e = 0; e < 2; ++e) {
-        const uint32_t q = min(q0 + 8 * j + e, a.R - 1);
+        const uint32_t q = min(q0 + 8 * j + e, span.R - 1);
         Lq[2 * j + e] = load_stat(a.L, hb + q, a.l_prec);
         Dq[2 * j + e] = load_stat(a.Dterm, hb + q, a.d_prec);
       }
@@ -621,6 +727,12 @@ __global__ void __launch_bounds__(2 * kWG, 1)
       // than one wave converts dO once, in a pass of its own, instead)
       uint4 *tile = reinterpret_cast<uint4 *>(ring.stage(n) + Cfg::kQBytes);
       for (uint32_t k = tid; k < Cfg::kQBytes / 16; k += Cfg::kThreads) tile[k] = bwd::bf16x8_to_f16x8(tile[k]);
+      fence_proxy_async_smem();
+      __syncthreads();
+    }
+    if (kVarlen && (qs + i + 1) * BM > span.R) {  // the sequence's last query block: the next sequence's Q and dO
+      zero_rows<DCH, BM, Cfg::kThreads>(ring.stage(n), span.R - (qs + i) * BM);
+      zero_rows<DCH, BM, Cfg::kThreads>(ring.stage(n) + Cfg::kQBytes, span.R - (qs + i) * BM);
       fence_proxy_async_smem();
       __syncthreads();
     }
@@ -637,15 +749,15 @@ __global__ void __launch_bounds__(2 * kWG, 1)
     fence_regs(dpt);
     if constexpr (kCausal) {  // S^T -> -inf where key > query + delta, so P^T = 0 there
       const int qlo = static_cast<int>((qs + i) * BM);
-      if (crosses_diagonal(static_cast<int>(key_base + Cfg::kTileN) - 1, qlo, a.delta))
-        mask_past_diagonal<true>(st, static_cast<int>(key_base + krow + frag_row(t)), qlo, a.delta);
+      if (crosses_diagonal(static_cast<int>(key_base + Cfg::kTileN) - 1, qlo, delta))
+        mask_past_diagonal<true>(st, static_cast<int>(key_base + krow + frag_row(t)), qlo, delta);
     }
 #pragma unroll
     for (uint32_t j = 0; j < BM / 8; ++j)
 #pragma unroll
       for (uint32_t e = 0; e < 4; ++e) {
         const uint32_t k = 4 * j + e, c = 2 * j + (e & 1);
-        const float p = q0 + 8 * j + (e & 1) < a.R ? ex2_approx(fmaf(st[k], a.scale_log2, -Lq[c])) : 0.f;
+        const float p = q0 + 8 * j + (e & 1) < span.R ? ex2_approx(fmaf(st[k], a.scale_log2, -Lq[c])) : 0.f;
         st[k] = p;                                  // P^T
         dpt[k] = p * fmaf(dpt[k], a.scale, -Dq[c]);  // dS^T
       }
@@ -668,10 +780,29 @@ __global__ void __launch_bounds__(2 * kWG, 1)
       hb += a.R;
     }
   }
-  const size_t kb = static_cast<size_t>(kv_head) * a.C * a.D;
+  const size_t kb = (static_cast<size_t>(kv_head) * a.C + span.k0) * a.D;
   const uint32_t row0 = key_base + krow, col0 = nchunk * 64;
-  store_acc(dv, a.dV + blockIdx.z * a.split_stride + kb, row0, a.C, col0, a.D, 1.f, 1.f);
-  store_acc(dk, a.dK + blockIdx.z * a.split_stride + kb, row0, a.C, col0, a.D, 1.f, 1.f);
+  const size_t split = kVarlen ? 0 : blockIdx.z * a.split_stride;
+  store_acc(dv, a.dV + split + kb, row0, span.C, col0, a.D, 1.f, 1.f);
+  store_acc(dk, a.dK + split + kb, row0, span.C, col0, a.D, 1.f, 1.f);
+}
+
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    attention_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
+                                       const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
+                                       const BwdArgs a) {
+  backward_key_value_body<DCH, kBF16, kConvertDO, kCausal, false>(mapQ, mapdO, mapK, mapV, a, Sequences{});
+}
+
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    packed_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ,
+                                              const __grid_constant__ CUtensorMap mapdO,
+                                              const __grid_constant__ CUtensorMap mapK,
+                                              const __grid_constant__ CUtensorMap mapV, const BwdArgs a,
+                                              const Sequences seq) {
+  backward_key_value_body<DCH, kBF16, kConvertDO, kCausal, true>(mapQ, mapdO, mapK, mapV, a, seq);
 }
 
 static uint32_t chunks(uint32_t D) { return D <= 64 ? 1 : (D <= 128 ? 2 : 4); }
@@ -758,12 +889,20 @@ static cudaError_t make_maps(const AttentionParams &p, bool with_dO, TensorMaps 
 }
 
 template <uint32_t DCH, bool kBF16, bool kCausal>
-cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cudaStream_t stream) {
+cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, const Sequences *seq, cudaStream_t stream) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
   auto kernel = attention_forward_wgmma<DCH, kBF16, kCausal>;
   TensorMaps m;
   cudaError_t e;
+  if (seq) {  // packed sequences: unsplit
+    auto packed = packed_forward_wgmma<DCH, kBF16, kCausal>;
+    if ((e = prepare(packed, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess) return e;
+    packed<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]),
+                                                             p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL],
+                                                             p.group, *seq);
+    return cudaGetLastError();
+  }
   if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess) return e;
   SplitArgs sp{plan.blocks_per_split, plan.splits, p.batch, nullptr, nullptr};
   const uint64_t rows_total = static_cast<uint64_t>(p.batch) * p.R;
@@ -812,14 +951,21 @@ static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
 // A backward kernel whose outputs are the BwdArgs fields out0 and, unless null, out1: FP32 tensors of `elems` elements
 // each.  Split: each split writes partial sums to the workspace, [split][output][elems], and sum_splits adds them into
 // the outputs.
+// Packed sequences (seq): `packed` runs instead, unsplit.
 using OutputSlot = float *BwdArgs::*;
-template <class Cfg, class Kernel>
-static cudaError_t launch_backward(Kernel kernel, const AttentionParams &p, const WgmmaPlan &plan, OutputSlot out0,
-                                   OutputSlot out1, size_t elems, cudaStream_t stream) {
+template <class Cfg, class Kernel, class PackedKernel>
+static cudaError_t launch_backward(Kernel kernel, PackedKernel packed, const AttentionParams &p, const WgmmaPlan &plan,
+                                   const Sequences *seq, OutputSlot out0, OutputSlot out1, size_t elems,
+                                   cudaStream_t stream) {
   constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
   const uint32_t outputs = out1 ? 2 : 1;
   TensorMaps m;
   cudaError_t e;
+  if (seq) {
+    if ((e = prepare(packed, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, true, &m)) != cudaSuccess) return e;
+    packed<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.dO, m.K, m.V, backward_args(p, plan), *seq);
+    return cudaGetLastError();
+  }
   if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, true, &m)) != cudaSuccess) return e;
   BwdArgs a = backward_args(p, plan);
   float *const dst0 = a.*out0, *const dst1 = out1 ? a.*out1 : nullptr;
@@ -900,6 +1046,17 @@ WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batc
   return p;
 }
 
+WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t max_column, uint32_t count,
+                               uint32_t batch, uint32_t group, bool convert_dO, uint32_t sm_count) {
+  // min_blocks = 0: one traversal range per tile
+  WgmmaPlan p = wgmma_plan(type, D, max_row, max_column, batch, group, 0, 1, convert_dO, sm_count);
+  p.grid.z = count;
+  p.convert_dO_first = type == MFA_BACKWARD_KEY_VALUE && convert_dO &&
+                       static_cast<uint64_t>(p.grid.x) * p.grid.y * count > sm_count;
+  p.launches = 1 + (p.convert_dO_first ? 1 : 0);
+  return p;
+}
+
 static bool row_major_16bit(const AttentionParams &p) {
   for (int s = 0; s < kSlots; ++s)
     if (p.transposed[s]) return false;
@@ -907,19 +1064,23 @@ static bool row_major_16bit(const AttentionParams &p) {
          p.D % 8 == 0 && p.D <= kWgmmaMaxHead;
 }
 
-static WgmmaPlan plan_for(int type, const AttentionParams &p, bool convert_dO) {
-  return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, convert_dO,
-                    device_sm_count(current_device()));
+static WgmmaPlan plan_for(int type, const AttentionParams &p, const Sequences *seq, bool convert_dO) {
+  const uint32_t sm_count = device_sm_count(current_device());
+  if (seq)
+    return wgmma_plan_sequences(type, p.D, seq->max_row, seq->max_column, seq->count, p.batch, p.group, convert_dO,
+                                sm_count);
+  return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, convert_dO, sm_count);
 }
 
-cudaError_t launch_wgmma_forward(const AttentionParams &p, cudaStream_t stream) {
+cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
   if (!row_major_16bit(p) || p.prec[sO] != FP32) {
     set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
     return cudaErrorInvalidValue;
   }
-  const WgmmaPlan plan = plan_for(MFA_FORWARD, p, false);
+  const WgmmaPlan plan = plan_for(MFA_FORWARD, p, seq, false);
   return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
-    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, stream);
+    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, seq,
+                                                                                                      stream);
   });
 }
 
@@ -932,22 +1093,24 @@ static cudaError_t check_backward(const AttentionParams &p) {
   return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_wgmma_backward_query(const AttentionParams &p, cudaStream_t stream) {
+cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
   if (cudaError_t e = check_backward(p)) return e;
   const bool convert = p.prec[sdO] != p.prec[sQ];
-  const WgmmaPlan plan = plan_for(MFA_BACKWARD_QUERY, p, convert);
+  const WgmmaPlan plan = plan_for(MFA_BACKWARD_QUERY, p, seq, convert);
   return hop::dispatch(p, convert, [&](auto dch, auto bf16, auto cvt, auto causal) {
     constexpr uint32_t DCH = decltype(dch)::value;
-    return hop::launch_backward<hop::QCfg<DCH>>(
-        hop::attention_backward_query_wgmma<DCH, decltype(bf16)::value, decltype(cvt)::value, decltype(causal)::value>, p,
-        plan, &hop::BwdArgs::dQ, nullptr, static_cast<size_t>(p.batch) * p.R * p.D, stream);
+    constexpr bool kBF16 = decltype(bf16)::value, kConvert = decltype(cvt)::value, kCausal = decltype(causal)::value;
+    return hop::launch_backward<hop::QCfg<DCH>>(hop::attention_backward_query_wgmma<DCH, kBF16, kConvert, kCausal>,
+                                                hop::packed_backward_query_wgmma<DCH, kBF16, kConvert, kCausal>,
+                                                p, plan, seq, &hop::BwdArgs::dQ, nullptr,
+                                                static_cast<size_t>(p.batch) * p.R * p.D, stream);
   });
 }
 
-cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream_t stream) {
+cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
   if (cudaError_t e = check_backward(p)) return e;
   const bool convert = p.prec[sdO] != p.prec[sQ];
-  const WgmmaPlan plan = plan_for(MFA_BACKWARD_KEY_VALUE, p, convert);
+  const WgmmaPlan plan = plan_for(MFA_BACKWARD_KEY_VALUE, p, seq, convert);
   AttentionParams q = p;
   if (plan.convert_dO_first) {
     const uint64_t elements = static_cast<uint64_t>(p.batch) * p.R * p.D;
@@ -960,9 +1123,11 @@ cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, cudaStream
   }
   return hop::dispatch(q, convert && !plan.convert_dO_first, [&](auto dch, auto bf16, auto cvt, auto causal) {
     constexpr uint32_t DCH = decltype(dch)::value;
+    constexpr bool kBF16 = decltype(bf16)::value, kConvert = decltype(cvt)::value, kCausal = decltype(causal)::value;
     return hop::launch_backward<hop::KVCfg<DCH>>(
-        hop::attention_backward_key_value_wgmma<DCH, decltype(bf16)::value, decltype(cvt)::value, decltype(causal)::value>,
-        q, plan, &hop::BwdArgs::dV, &hop::BwdArgs::dK, static_cast<size_t>(q.batch / q.group) * q.C * q.D,  // per K/V head
+        hop::attention_backward_key_value_wgmma<DCH, kBF16, kConvert, kCausal>,
+        hop::packed_backward_key_value_wgmma<DCH, kBF16, kConvert, kCausal>, q, plan, seq, &hop::BwdArgs::dV,
+        &hop::BwdArgs::dK, static_cast<size_t>(q.batch / q.group) * q.C * q.D,  // per K/V head
         stream);
   });
 }

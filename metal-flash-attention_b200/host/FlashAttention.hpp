@@ -119,6 +119,9 @@ struct AttentionDescriptor {  // AttentionDescriptor.swift:10-27
   }
 };
 
+// {count, max_row, max_column, row_offsets, column_offsets}: the offsets are int32 device pointers (cu_seqlens)
+using SequenceTable = mfa_sequence_table_t;
+
 class AttentionKernel {  // AttentionKernel.swift:11-50
  public:
   explicit AttentionKernel(const AttentionKernelDescriptor &descriptor) { check(mfa_attention_kernel_create(&descriptor.c, &handle_)); }
@@ -153,6 +156,17 @@ class AttentionKernel {  // AttentionKernel.swift:11-50
   void encode(const mfa_function_constants_t &constants, const std::array<void *, MFA_BUFFER_COUNT> &buffers,
               void *cudaStream = nullptr) const {
     check(mfa_attention_kernel_encode(handle_, &constants, buffers.data(), cudaStream));
+  }
+  // packed variable-length sequences (library extension, mfa_sequence_table_t)
+  uint32_t gridSize(const mfa_function_constants_t &constants, const SequenceTable &sequences) const {
+    uint32_t v; check(mfa_attention_kernel_grid_size_sequences(handle_, &constants, &sequences, &v)); return v;
+  }
+  uint32_t launchCount(const mfa_function_constants_t &constants, const SequenceTable &sequences) const {
+    uint32_t v; check(mfa_attention_kernel_launch_count_sequences(handle_, &constants, &sequences, &v)); return v;
+  }
+  void encode(const mfa_function_constants_t &constants, const SequenceTable &sequences,
+              const std::array<void *, MFA_BUFFER_COUNT> &buffers, void *cudaStream = nullptr) const {
+    check(mfa_attention_kernel_encode_sequences(handle_, &constants, &sequences, buffers.data(), cudaStream));
   }
  private:
   mfa_attention_kernel_t *handle_ = nullptr;

@@ -382,6 +382,47 @@ public final class AttentionKernel {
     var constants = constants
     check(mfa_attention_kernel_encode(handle, &constants, &table, stream))
   }
+
+  // ---- library extension: packed variable-length sequences (mfa_sequence_table_t, FlashAttention's cu_seqlens)
+  public func gridSize(constants: mfa_function_constants_t, sequences: SequenceTable) -> UInt32 {
+    var constants = constants
+    var sequences = sequences
+    var out: UInt32 = 0
+    check(mfa_attention_kernel_grid_size_sequences(handle, &constants, &sequences, &out))
+    return out
+  }
+  public func launchCount(constants: mfa_function_constants_t, sequences: SequenceTable) -> UInt32 {
+    var constants = constants
+    var sequences = sequences
+    var out: UInt32 = 0
+    check(mfa_attention_kernel_launch_count_sequences(handle, &constants, &sequences, &out))
+    return out
+  }
+  /// `encode` over the sequences of `sequences`: every problem's rows are cut into the sequences of the device offset
+  /// tables, and each sequence attends only to its own keys.
+  public func encode(constants: mfa_function_constants_t, sequences: SequenceTable,
+                     buffers: [AttentionOperand: UnsafeMutableRawPointer],
+                     stream: UnsafeMutableRawPointer? = nil) {
+    var table = [UnsafeMutableRawPointer?](repeating: nil, count: Int(MFA_BUFFER_COUNT))
+    for (operand, pointer) in buffers {
+      guard let binding = operand.bufferBinding else { fatalError("Operand \(operand) has no buffer binding.") }
+      table[Int(binding)] = pointer
+    }
+    var constants = constants
+    var sequences = sequences
+    check(mfa_attention_kernel_encode_sequences(handle, &constants, &sequences, &table, stream))
+  }
+}
+
+/// library extension: packed variable-length sequences.  `rowOffsets` / `columnOffsets` are DEVICE pointers to
+/// `count + 1` Int32 entries each; `maxRow` / `maxColumn` are at least every sequence's query / key length.
+public typealias SequenceTable = mfa_sequence_table_t
+extension mfa_sequence_table_t {
+  public init(count: UInt32, maxRow: UInt32, maxColumn: UInt32, rowOffsets: UnsafePointer<Int32>,
+              columnOffsets: UnsafePointer<Int32>) {
+    self.init(count: count, max_row: maxRow, max_column: maxColumn, row_offsets: rowOffsets,
+              column_offsets: columnOffsets)
+  }
 }
 
 /// library extension: grouped-query / multi-query attention, a launch-time constant like R, C and the batch.  The
