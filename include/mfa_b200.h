@@ -340,6 +340,55 @@ MFA_API int mfa_attention_kernel_launch_count_sequences(const mfa_attention_kern
                                                         const mfa_sequence_table_t *sequences, uint32_t *out);
 
 /* ------------------------------------------------------------------------------------------ */
+/* Paged K/V cache (library extension; forward only)                                           */
+/* ------------------------------------------------------------------------------------------ */
+/** The forward over packed query sequences whose keys and values live in a paged cache, read in place: vLLM's block
+ *  table, FlashAttention's flash_attn_with_kvcache(..., block_table=).  The pool is cut into pages of page_size = P
+ *  key rows; sequence s owns the Cs keys whose pages page_table[s][0 .. ceil(Cs / P)) name, in order.
+ *
+ *  Layouts (function constants row, column, batch_count = H, kv_group = G):
+ *    Q, O   [H][row][D] and L [H][row], as in a packed call: sequence s owns rows [row_offsets[s], row_offsets[s + 1]).
+ *    K, V   page pools [num_pages][P][H / G][D] (the layout serving engines keep), column = num_pages * P pool rows.
+ *           Key i of sequence s, K/V head kv, is pool row page_table[s][i / P] * P + i % P, head kv.
+ *  Query head h reads K/V head h / G.  Within a sequence the output is attention of its Rs queries over its Cs keys;
+ *  causal is bottom-right aligned per sequence (delta = Cs - Rs: the queries are the last Rs keys, which a decode or
+ *  chunked-prefill step appends to the cache before the call).  A row that sees no key, including every row when
+ *  Cs = 0, gets O = 0 and L = +inf.  Rows outside every sequence are never written.  Paged calls are never split.
+ *
+ *  The tables are DEVICE memory, read by the kernels only (a paged encode can be captured into a CUDA graph and
+ *  replayed after column_lengths and page_table changed).  The host returns MFA_ERROR_INVALID_ARGUMENT, naming the
+ *  field, for: a NULL table or device pointer; count of 0 or above 65535; max_row of 0 or above row; a page_size that
+ *  is not a power of two, is below 16, or does not divide column; page_stride of 0; a backward kernel type; any
+ *  transposed operand; on MFA_BACKEND_TCGEN05 a head dimension that is not a multiple of 8; batch_count above 16384
+ *  (the pools interleave the heads of every token, so a batch is never sliced).  The kernels clamp what they read, so
+ *  malformed contents never reach outside the caller's buffers: every query range as in mfa_sequence_table_t, every
+ *  Cs into [0, page_stride * P] (no page-table row is read past its end), every page id into [0, num_pages).
+ *  Page-table entries at or past ceil(Cs / P) are never read, and rows of a sequence's last page at or past Cs never
+ *  reach its output (whatever they hold, NaN included).  As for packed calls, a sequence longer than max_row breaks
+ *  the contract: its rows past the maximum may be left unwritten. */
+typedef struct mfa_paged_kv {
+  uint32_t count;                /* S >= 1 sequences */
+  uint32_t max_row;              /* host value >= every Rs: sizes the grid */
+  const int32_t *row_offsets;    /* device, S + 1 entries: the packed query rows, as mfa_sequence_table_t.row_offsets */
+  const int32_t *column_lengths; /* device, S entries: Cs, the keys of sequence s (its cache length, new tokens included) */
+  const int32_t *page_table;     /* device, [S][page_stride]: entry j holds the page of keys [j * P, (j + 1) * P) */
+  uint32_t page_stride;          /* entries per page_table row */
+  uint32_t page_size;            /* P: a power of two, >= 16, dividing column */
+} mfa_paged_kv_t;
+/** mfa_attention_kernel_encode of a forward kernel over a paged K/V cache. */
+MFA_API int mfa_attention_kernel_encode_paged(const mfa_attention_kernel_t *kernel,
+                                              const mfa_function_constants_t *constants, const mfa_paged_kv_t *paged,
+                                              void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
+/** Grid size of a paged call: ceil(max_row / parallelization) x batch_count x count. */
+MFA_API int mfa_attention_kernel_grid_size_paged(const mfa_attention_kernel_t *kernel,
+                                                 const mfa_function_constants_t *constants,
+                                                 const mfa_paged_kv_t *paged, uint32_t *out);
+/** Kernels one paged encode launches: 1. */
+MFA_API int mfa_attention_kernel_launch_count_paged(const mfa_attention_kernel_t *kernel,
+                                                    const mfa_function_constants_t *constants,
+                                                    const mfa_paged_kv_t *paged, uint32_t *out);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Kernel cache keyed by descriptor                                                            */
 /* ------------------------------------------------------------------------------------------ */
 /** The analogue of the reference's pipeline cache (GEMMKernel.register(descriptor:) / pipelineCache[descriptor],

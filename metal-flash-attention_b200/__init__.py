@@ -104,6 +104,21 @@ class SequenceTable(ctypes.Structure):
         super().__init__(int(count), int(max_row), int(max_column), row_offsets or None, column_offsets or None)
 
 
+class PagedKV(ctypes.Structure):
+    """mfa_paged_kv_t: the forward over packed queries (row_offsets, as in SequenceTable) whose keys and values live in
+    page pools [num_pages][page_size][Hkv][D] (vLLM's block table).  Sequence s has column_lengths[s] keys, key i in pool
+    row page_table[s * page_stride + i // page_size] * page_size + i % page_size.  The three tables are int32 DEVICE
+    pointers; max_row bounds every sequence's query count."""
+    _fields_ = [("count", ctypes.c_uint32), ("max_row", ctypes.c_uint32), ("row_offsets", ctypes.c_void_p),
+                ("column_lengths", ctypes.c_void_p), ("page_table", ctypes.c_void_p), ("page_stride", ctypes.c_uint32),
+                ("page_size", ctypes.c_uint32)]
+
+    def __init__(self, count=0, max_row=0, row_offsets=0, column_lengths=0, page_table=0, page_stride=0,
+                 page_size=0):
+        super().__init__(int(count), int(max_row), row_offsets or None, column_lengths or None, page_table or None,
+                         int(page_stride), int(page_size))
+
+
 def _load():
     if not os.path.exists(_LIB_PATH):
         raise ImportError(
@@ -146,6 +161,12 @@ def _load():
                                                              c.POINTER(SequenceTable), c.POINTER(c.c_uint32)]
     lib.mfa_attention_kernel_launch_count_sequences.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
                                                                 c.POINTER(SequenceTable), c.POINTER(c.c_uint32)]
+    lib.mfa_attention_kernel_encode_paged.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants), c.POINTER(PagedKV),
+                                                      c.POINTER(c.c_void_p * MFA_BUFFER_COUNT), c.c_void_p]
+    lib.mfa_attention_kernel_grid_size_paged.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                         c.POINTER(PagedKV), c.POINTER(c.c_uint32)]
+    lib.mfa_attention_kernel_launch_count_paged.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                            c.POINTER(PagedKV), c.POINTER(c.c_uint32)]
     lib.mfa_attention_kernel_cache_fetch.argtypes = [c.POINTER(_CDescriptor), c.c_int, c.POINTER(c.c_void_p)]
     lib.mfa_attention_kernel_cache_size.restype = c.c_int
     lib.mfa_attention_run_host.argtypes = [c.POINTER(_CDescriptor), c.c_uint32,
@@ -494,6 +515,11 @@ class AttentionKernelDescriptor:
 # -------------------------------------------------------------------------------------------------
 # AttentionKernel
 # -------------------------------------------------------------------------------------------------
+def _one_table(sequences, paged):
+    if sequences is not None and paged is not None:
+        raise MFAError(-2, "Pass sequences= or paged=, not both: a paged call carries its own query offsets.")
+
+
 class AttentionKernel:
     """AttentionKernel.swift:11-50.  `encode` performs what the reference's callers do by hand
     (makeLibrary / makeComputePipelineState / setBuffer x10 / dispatchThreadgroups,
@@ -543,19 +569,30 @@ class AttentionKernel:
         _check(_lib.mfa_attention_kernel_threadgroup_memory_allocation(self._handle, ctypes.byref(out)))
         return out.value
 
-    def gridSize(self, constants: FunctionConstantValues, sequences: Optional[SequenceTable] = None) -> int:
-        """sequences: packed variable-length sequences (mfa_attention_kernel_grid_size_sequences)."""
+    def gridSize(self, constants: FunctionConstantValues, sequences: Optional[SequenceTable] = None,
+                 paged: Optional[PagedKV] = None) -> int:
+        """sequences: packed variable-length sequences (mfa_attention_kernel_grid_size_sequences); paged: a paged K/V
+        cache (mfa_attention_kernel_grid_size_paged)."""
         out = ctypes.c_uint32()
-        if sequences is None:
+        _one_table(sequences, paged)
+        if paged is not None:
+            _check(_lib.mfa_attention_kernel_grid_size_paged(self._handle, ctypes.byref(constants._c),
+                                                             ctypes.byref(paged), ctypes.byref(out)))
+        elif sequences is None:
             _check(_lib.mfa_attention_kernel_grid_size(self._handle, ctypes.byref(constants._c), ctypes.byref(out)))
         else:
             _check(_lib.mfa_attention_kernel_grid_size_sequences(self._handle, ctypes.byref(constants._c),
                                                                  ctypes.byref(sequences), ctypes.byref(out)))
         return out.value
 
-    def launchCount(self, constants: FunctionConstantValues, sequences: Optional[SequenceTable] = None) -> int:
+    def launchCount(self, constants: FunctionConstantValues, sequences: Optional[SequenceTable] = None,
+                    paged: Optional[PagedKV] = None) -> int:
         out = ctypes.c_uint32()
-        if sequences is None:
+        _one_table(sequences, paged)
+        if paged is not None:
+            _check(_lib.mfa_attention_kernel_launch_count_paged(self._handle, ctypes.byref(constants._c),
+                                                                ctypes.byref(paged), ctypes.byref(out)))
+        elif sequences is None:
             _check(_lib.mfa_attention_kernel_launch_count(self._handle, ctypes.byref(constants._c), ctypes.byref(out)))
         else:
             _check(_lib.mfa_attention_kernel_launch_count_sequences(self._handle, ctypes.byref(constants._c),
@@ -567,16 +604,21 @@ class AttentionKernel:
         return _lib.mfa_attention_kernel_source_name(self._handle).decode()
 
     def encode(self, constants: FunctionConstantValues, buffers: Dict[AttentionOperand, int],
-               stream: int = 0, sequences: Optional[SequenceTable] = None) -> None:
+               stream: int = 0, sequences: Optional[SequenceTable] = None, paged: Optional[PagedKV] = None) -> None:
         """buffers: {AttentionOperand: device pointer}; stream: cudaStream_t as int (0 = default).  sequences: packed
-        variable-length sequences over the rows of every problem (mfa_attention_kernel_encode_sequences)."""
+        variable-length sequences over the rows of every problem (mfa_attention_kernel_encode_sequences).  paged: the
+        forward over a paged K/V cache, K and V pointing at the page pools (mfa_attention_kernel_encode_paged)."""
+        _one_table(sequences, paged)
         arr = (ctypes.c_void_p * MFA_BUFFER_COUNT)()
         for op, ptr in buffers.items():
             binding = AttentionOperand(op).bufferBinding
             if binding is None:
                 raise MFAError(-2, f"Operand {AttentionOperand(op).name} has no buffer binding.")
             arr[binding] = ptr
-        if sequences is None:
+        if paged is not None:
+            _check(_lib.mfa_attention_kernel_encode_paged(self._handle, ctypes.byref(constants._c), ctypes.byref(paged),
+                                                          ctypes.byref(arr), ctypes.c_void_p(stream)))
+        elif sequences is None:
             _check(_lib.mfa_attention_kernel_encode(self._handle, ctypes.byref(constants._c), ctypes.byref(arr),
                                                     ctypes.c_void_p(stream)))
         else:
@@ -587,6 +629,6 @@ class AttentionKernel:
 
 __all__ = [
     "AttentionDescriptor", "AttentionKernelDescriptor", "AttentionKernel", "AttentionKernelType",
-    "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError", "SequenceTable",
+    "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError", "SequenceTable", "PagedKV",
     "library_path", "version", "setParameterTable", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
 ]

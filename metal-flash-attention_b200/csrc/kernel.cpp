@@ -182,6 +182,59 @@ static int sequences_of(const mfa_attention_kernel *k, const mfa_function_consta
   return MFA_SUCCESS;
 }
 
+// The launch form of a paged K/V table, after the checks the host can make without reading device memory
+static int paged_of(const mfa_attention_kernel *k, const mfa_function_constants_t *c, const mfa_paged_kv_t *t,
+                    PagedKV *out) {
+  if (!t) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL paged K/V table.");
+  if (k->type != MFA_FORWARD)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: only the forward kernel reads a paged cache.");
+  int n = 0;
+  const int *ops = operands_of(k->type, &n);
+  for (int i = 0; i < n; ++i)
+    if ((k->descriptor.transpose_state_mask >> ops[i]) & 1)
+      return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Paged K/V needs row-major operands; ") +
+                                                  mfa_operand_name((mfa_operand_t)ops[i]) + " is transposed.");
+  if (k->backend == MFA_BACKEND_TCGEN05 && k->descriptor.head_dimension % 8 != 0)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V on MFA_BACKEND_TCGEN05 needs a head dimension that is a multiple "
+                                            "of 8 (head " + std::to_string(k->descriptor.head_dimension) + ").");
+  if (!t->row_offsets || !t->column_lengths || !t->page_table)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Paged K/V: ") +
+                                                (!t->row_offsets ? "row_offsets" : !t->column_lengths ? "column_lengths"
+                                                                                                      : "page_table") +
+                                                " must not be NULL.");
+  if (t->count == 0 || t->count > kMaxSequences)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: count " + std::to_string(t->count) + " is outside [1, " +
+                                                std::to_string(kMaxSequences) + "].");
+  if (t->max_row == 0 || t->max_row > c->row)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: max_row " + std::to_string(t->max_row) +
+                                                " is outside [1, row = " + std::to_string(c->row) + "].");
+  const uint32_t P = t->page_size;
+  if (P < 16 || (P & (P - 1)) != 0 || c->column % P != 0)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: page_size " + std::to_string(P) +
+                                                " must be a power of two, at least 16, dividing column = " +
+                                                std::to_string(c->column) + ".");
+  if (t->page_stride == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: page_stride 0 must be at least 1.");
+  const uint32_t batch = c->batch_count ? c->batch_count : 1;
+  if (batch > kMaxBatchPerLaunch)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: batch_count " + std::to_string(batch) + " exceeds " +
+                                                std::to_string(kMaxBatchPerLaunch) + " (a paged call is one launch).");
+  uint32_t group = 1;
+  const int status = kv_group_of(c, &group);
+  if (status != MFA_SUCCESS) return status;
+  uint32_t shift = 0;
+  while ((1u << shift) < P) ++shift;
+  const uint64_t max_keys = static_cast<uint64_t>(t->page_stride) << shift;
+  *out = PagedKV{t->row_offsets, t->column_lengths, t->page_table, c->row, c->column / P, shift, t->page_stride,
+                 static_cast<uint32_t>(max_keys < 0x7fffffffu ? max_keys : 0x7fffffffu), batch / group, t->count,
+                 t->max_row};
+  return MFA_SUCCESS;
+}
+// The grid of a paged call is that of a packed call whose longest query sequence has max_row rows (a forward's grid
+// does not depend on the keys)
+static Sequences grid_of(const PagedKV &pk) {
+  return Sequences{pk.row_offsets, nullptr, pk.rows, 0, pk.count, pk.max_row, 1};
+}
+
 // encode() of problems of the full R x C shape (seq == nullptr) or of packed sequences
 static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, const Sequences *seq,
                   void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
@@ -379,6 +432,46 @@ int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_
                                 void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   return encode(kernel, constants, nullptr, buffers, cuda_stream);
+}
+
+int mfa_attention_kernel_grid_size_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                                         const mfa_paged_kv_t *table, uint32_t *out) {
+  if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  PagedKV pk;
+  const int status = paged_of(kernel, c, table, &pk);
+  if (status != MFA_SUCCESS) return status;
+  const Sequences seq = grid_of(pk);
+  return grid_size(kernel, c, &seq, out);
+}
+
+int mfa_attention_kernel_launch_count_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                                            const mfa_paged_kv_t *table, uint32_t *out) {
+  if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  PagedKV pk;
+  const int status = paged_of(kernel, c, table, &pk);
+  if (status != MFA_SUCCESS) return status;
+  *out = 1;  // never staged (row-major, head % 8 == 0 on the tensor cores), never split, one batch slice
+  return MFA_SUCCESS;
+}
+
+int mfa_attention_kernel_encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
+                                      const mfa_paged_kv_t *table, void *const buffers[MFA_BUFFER_COUNT],
+                                      void *cuda_stream) {
+  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
+  PagedKV pk;
+  int status = paged_of(kernel, constants, table, &pk);
+  if (status != MFA_SUCCESS) return status;
+  if ((status = check_device()) != MFA_SUCCESS) return status;
+  AttentionParams p;
+  if ((status = build_params(kernel, constants, buffers, p)) != MFA_SUCCESS) return status;
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const cudaError_t e = kernel->backend == MFA_BACKEND_TCGEN05 ? launch_wgmma_forward_paged(p, pk, stream)
+                                                              : launch_simt_forward_paged(p, pk, stream);
+  if (e != cudaSuccess)
+    return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " (paged K/V) failed: " +
+                                    cudaGetErrorString(e) + " " + last_launch_detail());
+  return MFA_SUCCESS;
 }
 
 int mfa_attention_kernel_encode_sequences(const mfa_attention_kernel_t *kernel,

@@ -64,11 +64,41 @@ __device__ __forceinline__ SequenceSpan sequence_span(const Sequences &s, uint32
 }
 #endif
 
+// Paged K/V (mfa_paged_kv_t), the forward's kernel argument: packed query rows as in Sequences, and the keys of
+// sequence s in the pages page_table[s][0 .. ceil(Cs / P)) of K / V pools [pages][P][kv_heads][D].
+struct PagedKV {
+  const int32_t *row_offsets, *column_lengths, *page_table;  // device memory: count + 1, count, count x page_stride
+  uint32_t rows;                 // query rows of each problem (AttentionParams R)
+  uint32_t pages, page_shift;    // pages in each pool (column / P), log2(P)
+  uint32_t page_stride;          // entries per page_table row
+  uint32_t max_keys;             // page_stride * P, at most INT32_MAX: no Cs reaches past its page_table row
+  uint32_t kv_heads;             // heads of each pool row (batch / group)
+  uint32_t count, max_row;       // host values: they size the grid
+};
+#ifdef __CUDACC__
+// Sequence i of a paged call: its query rows (clamped as in sequence_span), k0 = 0 and Cs clamped into [0, max_keys]
+__device__ __forceinline__ SequenceSpan paged_span(const PagedKV &pk, uint32_t i) {
+  SequenceSpan r;
+  r.R = sequence_rows(pk.row_offsets, i, pk.rows, &r.q0);
+  r.k0 = 0;
+  r.C = static_cast<uint32_t>(min(max(__ldg(pk.column_lengths + i), 0), static_cast<int>(pk.max_keys)));
+  return r;
+}
+// The pool row of key `key` of the sequence whose page_table row is `table` (key < its Cs), the page id clamped into
+// [0, pages)
+__device__ __forceinline__ uint32_t paged_row(const PagedKV &pk, const int32_t *table, uint32_t key) {
+  const int page = min(max(__ldg(table + (key >> pk.page_shift)), 0), static_cast<int>(pk.pages) - 1);
+  return (static_cast<uint32_t>(page) << pk.page_shift) | (key & ((1u << pk.page_shift) - 1));
+}
+#endif
+
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
 // seq: packed sequences, or nullptr for problems of the full R x C shape
 cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
 cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
 cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
+// paged K/V: the forward only, row-major operands
+cudaError_t launch_simt_forward_paged(const AttentionParams &p, const PagedKV &pk, cudaStream_t stream);
 void simt_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
                    uint32_t *head);
 
@@ -78,6 +108,8 @@ constexpr uint32_t kWgmmaMaxHead = 256;
 cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
 cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
 cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
+// paged K/V: the forward only, unsplit, grid (tiles of max_row, batch, count)
+cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, cudaStream_t stream);
 
 // How the launcher of kernel `type` (mfa_kernel_type_t) runs one problem of padded head dimension D; every field is
 // derived from the kernels' compile-time configurations.  R, C and batch do not affect the geometry fields.

@@ -103,9 +103,39 @@ __device__ __forceinline__ void load_tile(float *dst, const Operand &op, uint32_
   }
 }
 
+// Paged K/V (simt_forward_kernel_paged): the keys of one sequence and K/V head in a pool [pages][P][heads][D], row-major;
+// key s is pool row paged_row(s) (the page id clamped into [0, pages)), rows at or past seq read as zero
+struct PagedOperand {
+  const void *ptr;
+  const int32_t *table;  // the sequence's page_table row
+  uint32_t seq;          // Cs
+  uint32_t D, heads, head;
+  uint32_t pages, page_shift;
+  int prec;
+};
+
+template <int COLS, int LD>
+__device__ __forceinline__ void load_tile(float *dst, const PagedOperand &op, uint32_t s0, uint32_t d0, uint32_t dEnd,
+                                          int tid) {
+  constexpr int kElems = kBlock * COLS;
+#pragma unroll 4
+  for (int e = tid; e < kElems; e += kThreads) {
+    const int s = e / COLS, d = e % COLS;
+    const uint32_t gs = s0 + s, gd = d0 + d;
+    float v = 0.f;
+    if (gs < op.seq && gd < dEnd) {
+      const int page = min(max(__ldg(op.table + (gs >> op.page_shift)), 0), static_cast<int>(op.pages) - 1);
+      const size_t row = (static_cast<size_t>(page) << op.page_shift) | (gs & ((1u << op.page_shift) - 1));
+      v = load_elem(op.ptr, (row * op.heads + op.head) * op.D + gd, op.prec);
+    }
+    dst[s * LD + d] = v;
+  }
+}
+
 // acc[i][j] += sum_d A[a0 + ty + 16 i][d] * B[b0 + tx + 16 j][d]       ("outer product" GEMM,
 // AttentionKernel+OuterProduct.swift:18-487: C[par x trav] = A[par x D] . B^T[trav x D])
-__device__ __forceinline__ void gemm_nt(float (&acc)[4][4], const Operand &A, uint32_t a0, const Operand &B,
+template <class OperandB>
+__device__ __forceinline__ void gemm_nt(float (&acc)[4][4], const Operand &A, uint32_t a0, const OperandB &B,
                                         uint32_t b0, float *sA, float *sB, int tid, int tx, int ty) {
   const uint32_t D = A.D;
   for (uint32_t d0 = 0; d0 < D; d0 += kDC) {
@@ -137,8 +167,8 @@ __device__ __forceinline__ void gemm_nt(float (&acc)[4][4], const Operand &A, ui
 
 // acc[q][i][0..3] += sum_k sP[ty + 16 i][k] * X[x0 + k][dlo + 64 q + 4 tx + (0..3)]   ("accumulate"
 // GEMM, AttentionKernel+Accumulate.swift:24-582: C[par x D] += A[par x trav] . B[trav x D])
-template <int NCH>
-__device__ __forceinline__ void accumulate(float (&acc)[NCH][4][4], const float *sP, const Operand &X, uint32_t x0,
+template <int NCH, class OperandX>
+__device__ __forceinline__ void accumulate(float (&acc)[NCH][4][4], const float *sP, const OperandX &X, uint32_t x0,
                                            uint32_t dlo, uint32_t dhi, float *sX, int tid, int tx, int ty) {
 #pragma unroll
   for (int q = 0; q < NCH; ++q) {
@@ -236,7 +266,7 @@ __device__ __forceinline__ void store_acc(const float (&acc)[NCH][4][4], const f
 // ------------------------------------------------------------------------------------------------
 // forward: O = softmax(Q K^T / sqrt(D)) V,  L = log2(e) * logsumexp          (one CTA per 64 rows)
 // ------------------------------------------------------------------------------------------------
-// (packed sequences: simt_forward_kernel_varlen, below, is this kernel's twin)
+// (packed sequences: simt_forward_kernel_varlen, below, is this kernel's twin, and simt_forward_kernel_paged theirs)
 template <int NCH>
 __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const AttentionParams p) {
   extern __shared__ __align__(16) float smem[];
@@ -593,6 +623,80 @@ __global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel_varlen(const 
   }
 }
 
+// Paged K/V: simt_forward_kernel_varlen with K and V read from the sequence's pages of the pools (PagedOperand)
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel_paged(const AttentionParams p, const PagedKV pk) {
+  extern __shared__ __align__(16) float smem[];
+  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
+  Span sp;
+  sp.s = paged_span(pk, blockIdx.z);
+  sp.offset = static_cast<int>(sp.s.C) - static_cast<int>(sp.s.R);
+  if (r0 >= sp.s.R) return;  // a tile past the sequence's end
+  const Operand Q = span_query(p, sQ, b, sp);
+  const int32_t *table = pk.page_table + static_cast<size_t>(blockIdx.z) * pk.page_stride;
+  const PagedOperand K{p.buf[sK], table, sp.s.C, p.D, pk.kv_heads, b / p.group, pk.pages, pk.page_shift, p.prec[sK]},
+      V{p.buf[sV], table, sp.s.C, p.D, pk.kv_heads, b / p.group, pk.pages, pk.page_shift, p.prec[sV]};
+  float m[4], l[4], acc[NCH][4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    m[i] = -FLT_MAX;
+    l[i] = FLT_TRUE_MIN;
+  }
+  zero_acc(acc);
+  const uint32_t cend = span_visible_columns(p, sp, r0);
+  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
+    float s[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
+    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float mx = -FLT_MAX;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (span_masked(p, sp, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
+        mx = fmaxf(mx, s[i][j]);
+      }
+      mx = row_max16(mx);
+      const float m_new = fmaxf(m[i], mx * p.scale_log2), correction = exp2f(m[i] - m_new);
+      float sum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float pv = exp2f(fmaf(s[i][j], p.scale_log2, -m_new));
+        sum += pv;
+        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv;
+      }
+      l[i] = fmaf(l[i], correction, row_sum16(sum));
+      m[i] = m_new;
+#pragma unroll
+      for (int q = 0; q < NCH; ++q)
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] *= correction;
+    }
+    accumulate<NCH>(acc, sP, V, c0, 0, p.D, sX, tid, tx, ty);
+  }
+  float inv[4];
+  bool empty[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    empty[i] = sp.s.C == 0 || (p.causal && static_cast<int>(r0 + ty + 16 * i) + sp.offset < 0);
+    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
+  }
+  span_store<NCH>(acc, inv, span_query(p, sO, b, sp), r0, 0, p.D, tx, ty);
+  if (tx == 0 && p.buf[sL] != nullptr) {
+    char *Lbase = span_stats(p, sL, b, sp);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint32_t r = r0 + ty + 16 * i;
+      if (r < sp.s.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
+    }
+  }
+}
+
 template <int NCH>
 __global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel_varlen(const AttentionParams p,
                                                                                  const Sequences seq) {
@@ -737,6 +841,13 @@ cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, 
     constexpr int NCH = decltype(nch)::value;
     if (seq) return simt::launch(simt::simt_forward_kernel_varlen<NCH>, grid, stream, p, *seq);
     return simt::launch(simt::simt_forward_kernel<NCH>, grid, stream, p);
+  });
+}
+
+cudaError_t launch_simt_forward_paged(const AttentionParams &p, const PagedKV &pk, cudaStream_t stream) {
+  const dim3 grid((pk.max_row + simt::kBlock - 1) / simt::kBlock, p.batch, pk.count);
+  return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
+    return simt::launch(simt::simt_forward_kernel_paged<decltype(nch)::value>, grid, stream, p, pk);
   });
 }
 

@@ -41,14 +41,16 @@ static EncodeTiledFn resolve_encode() {
 // A tensor map is a pure function of (base, shape, box, type): callers that re-encode the same buffers (a training
 // loop, the benchmark's back-to-back dispatches) get the 128-byte descriptor from a small per-thread table instead of
 // a cuTensorMapEncodeTiled driver call (~1.5 us each, three or four per launch, against kernels of 15-25 us for one
-// head).  The descriptor says nothing about buffer *contents*, so a hit can never be stale.
+// head).  The descriptor says nothing about buffer *contents*, so a hit can never be stale.  The key holds the layout:
+// a paged pool and a [batch][seq][D] matrix over the same base, sizes and box have different strides.
 namespace {
+enum MapLayout : uint32_t { kMatrix = 0, kPagePool = 1 };
 struct MapKey {
   const void *base;
-  uint32_t seq, D, batch, boxCols, boxRows, dtype;
+  uint32_t seq, D, batch, boxCols, boxRows, dtype, layout;
   bool operator==(const MapKey &o) const {
     return base == o.base && seq == o.seq && D == o.D && batch == o.batch && boxCols == o.boxCols &&
-           boxRows == o.boxRows && dtype == o.dtype;
+           boxRows == o.boxRows && dtype == o.dtype && layout == o.layout;
   }
 };
 struct MapEntry {
@@ -61,14 +63,18 @@ thread_local MapEntry g_map_cache[kMapCacheEntries];
 uint32_t map_slot(const MapKey &k) {
   uint64_t h = reinterpret_cast<uintptr_t>(k.base) * 0x9E3779B97F4A7C15ull;
   h ^= (static_cast<uint64_t>(k.seq) << 32 | k.D) * 0xC2B2AE3D27D4EB4Full;
-  h ^= (static_cast<uint64_t>(k.batch) << 32 | (k.boxRows << 8) | k.dtype) * 0x165667B19E3779F9ull;
+  h ^= (static_cast<uint64_t>(k.batch) << 32 | (k.layout << 24) | (k.boxRows << 8) | k.dtype) * 0x165667B19E3779F9ull;
   return static_cast<uint32_t>(h >> 40) % kMapCacheEntries;
 }
 }  // namespace
 
+// kMatrix: [batch][seq][D], boxes of boxCols x boxRows x 1.  kPagePool: [seq][batch][D] (seq pool rows of `batch`
+// heads each), dims {D, batch, seq}, boxes of boxCols x 1 x boxRows: one head of boxRows consecutive rows, which lands
+// in shared memory as the same [boxRows][boxCols] tile.
 static cudaError_t encode(CUtensorMap *map, CUtensorMapDataType dtype, uint32_t elemBytes, const void *base,
-                          uint32_t seq, uint32_t D, uint32_t batch, uint32_t boxCols, uint32_t boxRows) {
-  const MapKey key{base, seq, D, batch, boxCols, boxRows, static_cast<uint32_t>(dtype)};
+                          uint32_t seq, uint32_t D, uint32_t batch, uint32_t boxCols, uint32_t boxRows,
+                          MapLayout layout) {
+  const MapKey key{base, seq, D, batch, boxCols, boxRows, static_cast<uint32_t>(dtype), layout};
   MapEntry &entry = g_map_cache[map_slot(key)];
   if (entry.valid && entry.key == key) {
     *map = entry.map;
@@ -83,9 +89,11 @@ static cudaError_t encode(CUtensorMap *map, CUtensorMapDataType dtype, uint32_t 
     set_launch_detail("TMA needs 16-byte aligned buffers and row pitch (base=%p, D=%u)", base, D);
     return cudaErrorInvalidValue;
   }
-  cuuint64_t dims[3] = {D, seq, batch};
-  cuuint64_t strides[2] = {static_cast<cuuint64_t>(D) * elemBytes, static_cast<cuuint64_t>(seq) * D * elemBytes};
-  cuuint32_t box[3] = {boxCols, boxRows, 1};
+  const cuuint64_t row = static_cast<cuuint64_t>(D) * elemBytes;
+  const bool pool = layout == kPagePool;
+  cuuint64_t dims[3] = {D, pool ? batch : seq, pool ? seq : batch};
+  cuuint64_t strides[2] = {row, (pool ? batch : seq) * row};
+  cuuint32_t box[3] = {boxCols, pool ? 1 : boxRows, pool ? boxRows : 1};
   cuuint32_t elemStrides[3] = {1, 1, 1};
   CUresult r = fn(map, dtype, 3, const_cast<void *>(base), dims, strides, box, elemStrides, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -103,7 +111,12 @@ static cudaError_t encode(CUtensorMap *map, CUtensorMapDataType dtype, uint32_t 
 cudaError_t make_tensor_map_16bit(CUtensorMap *map, const void *base, uint32_t seq, uint32_t D, uint32_t batch,
                                   uint32_t box_rows) {
   // BF16 and FP16 move identically through TMA; the 16-bit "type" only matters for OOB fill (zeros).
-  return encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, seq, D, batch, 64, box_rows);
+  return encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, seq, D, batch, 64, box_rows, kMatrix);
+}
+
+cudaError_t make_tensor_map_page_pool(CUtensorMap *map, const void *base, uint32_t rows, uint32_t heads, uint32_t D,
+                                      uint32_t box_rows) {
+  return encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, rows, D, heads, 64, box_rows, kPagePool);
 }
 
 }  // namespace mfa

@@ -13,6 +13,11 @@ namespace mfa {
 cudaError_t make_tensor_map_16bit(CUtensorMap *map, const void *base, uint32_t seq, uint32_t D, uint32_t batch,
                                   uint32_t box_rows);
 
+// Page pool [rows][heads][D] of 16-bit elements (a paged K/V cache): dims {D, heads, rows}, boxes of 64 (D) x 1 (head)
+// x box_rows (rows), loaded at (column, head, row) into the same [box_rows][64] 128-byte-swizzled tile as above.
+cudaError_t make_tensor_map_page_pool(CUtensorMap *map, const void *base, uint32_t rows, uint32_t heads, uint32_t D,
+                                      uint32_t box_rows);
+
 void set_launch_detail(const char *fmt, ...);
 
 }  // namespace mfa

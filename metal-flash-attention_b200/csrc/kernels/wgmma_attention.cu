@@ -27,6 +27,11 @@
 // Packed sequences (the packed_* entry points, kVarlen in the shared bodies): grid.z is the sequence; a CTA takes its
 // sequence's rows from the offset tables, leaves when its tile starts past the sequence's end, works on the sequence's
 // R, C and delta, and zeroes the rows of its last streamed block that belong to the next sequence.  Never split.
+//
+// Paged K/V (the paged_* forward, KVLayout::kPaged in forward_body): queries packed as above, keys and values in pools
+// [pages][P][kv_heads][D] read through a 3-D tensor map {D, kv_heads, pool rows} with boxes of 64 x 1 x min(P, BN), so
+// each box lands as the same [rows][64] swizzled tile.  A stage takes BN / min(P, BN) boxes per column chunk and tensor,
+// each at the pool row of its page; thread 0 reads the block's page ids just before it issues its boxes.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -307,13 +312,56 @@ struct FwdCfg {
   using Smem = SmemLayout<kQBytes, kKVBytes>;  // resident Q; stage: K, V
 };
 
-// The body of the forward kernels.  R, C: the rows of each problem's buffers.  kVarlen (packed sequences): the CTA works
-// on sequence blockIdx.z, whose span replaces R, C and delta in the ranges and masks and offsets every row; never split.
-template <uint32_t DCH, bool kBF16, bool kCausal, bool kVarlen>
+// Where the forward's keys come from: every problem's [C][D] rows (kFixed), a packed sequence's rows of them
+// (kPacked), or a sequence's pages of the K / V pools (kPaged)
+enum class KVLayout { kFixed, kPacked, kPaged };
+
+// Paged K/V: the TMA boxes of key block `block` into the DCH-chunk K tile at dst and the V tile `kv_bytes` after it,
+// `box` rows each (min(P, BN)).  P >= BN: one box per chunk and tensor, at the block's page.  P < BN: the page ids of
+// every box are read first, so that their loads overlap, then each box is issued for K and V.  Boxes that start at or
+// past the sequence's C never read the page table: they load pool row 0, and the caller zeroes every row past C before
+// the MMAs.
+template <uint32_t DCH, uint32_t BN>
+__device__ __forceinline__ void load_paged_kv(uint8_t *dst, uint32_t kv_bytes, const CUtensorMap *mapK,
+                                              const CUtensorMap *mapV, uint64_t *bar, const PagedKV &pk,
+                                              const int32_t *table, uint32_t block, uint32_t box, uint32_t C,
+                                              uint32_t kv_head) {
+  if (box == BN) {  // (a streamed block starts below C)
+    const uint32_t row = paged_row(pk, table, block * BN);
+#pragma unroll
+    for (uint32_t c = 0; c < DCH; ++c) {
+      tma_load_3d(dst + c * BN * 128, mapK, bar, c * 64, kv_head, row);
+      tma_load_3d(dst + kv_bytes + c * BN * 128, mapV, bar, c * 64, kv_head, row);
+    }
+    return;
+  }
+  constexpr uint32_t kMaxBoxes = BN / 16;  // P >= 16
+  uint32_t rows[kMaxBoxes];
+#pragma unroll
+  for (uint32_t i = 0; i < kMaxBoxes; ++i) {
+    const uint32_t key = block * BN + i * box;
+    rows[i] = i * box < BN && key < C ? paged_row(pk, table, key) : 0u;
+  }
+#pragma unroll
+  for (uint32_t i = 0; i < kMaxBoxes; ++i) {
+    if (i * box >= BN) break;
+#pragma unroll
+    for (uint32_t c = 0; c < DCH; ++c) {
+      tma_load_3d(dst + c * BN * 128 + i * box * 128, mapK, bar, c * 64, kv_head, rows[i]);
+      tma_load_3d(dst + kv_bytes + c * BN * 128 + i * box * 128, mapV, bar, c * 64, kv_head, rows[i]);
+    }
+  }
+}
+
+// The body of the forward kernels.  R, C: the rows of each problem's buffers (paged: C is unused).  kPacked / kPaged:
+// the CTA works on sequence blockIdx.z, whose span replaces R, C and delta in the ranges and masks and offsets every
+// query row, and zeroes the rows of its last key block past the sequence's keys; never split.
+template <uint32_t DCH, bool kBF16, bool kCausal, KVLayout kLayout>
 __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUtensorMap &mapK, const CUtensorMap &mapV,
                                              float *__restrict__ O, void *__restrict__ L, uint32_t R, uint32_t C,
                                              uint32_t D, float scale_log2, int l_prec, const SplitArgs &sp, int delta,
-                                             uint32_t group, const Sequences &seq) {
+                                             uint32_t group, const Sequences &seq, const PagedKV &pk) {
+  constexpr bool kVarlen = kLayout != KVLayout::kFixed;
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -325,7 +373,7 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   SequenceSpan span{0, R, 0, C};
   uint32_t kb0, per_split;
   if constexpr (kVarlen) {
-    span = sequence_span(seq, blockIdx.z);
+    span = kLayout == KVLayout::kPaged ? paged_span(pk, blockIdx.z) : sequence_span(seq, blockIdx.z);
     if (row_base >= span.R) return;  // a tile past the sequence's end
     delta = static_cast<int>(span.C) - static_cast<int>(span.R);
     kb0 = 0;
@@ -336,9 +384,17 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   }
   const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, span.R, span.C, delta, kb0, per_split);
 
+  // paged: this sequence's page_table row, and the rows of one TMA box
+  const int32_t *table = kLayout == KVLayout::kPaged ? pk.page_table + static_cast<size_t>(blockIdx.z) * pk.page_stride
+                                                     : nullptr;
+  const uint32_t box = kLayout == KVLayout::kPaged ? min(1u << pk.page_shift, BN) : BN;
   auto load_kv = [&](uint32_t j, uint8_t *dst, uint64_t *bar) {
-    load_tile<DCH, BN>(dst, &mapK, bar, span.k0 + (kb0 + j) * BN, kv_head);
-    load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, bar, span.k0 + (kb0 + j) * BN, kv_head);
+    if constexpr (kLayout == KVLayout::kPaged) {
+      load_paged_kv<DCH, BN>(dst, Cfg::kKVBytes, &mapK, &mapV, bar, pk, table, kb0 + j, box, span.C, kv_head);
+    } else {
+      load_tile<DCH, BN>(dst, &mapK, bar, span.k0 + (kb0 + j) * BN, kv_head);
+      load_tile<DCH, BN>(dst + Cfg::kKVBytes, &mapV, bar, span.k0 + (kb0 + j) * BN, kv_head);
+    }
   };
   if (tid == 0) {
     prefetch_tensormap(&mapQ);
@@ -357,7 +413,8 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   ring.wait_resident();
   for (uint32_t j = 0; j < blocks; ++j) {
     ring.wait(j);
-    if (kVarlen && (j + 1) * BN > span.C) {  // the sequence's last key block: the next sequence's keys and values
+    // the sequence's last key block: the next sequence's keys and values (packed), or whatever the page holds past C
+    if (kVarlen && (j + 1) * BN > span.C) {
       zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j), span.C - j * BN);
       zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, span.C - j * BN);
       fence_proxy_async_smem();
@@ -462,8 +519,8 @@ __global__ void __launch_bounds__(2 * kWG, 1)
                             const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
                             uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp,
                             int delta, uint32_t group) {
-  forward_body<DCH, kBF16, kCausal, false>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, sp, delta, group,
-                                           Sequences{});
+  forward_body<DCH, kBF16, kCausal, KVLayout::kFixed>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, sp, delta,
+                                                      group, Sequences{}, PagedKV{});
 }
 
 // Packed sequences: grid (tiles of the longest sequence, heads, sequences)
@@ -474,7 +531,19 @@ __global__ void __launch_bounds__(2 * kWG, 1)
                                    void *__restrict__ L, uint32_t R, uint32_t C, uint32_t D, float scale_log2,
                                    int l_prec, uint32_t group, const Sequences seq) {
   const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
-  forward_body<DCH, kBF16, kCausal, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, unsplit, 0, group, seq);
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPacked>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, unsplit, 0,
+                                                       group, seq, PagedKV{});
+}
+
+// Paged K/V: grid (tiles of the longest query sequence, heads, sequences); mapK / mapV are page-pool maps
+template <uint32_t DCH, bool kBF16, bool kCausal>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    paged_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                        const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L, uint32_t R,
+                        uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk) {
+  const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, unsplit, 0,
+                                                      group, Sequences{}, pk);
 }
 
 // ================================================================================================ backward dQ
@@ -925,6 +994,26 @@ cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cons
   return cudaGetLastError();
 }
 
+// Paged K/V: Q in the usual map, K and V as page pools of p.C rows, boxes of min(P, BN) rows
+template <uint32_t DCH, bool kBF16, bool kCausal>
+cudaError_t launch_forward_paged(const AttentionParams &p, const WgmmaPlan &plan, const PagedKV &pk,
+                                 cudaStream_t stream) {
+  using Cfg = FwdCfg<DCH>;
+  constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
+  auto kernel = paged_forward_wgmma<DCH, kBF16, kCausal>;
+  const uint32_t box = min(1u << pk.page_shift, Cfg::BN);
+  TensorMaps m;
+  cudaError_t e;
+  if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess ||
+      (e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, Cfg::kQueryBoxRows)) != cudaSuccess ||
+      (e = make_tensor_map_page_pool(&m.K, p.buf[sK], p.C, pk.kv_heads, p.D, box)) != cudaSuccess ||
+      (e = make_tensor_map_page_pool(&m.V, p.buf[sV], p.C, pk.kv_heads, p.D, box)) != cudaSuccess)
+    return e;
+  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL],
+                                                           p.R, p.D, p.scale_log2, p.prec[sL], p.group, pk);
+  return cudaGetLastError();
+}
+
 static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
   BwdArgs a;
   a.O = static_cast<const float *>(p.buf[sO]);
@@ -1081,6 +1170,20 @@ cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq,
   return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
     return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, seq,
                                                                                                       stream);
+  });
+}
+
+cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, cudaStream_t stream) {
+  if (!row_major_16bit(p) || p.prec[sO] != FP32) {
+    set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
+    return cudaErrorInvalidValue;
+  }
+  // (the plan of a packed call whose longest sequence has max_row queries: the key axis does not enter the grid)
+  const WgmmaPlan plan = wgmma_plan_sequences(MFA_FORWARD, p.D, pk.max_row, 1, pk.count, p.batch, p.group, false,
+                                              device_sm_count(current_device()));
+  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
+    return hop::launch_forward_paged<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, pk,
+                                                                                                            stream);
   });
 }
 

@@ -121,6 +121,8 @@ struct AttentionDescriptor {  // AttentionDescriptor.swift:10-27
 
 // {count, max_row, max_column, row_offsets, column_offsets}: the offsets are int32 device pointers (cu_seqlens)
 using SequenceTable = mfa_sequence_table_t;
+// {count, max_row, row_offsets, column_lengths, page_table, page_stride, page_size}: a paged K/V cache, int32 device tables
+using PagedKV = mfa_paged_kv_t;
 
 class AttentionKernel {  // AttentionKernel.swift:11-50
  public:
@@ -167,6 +169,17 @@ class AttentionKernel {  // AttentionKernel.swift:11-50
   void encode(const mfa_function_constants_t &constants, const SequenceTable &sequences,
               const std::array<void *, MFA_BUFFER_COUNT> &buffers, void *cudaStream = nullptr) const {
     check(mfa_attention_kernel_encode_sequences(handle_, &constants, &sequences, buffers.data(), cudaStream));
+  }
+  // the forward over a paged K/V cache (library extension, mfa_paged_kv_t): K and V point at the page pools
+  uint32_t gridSize(const mfa_function_constants_t &constants, const PagedKV &paged) const {
+    uint32_t v; check(mfa_attention_kernel_grid_size_paged(handle_, &constants, &paged, &v)); return v;
+  }
+  uint32_t launchCount(const mfa_function_constants_t &constants, const PagedKV &paged) const {
+    uint32_t v; check(mfa_attention_kernel_launch_count_paged(handle_, &constants, &paged, &v)); return v;
+  }
+  void encode(const mfa_function_constants_t &constants, const PagedKV &paged,
+              const std::array<void *, MFA_BUFFER_COUNT> &buffers, void *cudaStream = nullptr) const {
+    check(mfa_attention_kernel_encode_paged(handle_, &constants, &paged, buffers.data(), cudaStream));
   }
  private:
   mfa_attention_kernel_t *handle_ = nullptr;

@@ -412,6 +412,36 @@ public final class AttentionKernel {
     var sequences = sequences
     check(mfa_attention_kernel_encode_sequences(handle, &constants, &sequences, &table, stream))
   }
+
+  // ---- library extension: the forward over a paged K/V cache (mfa_paged_kv_t, vLLM's block table)
+  public func gridSize(constants: mfa_function_constants_t, paged: PagedKV) -> UInt32 {
+    var constants = constants
+    var paged = paged
+    var out: UInt32 = 0
+    check(mfa_attention_kernel_grid_size_paged(handle, &constants, &paged, &out))
+    return out
+  }
+  public func launchCount(constants: mfa_function_constants_t, paged: PagedKV) -> UInt32 {
+    var constants = constants
+    var paged = paged
+    var out: UInt32 = 0
+    check(mfa_attention_kernel_launch_count_paged(handle, &constants, &paged, &out))
+    return out
+  }
+  /// The forward `encode` over a paged K/V cache: the K and V buffers are page pools [pages][pageSize][Hkv][D], read in
+  /// place through the device page table.
+  public func encode(constants: mfa_function_constants_t, paged: PagedKV,
+                     buffers: [AttentionOperand: UnsafeMutableRawPointer],
+                     stream: UnsafeMutableRawPointer? = nil) {
+    var table = [UnsafeMutableRawPointer?](repeating: nil, count: Int(MFA_BUFFER_COUNT))
+    for (operand, pointer) in buffers {
+      guard let binding = operand.bufferBinding else { fatalError("Operand \(operand) has no buffer binding.") }
+      table[Int(binding)] = pointer
+    }
+    var constants = constants
+    var paged = paged
+    check(mfa_attention_kernel_encode_paged(handle, &constants, &paged, &table, stream))
+  }
 }
 
 /// library extension: packed variable-length sequences.  `rowOffsets` / `columnOffsets` are DEVICE pointers to
@@ -422,6 +452,18 @@ extension mfa_sequence_table_t {
               columnOffsets: UnsafePointer<Int32>) {
     self.init(count: count, max_row: maxRow, max_column: maxColumn, row_offsets: rowOffsets,
               column_offsets: columnOffsets)
+  }
+}
+
+/// library extension: a paged K/V cache.  `rowOffsets` (count + 1), `columnLengths` (count) and `pageTable`
+/// (count x pageStride) are DEVICE pointers to Int32 entries; `maxRow` is at least every sequence's query count and
+/// `pageSize` a power of two >= 16.
+public typealias PagedKV = mfa_paged_kv_t
+extension mfa_paged_kv_t {
+  public init(count: UInt32, maxRow: UInt32, rowOffsets: UnsafePointer<Int32>, columnLengths: UnsafePointer<Int32>,
+              pageTable: UnsafePointer<Int32>, pageStride: UInt32, pageSize: UInt32) {
+    self.init(count: count, max_row: maxRow, row_offsets: rowOffsets, column_lengths: columnLengths,
+              page_table: pageTable, page_stride: pageStride, page_size: pageSize)
   }
 }
 
