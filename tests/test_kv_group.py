@@ -31,10 +31,12 @@ LOG2E = 1.44269504089
 GOLDEN = os.path.join(ROOT, "tests", "golden", "gqa_default_outputs.json")
 
 
-def _descriptor(R, C, D, mode="bf16", batch=1, causal=False, transpose=(False,) * 4):
-    """mode: "bf16" / "fp16" (all operands of that type), "reference" (FP16 Q/K/V, BF16 dO) or "fp32" (SIMT family)."""
+def _descriptor(R, C, D, mode="bf16", batch=1, causal=False, transpose=(False,) * 4, lowMid=False):
+    """mode: "bf16" / "fp16" (all operands of that type), "reference" (FP16 Q/K/V, BF16 dO) or "fp32" (SIMT family).
+    lowMid: L stored as FP16 and D as BF16 (lowPrecisionIntermediates)."""
     desc = mfa.AttentionDescriptor()
     desc.lowPrecisionInputs = mode != "fp32"
+    desc.lowPrecisionIntermediates = lowMid
     desc.matrixDimensions = (R, C, D)
     desc.transposeState = tuple(transpose)
     desc.batchCount = batch

@@ -227,19 +227,28 @@ def _upload(a, prec):
     return torch.from_numpy(raw.view(np.int16) if prec != P.FP32 else raw).cuda()
 
 
-def _outputs(H, T, D):
+def _outputs(H, T, D, prec_L=P.FP32):
+    """NaN-sentinel O (FP32) and L (FP32, or 0xFFFF -- NaN -- in a 16-bit L)."""
     import torch
-    return (torch.full((H * T * D,), float("nan"), device="cuda"), torch.full((H * T,), float("nan"), device="cuda"))
+    L = (torch.full((H * T,), float("nan"), device="cuda") if prec_L == P.FP32 else
+         torch.full((H * T,), -1, dtype=torch.int16, device="cuda"))
+    return torch.full((H * T * D,), float("nan"), device="cuda"), L
+
+
+def _download_L(L, prec_L, H, T):
+    """L as float32 [H][T] (decoded from a 16-bit L)"""
+    a = L.cpu().numpy()
+    return (a if prec_L == P.FP32 else oracle.decode(a.view(np.uint16), int(prec_L))).reshape(H, T)
 
 
 def run_packed_forward(desc, G, Q, K, V, qo, ko):
     """The packed forward over contiguous keys: {O: [H][T][D], L: [H][T]} float32 (raw, L in log2 units)."""
     import torch
     prec = desc.memoryPrecisions
-    assert prec[Op.O] == P.FP32 and prec[Op.L] == P.FP32
+    assert prec[Op.O] == P.FP32
     H, T, D = Q.shape
     q, k, v = _upload(Q, prec[Op.Q]), _upload(K, prec[Op.K]), _upload(V, prec[Op.V])
-    O, L = _outputs(H, T, D)
+    O, L = _outputs(H, T, D, prec[Op.L])
     tq, tk = (torch.tensor(x, dtype=torch.int32, device="cuda") for x in (qo, ko))
     rq, rk = np.diff(qo), np.diff(ko)
     table = mfa.SequenceTable(len(qo) - 1, max(1, int(rq.max())), max(1, int(rk.max())), tq.data_ptr(), tk.data_ptr())
@@ -248,7 +257,7 @@ def run_packed_forward(desc, G, Q, K, V, qo, ko):
                   {Op.Q: q.data_ptr(), Op.K: k.data_ptr(), Op.V: v.data_ptr(), Op.O: O.data_ptr(), Op.L: L.data_ptr()},
                   sequences=table)
     torch.cuda.synchronize()
-    return {"O": O.cpu().numpy().reshape(H, T, D), "L": L.cpu().numpy().reshape(H, T)}
+    return {"O": O.cpu().numpy().reshape(H, T, D), "L": _download_L(L, prec[Op.L], H, T)}
 
 
 class PagedRun:
@@ -260,7 +269,8 @@ class PagedRun:
         self.H, self.T, self.D = Q.shape
         self.page_size = Kp.shape[1]
         self.q, self.k, self.v = _upload(Q, prec[Op.Q]), _upload(Kp, prec[Op.K]), _upload(Vp, prec[Op.V])
-        self.O, self.L = _outputs(self.H, self.T, self.D)
+        self.prec_L = prec[Op.L]
+        self.O, self.L = _outputs(self.H, self.T, self.D, self.prec_L)
         self.rows = torch.tensor(qo, dtype=torch.int32, device="cuda")
         self.lengths = torch.tensor(np.asarray(lengths, np.int64), dtype=torch.int32, device="cuda")
         self.table = torch.tensor(np.clip(table, -2**31, 2**31 - 1), dtype=torch.int32, device="cuda")
@@ -278,7 +288,7 @@ class PagedRun:
         import torch
         torch.cuda.synchronize()
         return {"O": self.O.cpu().numpy().reshape(self.H, self.T, self.D),
-                "L": self.L.cpu().numpy().reshape(self.H, self.T)}
+                "L": _download_L(self.L, self.prec_L, self.H, self.T)}
 
 
 def run_paged_forward(desc, G, Q, Kp, Vp, qo, lengths, table):

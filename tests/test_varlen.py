@@ -49,9 +49,10 @@ def reference(inputs, G, qo, ko, causal):
     return out
 
 
-def _descriptor(R, C, D, mode, batch, causal, transpose=(False,) * 4):
+def _descriptor(R, C, D, mode, batch, causal, transpose=(False,) * 4, lowMid=False):
     desc = mfa.AttentionDescriptor()
     desc.lowPrecisionInputs = mode != "fp32"
+    desc.lowPrecisionIntermediates = lowMid
     desc.matrixDimensions = (R, C, D)
     desc.transposeState = tuple(transpose)
     desc.batchCount = batch
