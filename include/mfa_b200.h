@@ -389,6 +389,26 @@ MFA_API int mfa_attention_kernel_launch_count_paged(const mfa_attention_kernel_t
                                                     const mfa_paged_kv_t *paged, uint32_t *out);
 
 /* ------------------------------------------------------------------------------------------ */
+/* Sliding-window attention (library extension)                                                */
+/* ------------------------------------------------------------------------------------------ */
+/** A key band around the (bottom-right aligned) diagonal, FlashAttention's window_size: with delta = C - R, or Cs - Rs
+ *  per sequence in packed and paged calls, query row i sees key j iff
+ *      i + delta - left  <=  j  <=  i + delta + right,
+ *  and a side of -1 has no bound.  A window of W keys ending at the diagonal is (W - 1, 0) on a causal kernel.  A row
+ *  that sees no key gets O = 0, L = +inf, D = 0, dQ = 0, and a key that no row sees gets dK = dV = 0.  Every block
+ *  and every page wholly outside the band is skipped: a paged forward never reads the page-table entries, nor loads the
+ *  pages, whose keys lie outside the band of every query row of their sequence (for a causal (left, 0) window: the
+ *  entries j with (j + 1) * P <= Cs - Rs - left), so a serving engine can recycle those pages. */
+typedef struct mfa_attention_window {
+  int32_t left, right; /* >= -1; a causal kernel takes right = 0 or -1 (both mean the diagonal) */
+} mfa_attention_window_t;
+/** mfa_attention_kernel_create of a kernel that applies `window`: every encode, grid-size and launch-count entry point
+ *  (fixed, _sequences, _paged) honours it.  MFA_ERROR_INVALID_ARGUMENT, naming the field, for a NULL window, a value
+ *  below -1, or right > 0 on a causal kernel.  The source name carries the window ("..._window<4095,0>"). */
+MFA_API int mfa_attention_kernel_create_windowed(const mfa_attention_kernel_descriptor_t *kernel_descriptor,
+                                                 const mfa_attention_window_t *window, mfa_attention_kernel_t **out);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Kernel cache keyed by descriptor                                                            */
 /* ------------------------------------------------------------------------------------------ */
 /** The analogue of the reference's pipeline cache (GEMMKernel.register(descriptor:) / pipelineCache[descriptor],
@@ -398,6 +418,11 @@ MFA_API int mfa_attention_kernel_launch_count_paged(const mfa_attention_kernel_t
  *  library (do NOT destroy it), is immutable, and stays valid until the process exits.  Thread-safe. */
 MFA_API int mfa_attention_kernel_cache_fetch(const mfa_attention_descriptor_t *descriptor, mfa_kernel_type_t type,
                                              const mfa_attention_kernel_t **out);
+/** mfa_attention_kernel_cache_fetch of a windowed kernel (mfa_attention_kernel_create_windowed), keyed by
+ *  (descriptor, type, window): the same window returns the same handle. */
+MFA_API int mfa_attention_kernel_cache_fetch_windowed(const mfa_attention_descriptor_t *descriptor,
+                                                      mfa_kernel_type_t type, const mfa_attention_window_t *window,
+                                                      const mfa_attention_kernel_t **out);
 /** Number of kernel objects the cache currently holds. */
 MFA_API int mfa_attention_kernel_cache_size(void);
 
@@ -417,7 +442,9 @@ MFA_API int mfa_attention_kernel_cache_size(void);
  *  With batch_count > 1 the independent problems are processed in chunks that rotate over three
  *  streams, so uploads, kernels and downloads of neighbouring chunks overlap (pass page-locked host
  *  memory to get the overlap; pageable memory still works, serialised by the driver).
- *  Every problem has its own K and V here (kv_group = 1): grouped K/V goes through mfa_attention_kernel_encode. */
+ *  Every problem has its own K and V here (kv_group = 1): grouped K/V goes through mfa_attention_kernel_encode.
+ *  There is no window here either: a sliding window goes through mfa_attention_kernel_create_windowed /
+ *  mfa_attention_kernel_cache_fetch_windowed and mfa_attention_kernel_encode. */
 MFA_API int mfa_attention_run_host(const mfa_attention_descriptor_t *descriptor, uint32_t run_mask,
                                    void *const host_buffers[MFA_BUFFER_COUNT], int device);
 

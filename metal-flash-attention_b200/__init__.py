@@ -119,6 +119,18 @@ class PagedKV(ctypes.Structure):
                          int(page_stride), int(page_size))
 
 
+class _CWindow(ctypes.Structure):
+    _fields_ = [("left", ctypes.c_int32), ("right", ctypes.c_int32)]
+
+
+def _window(window) -> "_CWindow":
+    left, right = (int(v) for v in window)
+    for name, v in (("left", left), ("right", right)):
+        if not -2**31 <= v < 2**31:   # (ctypes would wrap it; values in int32 are checked by the library)
+            raise MFAError(-2, f"Window: {name} {v} is outside [-1, {2**31 - 1}].")
+    return _CWindow(left, right)
+
+
 def _load():
     if not os.path.exists(_LIB_PATH):
         raise ImportError(
@@ -168,6 +180,10 @@ def _load():
     lib.mfa_attention_kernel_launch_count_paged.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
                                                             c.POINTER(PagedKV), c.POINTER(c.c_uint32)]
     lib.mfa_attention_kernel_cache_fetch.argtypes = [c.POINTER(_CDescriptor), c.c_int, c.POINTER(c.c_void_p)]
+    lib.mfa_attention_kernel_create_windowed.argtypes = [c.POINTER(_CKernelDescriptor), c.POINTER(_CWindow),
+                                                         c.POINTER(c.c_void_p)]
+    lib.mfa_attention_kernel_cache_fetch_windowed.argtypes = [c.POINTER(_CDescriptor), c.c_int, c.POINTER(_CWindow),
+                                                              c.POINTER(c.c_void_p)]
     lib.mfa_attention_kernel_cache_size.restype = c.c_int
     lib.mfa_attention_run_host.argtypes = [c.POINTER(_CDescriptor), c.c_uint32,
                                            c.POINTER(c.c_void_p * MFA_BUFFER_COUNT), c.c_int]
@@ -525,20 +541,35 @@ class AttentionKernel:
     (makeLibrary / makeComputePipelineState / setBuffer x10 / dispatchThreadgroups,
     SquareAttentionTest.swift:240-372) against DEVICE pointers."""
 
-    def __init__(self, descriptor: AttentionKernelDescriptor):
+    def __init__(self, descriptor: AttentionKernelDescriptor, window: Optional[Tuple[int, int]] = None):
+        """window: a sliding window (left, right) (mfa_attention_kernel_create_windowed): with delta = column - row,
+        query row i sees key j iff i + delta - left <= j <= i + delta + right, -1 leaving a side unbounded.  A causal
+        kernel takes right = 0 or -1; (W - 1, 0) is a window of W keys ending at the diagonal."""
         self._handle = ctypes.c_void_p()
         self._owned = True
-        _check(_lib.mfa_attention_kernel_create(ctypes.byref(descriptor._c), ctypes.byref(self._handle)))
+        if window is None:
+            _check(_lib.mfa_attention_kernel_create(ctypes.byref(descriptor._c), ctypes.byref(self._handle)))
+        else:
+            w = _window(window)
+            _check(_lib.mfa_attention_kernel_create_windowed(ctypes.byref(descriptor._c), ctypes.byref(w),
+                                                             ctypes.byref(self._handle)))
 
     @classmethod
-    def cached(cls, descriptor: AttentionDescriptor, type: AttentionKernelType) -> "AttentionKernel":
+    def cached(cls, descriptor: AttentionDescriptor, type: AttentionKernelType,
+               window: Optional[Tuple[int, int]] = None) -> "AttentionKernel":
         """mfa_attention_kernel_cache_fetch: the kernel object for (descriptor, type), built once per process and
-        owned by the library (the analogue of GEMMKernel.pipelineCache, GEMMDescriptor+PipelineCache.swift:16-36)."""
+        owned by the library (the analogue of GEMMKernel.pipelineCache, GEMMDescriptor+PipelineCache.swift:16-36).
+        window: a sliding window as in __init__ (mfa_attention_kernel_cache_fetch_windowed, keyed by the window too)."""
         self = cls.__new__(cls)
         self._handle = ctypes.c_void_p()
         self._owned = False
         c = descriptor._c()
-        _check(_lib.mfa_attention_kernel_cache_fetch(ctypes.byref(c), int(type), ctypes.byref(self._handle)))
+        if window is None:
+            _check(_lib.mfa_attention_kernel_cache_fetch(ctypes.byref(c), int(type), ctypes.byref(self._handle)))
+        else:
+            w = _window(window)
+            _check(_lib.mfa_attention_kernel_cache_fetch_windowed(ctypes.byref(c), int(type), ctypes.byref(w),
+                                                                  ctypes.byref(self._handle)))
         return self
 
     @staticmethod

@@ -4,6 +4,7 @@
 // Mirrors Sources/FlashAttention/Attention/AttentionKernel/AttentionKernel.swift.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <map>
@@ -20,6 +21,8 @@ struct mfa_attention_kernel {
   int backend;
   uint32_t threads, smem_bytes, par, trav, head;
   std::string source_name;
+  bool windowed;                   // mfa_attention_kernel_create_windowed
+  mfa_attention_window_t window;   // as given (-1: no bound on that side)
 };
 
 namespace mfa {
@@ -150,6 +153,17 @@ static int build_params(const mfa_attention_kernel *k, const mfa_function_consta
       return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Buffer ") + mfa_operand_name((mfa_operand_t)ops[i]) +
                                                   " (binding " + std::to_string(ops[i]) + ") is NULL.");
   return MFA_SUCCESS;
+}
+
+// The band a windowed kernel launches with over problems (or sequences) of at most `rows` x `columns`: -1 and anything
+// above rows + columns (which no band can exceed) become rows + columns, capped at INT32_MAX, and a causal kernel's
+// right side is the diagonal.  nullptr for a kernel without a window.
+static const Band *band_of(const mfa_attention_kernel *k, uint64_t rows, uint64_t columns, Band *out) {
+  if (!k->windowed) return nullptr;
+  const int64_t limit = static_cast<int64_t>(std::min<uint64_t>(rows + columns, 0x7fffffffu));
+  auto side = [&](int32_t v) { return static_cast<int32_t>(v < 0 || v > limit ? limit : v); };
+  *out = Band{side(k->window.left), k->descriptor.causal ? 0 : side(k->window.right)};
+  return out;
 }
 
 // The launch form of a packed-sequence table, after the checks the host can make without reading device memory
@@ -327,6 +341,29 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
   k->source_name = std::string("attention_") + typeNames[k->type] +
                    (k->backend == MFA_BACKEND_TCGEN05 ? "_tcgen05" : "_simt_fp32") + "<D=" + std::to_string(D) +
                    ">" + (kd->causal ? "_causal" : "");
+  k->windowed = false;
+  k->window = mfa_attention_window_t{-1, -1};
+  *out = k;
+  return MFA_SUCCESS;
+}
+
+int mfa_attention_kernel_create_windowed(const mfa_attention_kernel_descriptor_t *kd, const mfa_attention_window_t *window,
+                                         mfa_attention_kernel_t **out) {
+  if (!kd || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  if (!window) return fail(MFA_ERROR_INVALID_ARGUMENT, "Window: NULL window.");
+  if (window->left < -1)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Window: left " + std::to_string(window->left) + " is below -1.");
+  if (window->right < -1)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Window: right " + std::to_string(window->right) + " is below -1.");
+  if (kd->causal && window->right > 0)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Window: right " + std::to_string(window->right) +
+                                                " on a causal kernel, whose band ends at the diagonal (0 or -1).");
+  mfa_attention_kernel_t *k = nullptr;
+  const int status = mfa_attention_kernel_create(kd, &k);
+  if (status != MFA_SUCCESS) return status;
+  k->windowed = true;
+  k->window = *window;
+  k->source_name += "_window<" + std::to_string(window->left) + "," + std::to_string(window->right) + ">";
   *out = k;
   return MFA_SUCCESS;
 }
@@ -379,6 +416,7 @@ static int launch_count(const mfa_attention_kernel_t *kernel, const mfa_function
   if (status != MFA_SUCCESS) return status;
   const uint32_t sm_count = kernel->backend == MFA_BACKEND_TCGEN05 ? device_sm_count(current_device()) : 0;
   const bool convert_dO = d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q];
+  Band band;
   *out = 0;
   return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t, uint32_t batch) -> int {
     if (kernel->backend != MFA_BACKEND_TCGEN05)
@@ -389,7 +427,7 @@ static int launch_count(const mfa_attention_kernel_t *kernel, const mfa_function
                            .launches;
     else
       *out += staged + wgmma_plan(kernel->type, Dp, c->row, c->column, batch, group, d.split_min_blocks, d.split_max,
-                                  convert_dO, sm_count)
+                                  convert_dO, sm_count, band_of(kernel, c->row, c->column, &band))
                            .launches;
     return MFA_SUCCESS;
   });
@@ -466,8 +504,10 @@ int mfa_attention_kernel_encode_paged(const mfa_attention_kernel_t *kernel, cons
   AttentionParams p;
   if ((status = build_params(kernel, constants, buffers, p)) != MFA_SUCCESS) return status;
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  const cudaError_t e = kernel->backend == MFA_BACKEND_TCGEN05 ? launch_wgmma_forward_paged(p, pk, stream)
-                                                              : launch_simt_forward_paged(p, pk, stream);
+  Band storage;
+  const Band *band = band_of(kernel, p.R, pk.max_keys, &storage);
+  const cudaError_t e = kernel->backend == MFA_BACKEND_TCGEN05 ? launch_wgmma_forward_paged(p, pk, band, stream)
+                                                              : launch_simt_forward_paged(p, pk, band, stream);
   if (e != cudaSuccess)
     return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " (paged K/V) failed: " +
                                     cudaGetErrorString(e) + " " + last_launch_detail());
@@ -495,6 +535,8 @@ static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_const
   status = build_params(kernel, constants, buffers, p);
   if (status != MFA_SUCCESS) return status;
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  Band storage;
+  const Band *band = band_of(kernel, p.R, p.C, &storage);
 
   // Tensor-core family: operands with D % 8 != 0 or a transposed layout are staged row-major with pad8(D) columns, the
   // kernels run at the padded head dimension (the softmax scale stays 1 / sqrt(D) of the true D), and the FP32 outputs
@@ -547,15 +589,15 @@ static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_const
     }
     if (kernel->backend == MFA_BACKEND_TCGEN05) {
       switch (kernel->type) {
-        case MFA_FORWARD: e = launch_wgmma_forward(q, seq, stream); break;
-        case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, seq, stream); break;
-        default: e = launch_wgmma_backward_key_value(q, seq, stream); break;
+        case MFA_FORWARD: e = launch_wgmma_forward(q, seq, band, stream); break;
+        case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, seq, band, stream); break;
+        default: e = launch_wgmma_backward_key_value(q, seq, band, stream); break;
       }
     } else {
       switch (kernel->type) {
-        case MFA_FORWARD: e = launch_simt_forward(q, seq, stream); break;
-        case MFA_BACKWARD_QUERY: e = launch_simt_backward_query(q, seq, stream); break;
-        default: e = launch_simt_backward_key_value(q, seq, stream); break;
+        case MFA_FORWARD: e = launch_simt_forward(q, seq, band, stream); break;
+        case MFA_BACKWARD_QUERY: e = launch_simt_backward_query(q, seq, band, stream); break;
+        default: e = launch_simt_backward_key_value(q, seq, band, stream); break;
       }
     }
     if (e != cudaSuccess)
@@ -592,6 +634,8 @@ struct CacheKey {
   mfa_attention_descriptor_t descriptor;
   int type;
   unsigned table_generation;  // kernels created from an older parameter table are not handed out again
+  bool windowed;
+  mfa_attention_window_t window;
 };
 std::mutex g_cache_mutex;
 std::vector<std::pair<CacheKey, mfa_attention_kernel_t *>> g_kernel_cache;
@@ -610,12 +654,15 @@ bool same_descriptor(const mfa_attention_descriptor_t &a, const mfa_attention_de
 }
 }  // namespace
 
-int mfa_attention_kernel_cache_fetch(const mfa_attention_descriptor_t *descriptor, mfa_kernel_type_t type,
-                                     const mfa_attention_kernel_t **out) {
-  if (!descriptor || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+namespace {
+// window: nullptr for a kernel without one
+int cache_fetch(const mfa_attention_descriptor_t *descriptor, mfa_kernel_type_t type,
+                const mfa_attention_window_t *window, const mfa_attention_kernel_t **out) {
   std::lock_guard<std::mutex> lock(g_cache_mutex);
   for (const auto &entry : g_kernel_cache)
     if (entry.first.type == static_cast<int>(type) && entry.first.table_generation == parameter_table_generation() &&
+        entry.first.windowed == (window != nullptr) &&
+        (!window || (entry.first.window.left == window->left && entry.first.window.right == window->right)) &&
         same_descriptor(entry.first.descriptor, *descriptor)) {
       *out = entry.second;
       return MFA_SUCCESS;
@@ -624,10 +671,29 @@ int mfa_attention_kernel_cache_fetch(const mfa_attention_descriptor_t *descripto
   int status = mfa_attention_descriptor_kernel_descriptor(descriptor, type, &kd);
   if (status != MFA_SUCCESS) return status;
   mfa_attention_kernel_t *kernel = nullptr;
-  if ((status = mfa_attention_kernel_create(&kd, &kernel)) != MFA_SUCCESS) return status;
-  g_kernel_cache.push_back({CacheKey{*descriptor, static_cast<int>(type), parameter_table_generation()}, kernel});
+  if ((status = window ? mfa_attention_kernel_create_windowed(&kd, window, &kernel)
+                       : mfa_attention_kernel_create(&kd, &kernel)) != MFA_SUCCESS)
+    return status;
+  g_kernel_cache.push_back({CacheKey{*descriptor, static_cast<int>(type), parameter_table_generation(), window != nullptr,
+                                     window ? *window : mfa_attention_window_t{-1, -1}},
+                            kernel});
   *out = kernel;
   return MFA_SUCCESS;
+}
+}  // namespace
+
+int mfa_attention_kernel_cache_fetch(const mfa_attention_descriptor_t *descriptor, mfa_kernel_type_t type,
+                                     const mfa_attention_kernel_t **out) {
+  if (!descriptor || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  return cache_fetch(descriptor, type, nullptr, out);
+}
+
+int mfa_attention_kernel_cache_fetch_windowed(const mfa_attention_descriptor_t *descriptor, mfa_kernel_type_t type,
+                                              const mfa_attention_window_t *window,
+                                              const mfa_attention_kernel_t **out) {
+  if (!descriptor || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  if (!window) return fail(MFA_ERROR_INVALID_ARGUMENT, "Window: NULL window.");
+  return cache_fetch(descriptor, type, window, out);
 }
 
 int mfa_attention_kernel_cache_size(void) {

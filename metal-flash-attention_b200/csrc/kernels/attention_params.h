@@ -92,24 +92,39 @@ __device__ __forceinline__ uint32_t paged_row(const PagedKV &pk, const int32_t *
 }
 #endif
 
+// Sliding-window band (mfa_attention_window_t), a kernel argument of its own so that AttentionParams and the kernels
+// without a window keep their parameter lists: row i sees key j iff i + delta - left <= j <= i + delta + right.  The
+// host resolves -1 (no bound) and a causal kernel's right (the diagonal) before launch, and clamps both sides to
+// min(row + column, INT32_MAX), so the kernels see 0 <= left, right <= INT32_MAX; they add a side to delta or to an
+// index in 64 bits.
+struct Band {
+  int32_t left, right;
+};
+
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
-// seq: packed sequences, or nullptr for problems of the full R x C shape
-cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
-cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
-cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
+// seq: packed sequences, or nullptr for problems of the full R x C shape; band: a sliding window, or nullptr
+cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream);
+cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                       cudaStream_t stream);
+cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                           cudaStream_t stream);
 // paged K/V: the forward only, row-major operands
-cudaError_t launch_simt_forward_paged(const AttentionParams &p, const PagedKV &pk, cudaStream_t stream);
+cudaError_t launch_simt_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
+                                      cudaStream_t stream);
 void simt_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
                    uint32_t *head);
 
 // ---- tensor-core family (wgmma_attention.cu; the backend keeps its historical name "tcgen05" in the ABI) --------
 // 16-bit row-major operands with D % 8 == 0 and D <= kWgmmaMaxHead; kernel.cpp stages every other layout into that form.
 constexpr uint32_t kWgmmaMaxHead = 256;
-cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
-cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
-cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream);
+cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream);
+cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                        cudaStream_t stream);
+cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                            cudaStream_t stream);
 // paged K/V: the forward only, unsplit, grid (tiles of max_row, batch, count)
-cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, cudaStream_t stream);
+cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
+                                       cudaStream_t stream);
 
 // How the launcher of kernel `type` (mfa_kernel_type_t) runs one problem of padded head dimension D; every field is
 // derived from the kernels' compile-time configurations.  R, C and batch do not affect the geometry fields.
@@ -122,9 +137,10 @@ struct WgmmaPlan {
   uint32_t launches;                   // kernels the launcher issues
 };
 // batch = query problems, group = query problems per K/V problem (only the dK/dV plan, whose CTAs own K/V tiles,
-// depends on it)
+// depends on it).  band: a sliding window (host-resolved, as launched), whose width in traversal blocks, not the whole
+// traversal axis, is what the split cuts
 WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
-                     uint32_t max_splits, bool convert_dO, uint32_t sm_count);
+                     uint32_t max_splits, bool convert_dO, uint32_t sm_count, const Band *band = nullptr);
 // The plan of a packed call over `count` sequences of at most max_row x max_column: never split, grid (tiles of the
 // longest sequence, heads, count); the dO-conversion choice counts every CTA of that grid
 WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t max_column, uint32_t count,

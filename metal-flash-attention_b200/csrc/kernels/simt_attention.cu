@@ -17,6 +17,8 @@
 // can see, the mask is applied with the edge mask, and a row that sees no column gets O = 0, L = +inf.
 // Grouped K/V (p.group query problems per K/V problem): query problem b reads K / V problem b / p.group, and a dK/dV
 // CTA sums over the rows of every query problem of its group.
+// Sliding window (Band, the simt_band_* kernels at the end): row r sees column c iff
+// r + delta - left <= c <= r + delta + right; the loops visit only the 64-blocks that meet the CTA's band.
 //
 // Tiling: one CTA = 256 threads = a 64 x 64 block of the attention matrix; thread (tx, ty) owns
 // the 4 x 4 patch {rows ty+16i} x {cols tx+16j}.  Operands are staged through shared memory as
@@ -801,6 +803,280 @@ __global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel_va
   span_store<NCH>(accK, one, span_key(p, sdK, kvb, sp), c0, dlo, dhi, tx, ty);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Sliding window (Band): twins of the kernels above for the fixed-length (a span {0, R, 0, C}), packed and paged calls,
+// causal or not (the host passes a causal window as right = 0).  They visit only the 64-blocks that meet the band of
+// their rows (dK/dV: of their columns) and mask each element outside it.  Kernels of their own, with the band an
+// argument of its own, so that the kernels above and AttentionParams stay as they are.
+// ------------------------------------------------------------------------------------------------
+enum class Layout { kFixed, kPacked, kPaged };
+
+// The span a band kernel works on: the whole R x C problem, or sequence blockIdx.z
+template <Layout kLayout>
+__device__ __forceinline__ Span band_span(const AttentionParams &p, const Sequences &seq, const PagedKV &pk) {
+  Span sp;
+  if constexpr (kLayout == Layout::kFixed) {
+    sp.s = SequenceSpan{0, p.R, 0, p.C};
+  } else if constexpr (kLayout == Layout::kPacked) {
+    sp.s = sequence_span(seq, blockIdx.z);
+  } else {
+    sp.s = paged_span(pk, blockIdx.z);
+  }
+  sp.offset = static_cast<int>(sp.s.C) - static_cast<int>(sp.s.R);
+  return sp;
+}
+// The columns [*first, *end) of the 64-blocks that the rows [r0, min(r0 + 64, Rs)) see: [r0 + delta - left,
+// last row + delta + right] within [0, Cs), *first rounded down to a block
+__device__ __forceinline__ void band_columns(const Span &sp, const Band &band, uint32_t r0, uint32_t *first,
+                                             uint32_t *end) {
+  const int64_t lo = static_cast<int64_t>(r0) + sp.offset - band.left;
+  const int64_t hi = static_cast<int64_t>(min(r0 + kBlock, sp.s.R)) - 1 + sp.offset + band.right;
+  *first = lo <= 0 ? 0u : static_cast<uint32_t>(min(lo, static_cast<int64_t>(sp.s.C))) / kBlock * kBlock;
+  *end = hi < 0 ? 0u : static_cast<uint32_t>(min(hi + 1, static_cast<int64_t>(sp.s.C)));
+}
+// The rows [*first, *end) of the 64-blocks that see the columns [c0, min(c0 + 64, Cs)): [c0 - delta - right,
+// last column - delta + left] within [0, Rs), *first rounded down to a block
+__device__ __forceinline__ void band_rows(const Span &sp, const Band &band, uint32_t c0, uint32_t *first,
+                                          uint32_t *end) {
+  const int64_t lo = static_cast<int64_t>(c0) - sp.offset - band.right;
+  const int64_t hi = static_cast<int64_t>(min(c0 + kBlock, sp.s.C)) - 1 - sp.offset + band.left;
+  *first = lo <= 0 ? 0u : static_cast<uint32_t>(min(lo, static_cast<int64_t>(sp.s.R))) / kBlock * kBlock;
+  *end = hi < 0 ? 0u : static_cast<uint32_t>(min(hi + 1, static_cast<int64_t>(sp.s.R)));
+}
+// masked: column c is past the edge, or outside row r's band (64-bit: a side may be as large as INT32_MAX)
+__device__ __forceinline__ bool band_masked(const Span &sp, const Band &band, uint32_t r, uint32_t c) {
+  const int64_t d = static_cast<int64_t>(c) - r - sp.offset;  // column - (row + delta)
+  return c >= sp.s.C || d > band.right || -d > band.left;
+}
+// row r sees no column: the sequence has no keys, or its band lies wholly before or past them
+__device__ __forceinline__ bool band_empty(const Span &sp, const Band &band, uint32_t r) {
+  const int64_t diag = static_cast<int64_t>(r) + sp.offset;
+  return sp.s.C == 0 || diag + band.right < 0 || diag - band.left >= static_cast<int64_t>(sp.s.C);
+}
+
+// Paged K/V under a window: PagedOperand whose keys below `first` (before the band of every row of the CTA) read as
+// zero without touching their page-table entries or pages; keys at or past `seq` (the band's end) likewise
+struct BandPagedOperand {
+  PagedOperand page;
+  uint32_t first;
+};
+template <int COLS, int LD>
+__device__ __forceinline__ void load_tile(float *dst, const BandPagedOperand &op, uint32_t s0, uint32_t d0,
+                                          uint32_t dEnd, int tid) {
+  constexpr int kElems = kBlock * COLS;
+  const PagedOperand &pg = op.page;
+#pragma unroll 4
+  for (int e = tid; e < kElems; e += kThreads) {
+    const int s = e / COLS, d = e % COLS;
+    const uint32_t gs = s0 + s, gd = d0 + d;
+    float v = 0.f;
+    if (gs >= op.first && gs < pg.seq && gd < dEnd) {
+      const int page = min(max(__ldg(pg.table + (gs >> pg.page_shift)), 0), static_cast<int>(pg.pages) - 1);
+      const size_t row = (static_cast<size_t>(page) << pg.page_shift) | (gs & ((1u << pg.page_shift) - 1));
+      v = load_elem(pg.ptr, (row * pg.heads + pg.head) * pg.D + gd, pg.prec);
+    }
+    dst[s * LD + d] = v;
+  }
+}
+
+// The forward under a window, over the columns [c_first, c_end) with K / V read through OperandKV
+template <int NCH, class OperandKV>
+__device__ __forceinline__ void band_forward_body(const AttentionParams &p, const Span &sp, const Band &band,
+                                                  uint32_t b, uint32_t r0, const OperandKV &K, const OperandKV &V,
+                                                  uint32_t c_first, uint32_t c_end, float *smem) {
+  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const Operand Q = span_query(p, sQ, b, sp);
+  float m[4], l[4], acc[NCH][4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    m[i] = -FLT_MAX;
+    l[i] = FLT_TRUE_MIN;
+  }
+  zero_acc(acc);
+  for (uint32_t c0 = c_first; c0 < c_end; c0 += kBlock) {
+    float s[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
+    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float mx = -FLT_MAX;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (band_masked(sp, band, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
+        mx = fmaxf(mx, s[i][j]);
+      }
+      mx = row_max16(mx);
+      const float m_new = fmaxf(m[i], mx * p.scale_log2), correction = exp2f(m[i] - m_new);
+      float sum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float pv = exp2f(fmaf(s[i][j], p.scale_log2, -m_new));
+        sum += pv;
+        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv;
+      }
+      l[i] = fmaf(l[i], correction, row_sum16(sum));
+      m[i] = m_new;
+#pragma unroll
+      for (int q = 0; q < NCH; ++q)
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] *= correction;
+    }
+    accumulate<NCH>(acc, sP, V, c0, 0, p.D, sX, tid, tx, ty);
+  }
+  // a row that sees no key gets O = 0 and L = +inf
+  float inv[4];
+  bool empty[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    empty[i] = band_empty(sp, band, r0 + ty + 16 * i);
+    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
+  }
+  span_store<NCH>(acc, inv, span_query(p, sO, b, sp), r0, 0, p.D, tx, ty);
+  if (tx == 0 && p.buf[sL] != nullptr) {
+    char *Lbase = span_stats(p, sL, b, sp);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint32_t r = r0 + ty + 16 * i;
+      if (r < sp.s.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
+    }
+  }
+}
+
+template <int NCH, Layout kLayout>
+__global__ void __launch_bounds__(kThreads, 1) simt_band_forward_kernel(const AttentionParams p, const Sequences seq,
+                                                                        const PagedKV pk, const Band band) {
+  extern __shared__ __align__(16) float smem[];
+  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
+  const Span sp = band_span<kLayout>(p, seq, pk);
+  if (r0 >= sp.s.R) return;  // a tile past the sequence's end
+  uint32_t c_first, c_end;
+  band_columns(sp, band, r0, &c_first, &c_end);
+  if constexpr (kLayout == Layout::kPaged) {
+    const int32_t *table = pk.page_table + static_cast<size_t>(blockIdx.z) * pk.page_stride;
+    // (keys before the band of the tile's first row, and from c_end on, are never read)
+    const uint32_t first = static_cast<uint32_t>(
+        max(static_cast<int64_t>(r0) + sp.offset - band.left, static_cast<int64_t>(0)));
+    const BandPagedOperand K{{p.buf[sK], table, c_end, p.D, pk.kv_heads, b / p.group, pk.pages, pk.page_shift,
+                              p.prec[sK]},
+                             first},
+        V{{p.buf[sV], table, c_end, p.D, pk.kv_heads, b / p.group, pk.pages, pk.page_shift, p.prec[sV]}, first};
+    band_forward_body<NCH>(p, sp, band, b, r0, K, V, c_first, c_end, smem);
+  } else {
+    band_forward_body<NCH>(p, sp, band, b, r0, span_key(p, sK, b / p.group, sp), span_key(p, sV, b / p.group, sp),
+                           c_first, c_end, smem);
+  }
+}
+
+template <int NCH, Layout kLayout>
+__global__ void __launch_bounds__(kThreads, 1) simt_band_backward_query_kernel(const AttentionParams p,
+                                                                               const Sequences seq, const Band band) {
+  extern __shared__ __align__(16) float smem[];
+  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
+  const Span sp = band_span<kLayout>(p, seq, PagedKV{});
+  if (r0 >= sp.s.R) return;
+  const Operand Q = span_query(p, sQ, b, sp), K = span_key(p, sK, b / p.group, sp), V = span_key(p, sV, b / p.group, sp);
+  const Operand O = span_query(p, sO, b, sp), dO = span_query(p, sdO, b, sp);
+  const char *Lbase = span_stats(p, sL, b, sp);
+  char *Dbase = span_stats(p, sD, b, sp);
+  float Lrow[4], Drow[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t r = min(r0 + ty + 16 * i, sp.s.R - 1);
+    float part = 0.f;
+    for (uint32_t d = tx; d < p.D; d += 16)
+      part = fmaf(load_elem(dO.ptr, elem_index(dO, r, d), dO.prec), load_elem(O.ptr, elem_index(O, r, d), O.prec), part);
+    Drow[i] = row_sum16(part) * p.scale;
+    Lrow[i] = load_elem(Lbase, r, p.prec[sL]);
+    if (tx == 0 && r0 + ty + 16 * i < sp.s.R) store_elem(Dbase, r, p.prec[sD], Drow[i]);
+  }
+  float acc[NCH][4][4];
+  zero_acc(acc);
+  uint32_t c_first, c_end;
+  band_columns(sp, band, r0, &c_first, &c_end);
+  for (uint32_t c0 = c_first; c0 < c_end; c0 += kBlock) {
+    float s[4][4], dp[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
+    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
+    gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float pv = !band_masked(sp, band, r0 + ty + 16 * i, c0 + tx + 16 * j)
+                             ? exp2f(fmaf(s[i][j], p.scale_log2, -Lrow[i]))
+                             : 0.f;
+        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv * fmaf(dp[i][j], p.scale, -Drow[i]);
+      }
+    accumulate<NCH>(acc, sP, K, c0, 0, p.D, sX, tid, tx, ty);
+  }
+  const float one[4] = {1.f, 1.f, 1.f, 1.f};
+  span_store<NCH>(acc, one, span_query(p, sdQ, b, sp), r0, 0, p.D, tx, ty);
+}
+
+template <int NCH, Layout kLayout>
+__global__ void __launch_bounds__(kThreads, 1) simt_band_backward_key_value_kernel(const AttentionParams p,
+                                                                                   uint32_t dSlices,
+                                                                                   const Sequences seq,
+                                                                                   const Band band) {
+  extern __shared__ __align__(16) float smem[];
+  float *sA = smem, *sB = sA + kBlock * kLDA, *sPT = sB + kBlock * kLDA, *sX = sPT + kBlock * kLDP;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const uint32_t kvb = blockIdx.y / dSlices, slice = blockIdx.y % dSlices, c0 = blockIdx.x * kBlock;
+  const uint32_t dlo = slice * (NCH * kBlock), dhi = min(p.D, dlo + NCH * kBlock);
+  const Span sp = band_span<kLayout>(p, seq, PagedKV{});
+  if (c0 >= sp.s.C) return;  // (columns that no row sees still store their zeros)
+  const Operand K = span_key(p, sK, kvb, sp), V = span_key(p, sV, kvb, sp);
+  float accV[NCH][4][4], accK[NCH][4][4];
+  zero_acc(accV);
+  zero_acc(accK);
+  uint32_t r_first, r_end;
+  band_rows(sp, band, c0, &r_first, &r_end);
+  for (uint32_t b = kvb * p.group; b < (kvb + 1) * p.group; ++b) {
+    const Operand Q = span_query(p, sQ, b, sp), dO = span_query(p, sdO, b, sp);
+    const char *Lbase = span_stats(p, sL, b, sp), *Dbase = span_stats(p, sD, b, sp);
+    for (uint32_t r0 = r_first; r0 < r_end; r0 += kBlock) {
+      float s[4][4], dp[4][4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
+      gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
+      gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint32_t r = r0 + ty + 16 * i, rc = min(r, sp.s.R - 1);
+        const float Lr = load_elem(Lbase, rc, p.prec[sL]), Dr = load_elem(Dbase, rc, p.prec[sD]);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float e = r < sp.s.R && !band_masked(sp, band, r, c0 + tx + 16 * j)
+                              ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr))
+                              : 0.f;
+          dp[i][j] = e * fmaf(dp[i][j], p.scale, -Dr);  // dS
+          sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = e;  // P^T
+        }
+      }
+      accumulate<NCH>(accV, sPT, dO, r0, dlo, dhi, sX, tid, tx, ty);  // dV += P^T dO
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = dp[i][j];  // dS^T
+      accumulate<NCH>(accK, sPT, Q, r0, dlo, dhi, sX, tid, tx, ty);  // dK += dS^T Q
+    }
+  }
+  const float one[4] = {1.f, 1.f, 1.f, 1.f};
+  span_store<NCH>(accV, one, span_key(p, sdV, kvb, sp), c0, dlo, dhi, tx, ty);
+  span_store<NCH>(accK, one, span_key(p, sdK, kvb, sp), c0, dlo, dhi, tx, ty);
+}
+
 inline int chunks_for(uint32_t D) { return (D + kBlock - 1) / kBlock; }
 
 // Calls f(std::integral_constant<int, NCH>()) for the fewest of 1 / 2 / 4 / 8 (at most kMax) column chunks per CTA
@@ -835,32 +1111,50 @@ static dim3 simt_grid(uint32_t rows, uint32_t y, const Sequences *seq) {
   return dim3((rows + simt::kBlock - 1) / simt::kBlock, y, seq ? seq->count : 1);
 }
 
-cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
+cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream) {
   const dim3 grid = simt_grid(seq ? seq->max_row : p.R, p.batch, seq);
   return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
     constexpr int NCH = decltype(nch)::value;
+    using simt::Layout;
+    if (band && seq)
+      return simt::launch(simt::simt_band_forward_kernel<NCH, Layout::kPacked>, grid, stream, p, *seq, PagedKV{}, *band);
+    if (band)
+      return simt::launch(simt::simt_band_forward_kernel<NCH, Layout::kFixed>, grid, stream, p, Sequences{}, PagedKV{},
+                          *band);
     if (seq) return simt::launch(simt::simt_forward_kernel_varlen<NCH>, grid, stream, p, *seq);
     return simt::launch(simt::simt_forward_kernel<NCH>, grid, stream, p);
   });
 }
 
-cudaError_t launch_simt_forward_paged(const AttentionParams &p, const PagedKV &pk, cudaStream_t stream) {
+cudaError_t launch_simt_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
+                                      cudaStream_t stream) {
   const dim3 grid((pk.max_row + simt::kBlock - 1) / simt::kBlock, p.batch, pk.count);
   return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
+    if (band)
+      return simt::launch(simt::simt_band_forward_kernel<decltype(nch)::value, simt::Layout::kPaged>, grid, stream, p,
+                          Sequences{}, pk, *band);
     return simt::launch(simt::simt_forward_kernel_paged<decltype(nch)::value>, grid, stream, p, pk);
   });
 }
 
-cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
+cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                       cudaStream_t stream) {
   const dim3 grid = simt_grid(seq ? seq->max_row : p.R, p.batch, seq);
   return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
     constexpr int NCH = decltype(nch)::value;
+    using simt::Layout;
+    if (band && seq)
+      return simt::launch(simt::simt_band_backward_query_kernel<NCH, Layout::kPacked>, grid, stream, p, *seq, *band);
+    if (band)
+      return simt::launch(simt::simt_band_backward_query_kernel<NCH, Layout::kFixed>, grid, stream, p, Sequences{},
+                          *band);
     if (seq) return simt::launch(simt::simt_backward_query_kernel_varlen<NCH>, grid, stream, p, *seq);
     return simt::launch(simt::simt_backward_query_kernel<NCH>, grid, stream, p);
   });
 }
 
-cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
+cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                           cudaStream_t stream) {
   // two accumulators (dV, dK) per thread: keep at most 4 chunks (256 columns) of each in registers and
   // slice larger head dimensions over blockIdx.y (each slice recomputes S and dP).
   const int chunks = simt::chunks_for(p.D);
@@ -869,6 +1163,13 @@ cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Seque
     const uint32_t dSlices = (chunks + NCH - 1) / NCH;
     // one CTA row per K/V head
     const dim3 grid = simt_grid(seq ? seq->max_column : p.C, p.batch / p.group * dSlices, seq);
+    using simt::Layout;
+    if (band && seq)
+      return simt::launch(simt::simt_band_backward_key_value_kernel<NCH, Layout::kPacked>, grid, stream, p, dSlices,
+                          *seq, *band);
+    if (band)
+      return simt::launch(simt::simt_band_backward_key_value_kernel<NCH, Layout::kFixed>, grid, stream, p, dSlices,
+                          Sequences{}, *band);
     if (seq) return simt::launch(simt::simt_backward_key_value_kernel_varlen<NCH>, grid, stream, p, dSlices, *seq);
     return simt::launch(simt::simt_backward_key_value_kernel<NCH>, grid, stream, p, dSlices);
   });

@@ -20,6 +20,11 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+// Completes `bytes` of the transaction count the barrier's current phase expects without a copy (loads that a caller
+// decided not to issue)
+__device__ __forceinline__ void mbar_complete_tx(uint64_t *bar, uint32_t bytes) {
+  asm volatile("mbarrier.complete_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(

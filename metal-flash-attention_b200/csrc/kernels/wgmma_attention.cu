@@ -32,6 +32,14 @@
 // [pages][P][kv_heads][D] read through a 3-D tensor map {D, kv_heads, pool rows} with boxes of 64 x 1 x min(P, BN), so
 // each box lands as the same [rows][64] swizzled tile.  A stage takes BN / min(P, BN) boxes per column chunk and tensor,
 // each at the pool row of its page; thread 0 reads the block's page ids just before it issues its boxes.
+//
+// Sliding window (the band_* entry points, kBand in the shared bodies; Band in attention_params.h): row i sees key j iff
+// i + delta - left <= j <= i + delta + right, with left and right runtime arguments, so one instantiation serves every
+// window.  A CTA visits only the traversal blocks that meet its rows' (keys') band; only blocks that cross an edge of the
+// band are masked (mask_outside_band, whose edges are 64-bit: a side may be as large as INT32_MAX).  The bodies run with kCausal set, which brings the empty-row handling (reference value 0 for a
+// row without a key yet, L = -inf split partials, merge_splits<true>).  A fixed-length split range counts from the
+// tile's first visible block.  Paged: boxes of pages wholly outside the tile's band are not issued (their page-table
+// entries are never read); their bytes are completed on the barrier by hand and their rows zeroed.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -181,6 +189,15 @@ __device__ __forceinline__ void zero_rows(uint8_t *tile, uint32_t first) {
     reinterpret_cast<uint4 *>(tile + c * ROWS * 128 + first * 128)[i - c * units] = make_uint4(0u, 0u, 0u, 0u);
   }
 }
+// zero_rows of the rows [first, end)
+template <uint32_t DCH, uint32_t ROWS, uint32_t kThreads>
+__device__ __forceinline__ void zero_row_range(uint8_t *tile, uint32_t first, uint32_t end) {
+  const uint32_t units = (end - first) * 8;
+  for (uint32_t i = threadIdx.x; i < DCH * units; i += kThreads) {
+    const uint32_t c = i / units;
+    reinterpret_cast<uint4 *>(tile + c * ROWS * 128 + first * 128)[i - c * units] = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
 
 // FP32 accumulator rows -> global [rows][D] (row-major), columns < D, rows < limit
 template <int NR>
@@ -229,6 +246,37 @@ __device__ __forceinline__ uint32_t visible_query_blocks(uint32_t R, uint32_t qb
   return static_cast<uint32_t>(max(0, end - static_cast<int>(qs)));
 }
 
+// Sliding window: the blocks [first, end) of `block` rows of the axis of `length` rows that meet [lo, hi] (empty when
+// end <= first)
+template <uint32_t BLOCK>
+__device__ __forceinline__ int2 band_blocks(int64_t lo, int64_t hi, uint32_t length) {
+  const int first = lo <= 0 ? 0 : static_cast<int>(min(lo, static_cast<int64_t>(length)) / BLOCK);
+  const int end = hi < 0 ? 0 : static_cast<int>(min(hi / BLOCK + 1, static_cast<int64_t>((length + BLOCK - 1) / BLOCK)));
+  return make_int2(first, end);
+}
+// Forward / dQ: the key blocks the rows [row_base, min(row_base + rows, R)) see, keys [row_base + delta - left,
+// last row + delta + right]
+template <uint32_t BN>
+__device__ __forceinline__ int2 band_key_blocks(uint32_t row_base, uint32_t rows, uint32_t R, uint32_t C, int delta,
+                                                const Band &band) {
+  const int64_t last = static_cast<int64_t>(min(row_base + rows, R)) - 1;
+  return band_blocks<BN>(static_cast<int64_t>(row_base) + delta - band.left, last + delta + band.right, C);
+}
+// dK/dV: the query blocks that see the keys [key_base, min(key_base + keys, C)), queries [key_base - delta - right,
+// last key - delta + left]
+template <uint32_t BM>
+__device__ __forceinline__ int2 band_query_blocks(uint32_t key_base, uint32_t keys, uint32_t R, uint32_t C, int delta,
+                                                  const Band &band) {
+  const int64_t last = static_cast<int64_t>(min(key_base + keys, C)) - 1;
+  return band_blocks<BM>(static_cast<int64_t>(key_base) - delta - band.right, last - delta + band.left, R);
+}
+// The blocks of a CTA: the visible range [first, end) cut into split ranges of per_split blocks counted from `first`;
+// *start receives the CTA's first block
+__device__ __forceinline__ uint32_t band_split(int2 range, uint32_t split, uint32_t per_split, uint32_t *start) {
+  *start = static_cast<uint32_t>(range.x) + split * per_split;
+  return static_cast<uint32_t>(max(0, min(range.y, static_cast<int>(*start + per_split)) - static_cast<int>(*start)));
+}
+
 // ================================================================================================ masks
 // Causal: a block whose last key is `last_key` has elements past the diagonal for some row from `first_query` on
 __device__ __forceinline__ bool crosses_diagonal(int last_key, int first_query, int delta) {
@@ -251,6 +299,39 @@ __device__ __forceinline__ void mask_past_diagonal(float (&s)[NR], int row, int 
       if (kKeyRows ? r0 > c : c > r0) s[4 * i + e] = -INFINITY;
       if (kKeyRows ? r0 + 8 > c : c > r0 + 8) s[4 * i + 2 + e] = -INFINITY;
     }
+}
+
+// Sliding window: -inf for the elements outside the band (query + lower <= key <= query + upper; lower = delta - left,
+// upper = delta + right) of a 64 x N accumulator block, S (rows are queries, columns keys) or, kKeyRows, S^T (rows are
+// keys, columns queries); row and col0 as for mask_past_diagonal.  Each row's band of columns is formed in 64 bits and
+// clamped to the column range, so that neither a window side nor an index can overflow.
+__device__ __forceinline__ int clamp_column(int64_t c) {
+  return static_cast<int>(min(max(c, int64_t(-1)), static_cast<int64_t>(INT32_MAX)));
+}
+template <bool kKeyRows, int NR>
+__device__ __forceinline__ void mask_outside_band(float (&s)[NR], int row, int col0, int64_t lower, int64_t upper) {
+  int first[2], last[2];  // the columns [first, last] this thread's two rows keep
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t r = static_cast<int64_t>(row) + 8 * h;
+    first[h] = clamp_column(kKeyRows ? r - upper : r + lower);
+    last[h] = clamp_column(kKeyRows ? r - lower : r + upper);
+  }
+  const int c0 = col0 + 2 * static_cast<int>(threadIdx.x % 4);
+#pragma unroll
+  for (int i = 0; i < NR / 4; ++i)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int c = c0 + 8 * i + e;
+      if (c < first[0] || c > last[0]) s[4 * i + e] = -INFINITY;
+      if (c < first[1] || c > last[1]) s[4 * i + 2 + e] = -INFINITY;
+    }
+}
+// Sliding window: whether a block of keys [key_first, key_last] x queries [query_first, query_last] crosses an edge of
+// the band (64-bit, as mask_outside_band)
+__device__ __forceinline__ bool crosses_band(int key_first, int key_last, int query_first, int query_last,
+                                             int64_t lower, int64_t upper) {
+  return key_last > query_first + upper || key_first < query_last + lower;
 }
 
 // Keys past C: -inf in both rows of a 64 x N accumulator block of S whose first key column is key0
@@ -353,14 +434,51 @@ __device__ __forceinline__ void load_paged_kv(uint8_t *dst, uint32_t kv_bytes, c
   }
 }
 
+// Sliding window over a paged cache: the boxes of key block `block` that hold a key of [lo, hi] (the keys some row of
+// the tile sees, within [0, C)), as [first, end) box indices
+__device__ __forceinline__ uint2 band_boxes(uint32_t block, uint32_t BN, uint32_t box, int lo, int hi) {
+  const int key0 = static_cast<int>(block * BN);
+  const int first = max(lo - key0, 0) / static_cast<int>(box);
+  const int end = min(hi - key0, static_cast<int>(BN) - 1) / static_cast<int>(box) + 1;
+  return make_uint2(static_cast<uint32_t>(first), static_cast<uint32_t>(end));
+}
+// load_paged_kv of a windowed tile: only the boxes band_boxes names are issued, so the page-table entries and pages of
+// the others are never read; the bytes they would have brought are completed on `bar` by hand, and the caller zeroes
+// their rows
+template <uint32_t DCH, uint32_t BN>
+__device__ __forceinline__ void load_paged_kv_band(uint8_t *dst, uint32_t kv_bytes, const CUtensorMap *mapK,
+                                                   const CUtensorMap *mapV, uint64_t *bar, const PagedKV &pk,
+                                                   const int32_t *table, uint32_t block, uint32_t box, int lo, int hi,
+                                                   uint32_t kv_head) {
+  const uint2 kept = band_boxes(block, BN, box, lo, hi);
+  constexpr uint32_t kMaxBoxes = BN / 16;  // P >= 16
+  uint32_t rows[kMaxBoxes];
+#pragma unroll
+  for (uint32_t i = 0; i < kMaxBoxes; ++i)
+    rows[i] = i >= kept.x && i < kept.y ? paged_row(pk, table, block * BN + i * box) : 0u;
+  const uint32_t skipped = BN / box - (kept.y - kept.x);
+  if (skipped) mbar_complete_tx(bar, skipped * box * 128 * DCH * 2);
+#pragma unroll
+  for (uint32_t i = 0; i < kMaxBoxes; ++i) {
+    if (i < kept.x || i >= kept.y) continue;
+#pragma unroll
+    for (uint32_t c = 0; c < DCH; ++c) {
+      tma_load_3d(dst + c * BN * 128 + i * box * 128, mapK, bar, c * 64, kv_head, rows[i]);
+      tma_load_3d(dst + kv_bytes + c * BN * 128 + i * box * 128, mapV, bar, c * 64, kv_head, rows[i]);
+    }
+  }
+}
+
 // The body of the forward kernels.  R, C: the rows of each problem's buffers (paged: C is unused).  kPacked / kPaged:
 // the CTA works on sequence blockIdx.z, whose span replaces R, C and delta in the ranges and masks and offsets every
 // query row, and zeroes the rows of its last key block past the sequence's keys; never split.
-template <uint32_t DCH, bool kBF16, bool kCausal, KVLayout kLayout>
+// kBand: the sliding window `band` (with kCausal set).
+template <uint32_t DCH, bool kBF16, bool kCausal, KVLayout kLayout, bool kBand = false>
 __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUtensorMap &mapK, const CUtensorMap &mapV,
                                              float *__restrict__ O, void *__restrict__ L, uint32_t R, uint32_t C,
                                              uint32_t D, float scale_log2, int l_prec, const SplitArgs &sp, int delta,
-                                             uint32_t group, const Sequences &seq, const PagedKV &pk) {
+                                             uint32_t group, const Sequences &seq, const PagedKV &pk,
+                                             const Band &band = Band{}) {
   constexpr bool kVarlen = kLayout != KVLayout::kFixed;
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
@@ -382,14 +500,27 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
     kb0 = blockIdx.z * sp.blocks_per_split;
     per_split = sp.blocks_per_split;
   }
-  const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, span.R, span.C, delta, kb0, per_split);
+  uint32_t blocks;
+  if constexpr (kBand) {
+    blocks = band_split(band_key_blocks<BN>(row_base, Cfg::kTileM, span.R, span.C, delta, band),
+                        kVarlen ? 0u : blockIdx.z, per_split, &kb0);
+  } else {
+    blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, span.R, span.C, delta, kb0, per_split);
+  }
+  // window: the keys [band_lo, band_hi] some row of the tile sees, clamped into [-1, C]
+  const int64_t band_last = static_cast<int64_t>(min(row_base + Cfg::kTileM, span.R)) - 1;
+  const int band_lo = kBand ? static_cast<int>(max(static_cast<int64_t>(row_base) + delta - band.left, int64_t(-1))) : 0;
+  const int band_hi = kBand ? static_cast<int>(min(band_last + delta + band.right, static_cast<int64_t>(span.C))) : 0;
 
   // paged: this sequence's page_table row, and the rows of one TMA box
   const int32_t *table = kLayout == KVLayout::kPaged ? pk.page_table + static_cast<size_t>(blockIdx.z) * pk.page_stride
                                                      : nullptr;
   const uint32_t box = kLayout == KVLayout::kPaged ? min(1u << pk.page_shift, BN) : BN;
   auto load_kv = [&](uint32_t j, uint8_t *dst, uint64_t *bar) {
-    if constexpr (kLayout == KVLayout::kPaged) {
+    if constexpr (kLayout == KVLayout::kPaged && kBand) {
+      load_paged_kv_band<DCH, BN>(dst, Cfg::kKVBytes, &mapK, &mapV, bar, pk, table, kb0 + j, box, band_lo,
+                                  min(band_hi, static_cast<int>(span.C) - 1), kv_head);
+    } else if constexpr (kLayout == KVLayout::kPaged) {
       load_paged_kv<DCH, BN>(dst, Cfg::kKVBytes, &mapK, &mapV, bar, pk, table, kb0 + j, box, span.C, kv_head);
     } else {
       load_tile<DCH, BN>(dst, &mapK, bar, span.k0 + (kb0 + j) * BN, kv_head);
@@ -413,10 +544,23 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   ring.wait_resident();
   for (uint32_t j = 0; j < blocks; ++j) {
     ring.wait(j);
-    // the sequence's last key block: the next sequence's keys and values (packed), or whatever the page holds past C
-    if (kVarlen && (j + 1) * BN > span.C) {
-      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j), span.C - j * BN);
-      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, span.C - j * BN);
+    if constexpr (kLayout == KVLayout::kPaged && kBand) {
+      // the rows of the boxes that were not issued, and those past C
+      const uint2 kept = band_boxes(kb0 + j, BN, box, band_lo, min(band_hi, static_cast<int>(span.C) - 1));
+      const uint32_t first = kept.x * box, end = min(kept.y * box, span.C - (kb0 + j) * BN);
+      if (first > 0 || end < BN) {
+        zero_row_range<DCH, BN, Cfg::kThreads>(ring.stage(j), 0, first);
+        zero_row_range<DCH, BN, Cfg::kThreads>(ring.stage(j), end, BN);
+        zero_row_range<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, 0, first);
+        zero_row_range<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, end, BN);
+        fence_proxy_async_smem();
+        __syncthreads();
+      }
+    } else if (kVarlen && ((kBand ? kb0 : 0) + j + 1) * BN > span.C) {
+      // the sequence's last key block: the next sequence's keys and values (packed), or whatever the page holds past C
+      const uint32_t kb = (kBand ? kb0 : 0) + j;
+      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j), span.C - kb * BN);
+      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, span.C - kb * BN);
       fence_proxy_async_smem();
       __syncthreads();
     }
@@ -431,7 +575,13 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
 
     // keys past C: -inf before the row max
     if ((kb0 + j + 1) * BN > span.C) mask_past_edge(sc, (kb0 + j) * BN, span.C);
-    if constexpr (kCausal) {
+    if constexpr (kBand) {
+      const int key0 = static_cast<int>((kb0 + j) * BN), row = static_cast<int>(row_base + wg * kRows + frag_row(t));
+      const int64_t lower = static_cast<int64_t>(delta) - band.left, upper = static_cast<int64_t>(delta) + band.right;
+      if (crosses_band(key0, key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base),
+                       static_cast<int>(row_base + Cfg::kTileM) - 1, lower, upper))
+        mask_outside_band<false>(sc, row, key0, lower, upper);
+    } else if constexpr (kCausal) {
       const int key0 = static_cast<int>((kb0 + j) * BN);
       if (crosses_diagonal(key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base), delta))
         mask_past_diagonal<false>(sc, static_cast<int>(row_base + wg * kRows + frag_row(t)), key0, delta);
@@ -546,6 +696,37 @@ __global__ void __launch_bounds__(2 * kWG, 1)
                                                       group, Sequences{}, pk);
 }
 
+// Sliding window: the three forward kernels above with a band, causal or not (a causal window is a band with right = 0)
+template <uint32_t DCH, bool kBF16>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    band_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                       const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L, uint32_t R,
+                       uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp, int delta,
+                       uint32_t group, const Band band) {
+  forward_body<DCH, kBF16, true, KVLayout::kFixed, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, sp, delta,
+                                                         group, Sequences{}, PagedKV{}, band);
+}
+template <uint32_t DCH, bool kBF16>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    band_forward_packed_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                              const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
+                              uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, uint32_t group,
+                              const Sequences seq, const Band band) {
+  const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
+  forward_body<DCH, kBF16, true, KVLayout::kPacked, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, unsplit,
+                                                          0, group, seq, PagedKV{}, band);
+}
+template <uint32_t DCH, bool kBF16>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    band_forward_paged_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                             const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
+                             uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk,
+                             const Band band) {
+  const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
+  forward_body<DCH, kBF16, true, KVLayout::kPaged, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, unsplit, 0,
+                                                         group, Sequences{}, pk, band);
+}
+
 // ================================================================================================ backward dQ
 template <uint32_t DCH>
 struct QCfg {
@@ -571,11 +752,11 @@ struct BwdArgs {
   uint32_t group;  // query heads per K/V head: query head h reads K/V head h / group
 };
 
-// The body of the dQ kernels; kVarlen as in forward_body
-template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal, bool kVarlen>
+// The body of the dQ kernels; kVarlen and kBand as in forward_body
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal, bool kVarlen, bool kBand = false>
 __device__ __forceinline__ void backward_query_body(const CUtensorMap &mapQ, const CUtensorMap &mapdO,
                                                     const CUtensorMap &mapK, const CUtensorMap &mapV, const BwdArgs &a,
-                                                    const Sequences &seq) {
+                                                    const Sequences &seq, const Band &band = Band{}) {
   using Cfg = QCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -597,7 +778,13 @@ __device__ __forceinline__ void backward_query_body(const CUtensorMap &mapQ, con
     kb0 = blockIdx.z * a.blocks_per_split;
     per_split = a.blocks_per_split;
   }
-  const uint32_t blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, span.R, span.C, delta, kb0, per_split);
+  uint32_t blocks;
+  if constexpr (kBand) {
+    blocks = band_split(band_key_blocks<BN>(row_base, Cfg::kTileM, span.R, span.C, delta, band),
+                        kVarlen ? 0u : blockIdx.z, per_split, &kb0);
+  } else {
+    blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, span.R, span.C, delta, kb0, per_split);
+  }
 
   auto load_kv = [&](uint32_t j, uint8_t *dst, uint64_t *bar) {
     load_tile<DCH, BN>(dst, &mapK, bar, span.k0 + (kb0 + j) * BN, kv_head);
@@ -650,9 +837,10 @@ __device__ __forceinline__ void backward_query_body(const CUtensorMap &mapQ, con
   zero(dq);
   for (uint32_t j = 0; j < blocks; ++j) {
     ring.wait(j);
-    if (kVarlen && (j + 1) * BN > span.C) {  // the sequence's last key block: the next sequence's keys and values
-      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j), span.C - j * BN);
-      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, span.C - j * BN);
+    if (kVarlen && ((kBand ? kb0 : 0) + j + 1) * BN > span.C) {  // the sequence's last key block: the next sequence's
+      const uint32_t kb = (kBand ? kb0 : 0) + j;                  // keys and values
+      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j), span.C - kb * BN);
+      zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, span.C - kb * BN);
       fence_proxy_async_smem();
       __syncthreads();
     }
@@ -667,7 +855,13 @@ __device__ __forceinline__ void backward_query_body(const CUtensorMap &mapQ, con
     wgmma_wait<0>();
     fence_regs(sc);
     fence_regs(dp);
-    if constexpr (kCausal) {  // S -> -inf past the diagonal, so P = 0 there
+    if constexpr (kBand) {  // S -> -inf outside the band, so P = 0 there
+      const int key0 = static_cast<int>((kb0 + j) * BN);
+      const int64_t lower = static_cast<int64_t>(delta) - band.left, upper = static_cast<int64_t>(delta) + band.right;
+      if (crosses_band(key0, key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base),
+                       static_cast<int>(row_base + Cfg::kTileM) - 1, lower, upper))
+        mask_outside_band<false>(sc, static_cast<int>(r), key0, lower, upper);
+    } else if constexpr (kCausal) {  // S -> -inf past the diagonal, so P = 0 there
       const int key0 = static_cast<int>((kb0 + j) * BN);
       if (crosses_diagonal(key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base), delta))
         mask_past_diagonal<false>(sc, static_cast<int>(r), key0, delta);
@@ -714,6 +908,23 @@ __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
   backward_query_body<DCH, kBF16, kConvertDO, kCausal, true>(mapQ, mapdO, mapK, mapV, a, seq);
 }
 
+template <uint32_t DCH, bool kBF16, bool kConvertDO>
+__global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
+    band_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
+                              const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
+                              const BwdArgs a, const Band band) {
+  backward_query_body<DCH, kBF16, kConvertDO, true, false, true>(mapQ, mapdO, mapK, mapV, a, Sequences{}, band);
+}
+template <uint32_t DCH, bool kBF16, bool kConvertDO>
+__global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
+    band_backward_query_packed_wgmma(const __grid_constant__ CUtensorMap mapQ,
+                                     const __grid_constant__ CUtensorMap mapdO,
+                                     const __grid_constant__ CUtensorMap mapK,
+                                     const __grid_constant__ CUtensorMap mapV, const BwdArgs a, const Sequences seq,
+                                     const Band band) {
+  backward_query_body<DCH, kBF16, kConvertDO, true, true, true>(mapQ, mapdO, mapK, mapV, a, seq, band);
+}
+
 // ================================================================================================ backward dK/dV
 template <uint32_t DCH>
 struct KVCfg {
@@ -725,11 +936,13 @@ struct KVCfg {
   using Smem = SmemLayout<2 * kKBytes, kQBytes>;  // resident K, V; stage: Q, dO
 };
 
-// The body of the dK/dV kernels; kVarlen as in forward_body (a tile of keys whose sequence has no query stores zeros)
-template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal, bool kVarlen>
+// The body of the dK/dV kernels; kVarlen and kBand as in forward_body (a tile of keys whose sequence has no query, or
+// that no query sees, stores zeros)
+template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal, bool kVarlen, bool kBand = false>
 __device__ __forceinline__ void backward_key_value_body(const CUtensorMap &mapQ, const CUtensorMap &mapdO,
                                                         const CUtensorMap &mapK, const CUtensorMap &mapV,
-                                                        const BwdArgs &a, const Sequences &seq) {
+                                                        const BwdArgs &a, const Sequences &seq,
+                                                        const Band &band = Band{}) {
   using Cfg = KVCfg<DCH>;
   constexpr uint32_t BM = Cfg::BM, NA = Cfg::kAcc;
   extern __shared__ uint8_t smem_raw[];
@@ -750,10 +963,15 @@ __device__ __forceinline__ void backward_key_value_body(const CUtensorMap &mapQ,
     qb0 = blockIdx.z * a.blocks_per_split;
     per_split = a.blocks_per_split;
   }
-  // causal: this CTA's query blocks start at the first one that sees the tile's first key (query >= key_base - delta)
-  const uint32_t qs = kCausal ? max(qb0, first_query_block<BM>(key_base, delta)) : qb0;
-  const uint32_t blocks = kCausal ? visible_query_blocks<BM>(span.R, qb0, qs, per_split)
-                                  : min((span.R + BM - 1) / BM - qb0, per_split);
+  uint32_t qs, blocks;
+  if constexpr (kBand) {
+    blocks = band_split(band_query_blocks<BM>(key_base, Cfg::kTileN, span.R, span.C, delta, band),
+                        kVarlen ? 0u : blockIdx.z, per_split, &qs);
+  } else {
+    // causal: this CTA's query blocks start at the first one that sees the tile's first key (query >= key_base - delta)
+    qs = kCausal ? max(qb0, first_query_block<BM>(key_base, delta)) : qb0;
+    blocks = kCausal ? visible_query_blocks<BM>(span.R, qb0, qs, per_split) : min((span.R + BM - 1) / BM - qb0, per_split);
+  }
   // the same query blocks [qs, qs + blocks) of each of the group's query heads, as one flattened sequence n = g blocks
   // + i that drives the Q / dO ring: prefetch and barrier parity carry across head boundaries
   const uint32_t total = a.group * blocks;
@@ -816,7 +1034,13 @@ __device__ __forceinline__ void backward_key_value_body(const CUtensorMap &mapQ,
     wgmma_wait<0>();
     fence_regs(st);
     fence_regs(dpt);
-    if constexpr (kCausal) {  // S^T -> -inf where key > query + delta, so P^T = 0 there
+    if constexpr (kBand) {  // S^T -> -inf outside the band, so P^T = 0 there
+      const int qlo = static_cast<int>((qs + i) * BM), key = static_cast<int>(key_base + krow + frag_row(t));
+      const int64_t lower = static_cast<int64_t>(delta) - band.left, upper = static_cast<int64_t>(delta) + band.right;
+      if (crosses_band(static_cast<int>(key_base), static_cast<int>(key_base + Cfg::kTileN) - 1, qlo,
+                       qlo + static_cast<int>(BM) - 1, lower, upper))
+        mask_outside_band<true>(st, key, qlo, lower, upper);
+    } else if constexpr (kCausal) {  // S^T -> -inf where key > query + delta, so P^T = 0 there
       const int qlo = static_cast<int>((qs + i) * BM);
       if (crosses_diagonal(static_cast<int>(key_base + Cfg::kTileN) - 1, qlo, delta))
         mask_past_diagonal<true>(st, static_cast<int>(key_base + krow + frag_row(t)), qlo, delta);
@@ -872,6 +1096,23 @@ __global__ void __launch_bounds__(2 * kWG, 1)
                                               const __grid_constant__ CUtensorMap mapV, const BwdArgs a,
                                               const Sequences seq) {
   backward_key_value_body<DCH, kBF16, kConvertDO, kCausal, true>(mapQ, mapdO, mapK, mapV, a, seq);
+}
+
+template <uint32_t DCH, bool kBF16, bool kConvertDO>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    band_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
+                                  const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
+                                  const BwdArgs a, const Band band) {
+  backward_key_value_body<DCH, kBF16, kConvertDO, true, false, true>(mapQ, mapdO, mapK, mapV, a, Sequences{}, band);
+}
+template <uint32_t DCH, bool kBF16, bool kConvertDO>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    band_backward_key_value_packed_wgmma(const __grid_constant__ CUtensorMap mapQ,
+                                         const __grid_constant__ CUtensorMap mapdO,
+                                         const __grid_constant__ CUtensorMap mapK,
+                                         const __grid_constant__ CUtensorMap mapV, const BwdArgs a,
+                                         const Sequences seq, const Band band) {
+  backward_key_value_body<DCH, kBF16, kConvertDO, true, true, true>(mapQ, mapdO, mapK, mapV, a, seq, band);
 }
 
 static uint32_t chunks(uint32_t D) { return D <= 64 ? 1 : (D <= 128 ? 2 : 4); }
@@ -958,12 +1199,21 @@ static cudaError_t make_maps(const AttentionParams &p, bool with_dO, TensorMaps 
 }
 
 template <uint32_t DCH, bool kBF16, bool kCausal>
-cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, const Sequences *seq, cudaStream_t stream) {
+cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, const Sequences *seq, const Band *band,
+                           cudaStream_t stream) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
   auto kernel = attention_forward_wgmma<DCH, kBF16, kCausal>;
   TensorMaps m;
   cudaError_t e;
+  if (seq && band) {
+    auto packed = band_forward_packed_wgmma<DCH, kBF16>;
+    if ((e = prepare(packed, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess) return e;
+    packed<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]),
+                                                             p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL],
+                                                             p.group, *seq, *band);
+    return cudaGetLastError();
+  }
   if (seq) {  // packed sequences: unsplit
     auto packed = packed_forward_wgmma<DCH, kBF16, kCausal>;
     if ((e = prepare(packed, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess) return e;
@@ -972,7 +1222,9 @@ cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cons
                                                              p.group, *seq);
     return cudaGetLastError();
   }
-  if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess) return e;
+  if ((e = (band ? prepare(band_forward_wgmma<DCH, kBF16>, kSmemBytes) : prepare(kernel, kSmemBytes))) != cudaSuccess ||
+      (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess)
+    return e;
   SplitArgs sp{plan.blocks_per_split, plan.splits, p.batch, nullptr, nullptr};
   const uint64_t rows_total = static_cast<uint64_t>(p.batch) * p.R;
   if (plan.splits > 1) {
@@ -984,19 +1236,26 @@ cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cons
     sp.O_part = static_cast<float *>(ws);
     sp.L_part = sp.O_part + o_elems;
   }
-  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL],
-                                                           p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp, p.causal_offset,
-                                                           p.group);
+  if (band)
+    band_forward_wgmma<DCH, kBF16><<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(
+        m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp,
+        p.causal_offset, p.group, *band);
+  else
+    kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL],
+                                                             p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp,
+                                                             p.causal_offset, p.group);
   if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
   const uint64_t threads = rows_total * (p.D / 4);
-  merge_splits<kCausal><<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(
-      sp, static_cast<float *>(p.buf[sO]), p.buf[sL], p.prec[sL], rows_total, p.D);
+  // (a window can leave a row without a key in a split, or in every split, as causal does)
+  auto merge = band ? merge_splits<true> : merge_splits<kCausal>;
+  merge<<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(sp, static_cast<float *>(p.buf[sO]), p.buf[sL],
+                                                                          p.prec[sL], rows_total, p.D);
   return cudaGetLastError();
 }
 
 // Paged K/V: Q in the usual map, K and V as page pools of p.C rows, boxes of min(P, BN) rows
 template <uint32_t DCH, bool kBF16, bool kCausal>
-cudaError_t launch_forward_paged(const AttentionParams &p, const WgmmaPlan &plan, const PagedKV &pk,
+cudaError_t launch_forward_paged(const AttentionParams &p, const WgmmaPlan &plan, const PagedKV &pk, const Band *band,
                                  cudaStream_t stream) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
@@ -1004,13 +1263,19 @@ cudaError_t launch_forward_paged(const AttentionParams &p, const WgmmaPlan &plan
   const uint32_t box = min(1u << pk.page_shift, Cfg::BN);
   TensorMaps m;
   cudaError_t e;
-  if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess ||
+  if ((e = (band ? prepare(band_forward_paged_wgmma<DCH, kBF16>, kSmemBytes) : prepare(kernel, kSmemBytes))) !=
+          cudaSuccess ||
       (e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, Cfg::kQueryBoxRows)) != cudaSuccess ||
       (e = make_tensor_map_page_pool(&m.K, p.buf[sK], p.C, pk.kv_heads, p.D, box)) != cudaSuccess ||
       (e = make_tensor_map_page_pool(&m.V, p.buf[sV], p.C, pk.kv_heads, p.D, box)) != cudaSuccess)
     return e;
-  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL],
-                                                           p.R, p.D, p.scale_log2, p.prec[sL], p.group, pk);
+  if (band)
+    band_forward_paged_wgmma<DCH, kBF16><<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(
+        m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL], p.R, p.D, p.scale_log2, p.prec[sL], p.group, pk,
+        *band);
+  else
+    kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL],
+                                                             p.R, p.D, p.scale_log2, p.prec[sL], p.group, pk);
   return cudaGetLastError();
 }
 
@@ -1040,19 +1305,20 @@ static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
 // A backward kernel whose outputs are the BwdArgs fields out0 and, unless null, out1: FP32 tensors of `elems` elements
 // each.  Split: each split writes partial sums to the workspace, [split][output][elems], and sum_splits adds them into
 // the outputs.
-// Packed sequences (seq): `packed` runs instead, unsplit.
+// Packed sequences (seq): `packed` runs instead, unsplit.  `extra` (a window's Band) follows the kernels' arguments.
 using OutputSlot = float *BwdArgs::*;
-template <class Cfg, class Kernel, class PackedKernel>
+template <class Cfg, class Kernel, class PackedKernel, class... Extra>
 static cudaError_t launch_backward(Kernel kernel, PackedKernel packed, const AttentionParams &p, const WgmmaPlan &plan,
                                    const Sequences *seq, OutputSlot out0, OutputSlot out1, size_t elems,
-                                   cudaStream_t stream) {
+                                   cudaStream_t stream, const Extra &...extra) {
   constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
   const uint32_t outputs = out1 ? 2 : 1;
   TensorMaps m;
   cudaError_t e;
   if (seq) {
     if ((e = prepare(packed, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, true, &m)) != cudaSuccess) return e;
-    packed<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.dO, m.K, m.V, backward_args(p, plan), *seq);
+    packed<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.dO, m.K, m.V, backward_args(p, plan), *seq,
+                                                             extra...);
     return cudaGetLastError();
   }
   if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, true, &m)) != cudaSuccess) return e;
@@ -1068,7 +1334,7 @@ static cudaError_t launch_backward(Kernel kernel, PackedKernel packed, const Att
     a.*out0 = scratch;
     if (out1) a.*out1 = scratch + elems;
   }
-  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.dO, m.K, m.V, a);
+  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.dO, m.K, m.V, a, extra...);
   if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
   const size_t quads = elems / 4;  // D % 8 == 0
   sum_splits<<<dim3(static_cast<uint32_t>((quads + 255) / 256), outputs), 256, 0, stream>>>(
@@ -1093,7 +1359,7 @@ static cudaError_t dispatch(const AttentionParams &p, bool convert_dO, F f) {
 }  // namespace hop
 
 WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
-                     uint32_t max_splits, bool convert_dO, uint32_t sm_count) {
+                     uint32_t max_splits, bool convert_dO, uint32_t sm_count, const Band *band) {
   WgmmaPlan p{};
   auto geometry = [&](auto cfg) {
     using Cfg = decltype(cfg);
@@ -1115,7 +1381,14 @@ WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batc
   p.head = columns < padded ? columns : padded;
 
   const bool key_value = type == MFA_BACKWARD_KEY_VALUE;
-  const uint32_t tiles = ((key_value ? C : R) + p.par - 1) / p.par, total = ((key_value ? R : C) + p.trav - 1) / p.trav;
+  const uint32_t tiles = ((key_value ? C : R) + p.par - 1) / p.par;
+  uint32_t total = ((key_value ? R : C) + p.trav - 1) / p.trav;
+  if (band) {
+    // window: a tile's band covers par + left + right traversal rows, so it meets at most this many blocks (the
+    // kernels count each split range from the tile's first visible block)
+    const uint64_t width = (static_cast<uint64_t>(p.par) + band->left + band->right + p.trav - 1) / p.trav + 1;
+    if (width < total) total = static_cast<uint32_t>(width);
+  }
   // CTAs per tile row: one per query head, or for dK/dV one per K/V head (it walks the query heads of its group; the
   // split cuts each head's query blocks the same way)
   const uint32_t heads = key_value ? batch / group : batch;
@@ -1153,27 +1426,29 @@ static bool row_major_16bit(const AttentionParams &p) {
          p.D % 8 == 0 && p.D <= kWgmmaMaxHead;
 }
 
-static WgmmaPlan plan_for(int type, const AttentionParams &p, const Sequences *seq, bool convert_dO) {
+static WgmmaPlan plan_for(int type, const AttentionParams &p, const Sequences *seq, const Band *band,
+                          bool convert_dO) {
   const uint32_t sm_count = device_sm_count(current_device());
   if (seq)
     return wgmma_plan_sequences(type, p.D, seq->max_row, seq->max_column, seq->count, p.batch, p.group, convert_dO,
                                 sm_count);
-  return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, convert_dO, sm_count);
+  return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, convert_dO, sm_count, band);
 }
 
-cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
+cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream) {
   if (!row_major_16bit(p) || p.prec[sO] != FP32) {
     set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
     return cudaErrorInvalidValue;
   }
-  const WgmmaPlan plan = plan_for(MFA_FORWARD, p, seq, false);
+  const WgmmaPlan plan = plan_for(MFA_FORWARD, p, seq, band, false);
   return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
-    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, seq,
+    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, seq, band,
                                                                                                       stream);
   });
 }
 
-cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, cudaStream_t stream) {
+cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
+                                       cudaStream_t stream) {
   if (!row_major_16bit(p) || p.prec[sO] != FP32) {
     set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
     return cudaErrorInvalidValue;
@@ -1183,7 +1458,7 @@ cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &
                                               device_sm_count(current_device()));
   return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
     return hop::launch_forward_paged<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, pk,
-                                                                                                            stream);
+                                                                                                            band, stream);
   });
 }
 
@@ -1196,13 +1471,19 @@ static cudaError_t check_backward(const AttentionParams &p) {
   return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
+cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                        cudaStream_t stream) {
   if (cudaError_t e = check_backward(p)) return e;
   const bool convert = p.prec[sdO] != p.prec[sQ];
-  const WgmmaPlan plan = plan_for(MFA_BACKWARD_QUERY, p, seq, convert);
+  const WgmmaPlan plan = plan_for(MFA_BACKWARD_QUERY, p, seq, band, convert);
   return hop::dispatch(p, convert, [&](auto dch, auto bf16, auto cvt, auto causal) {
     constexpr uint32_t DCH = decltype(dch)::value;
     constexpr bool kBF16 = decltype(bf16)::value, kConvert = decltype(cvt)::value, kCausal = decltype(causal)::value;
+    if (band)
+      return hop::launch_backward<hop::QCfg<DCH>>(hop::band_backward_query_wgmma<DCH, kBF16, kConvert>,
+                                                  hop::band_backward_query_packed_wgmma<DCH, kBF16, kConvert>, p, plan,
+                                                  seq, &hop::BwdArgs::dQ, nullptr,
+                                                  static_cast<size_t>(p.batch) * p.R * p.D, stream, *band);
     return hop::launch_backward<hop::QCfg<DCH>>(hop::attention_backward_query_wgmma<DCH, kBF16, kConvert, kCausal>,
                                                 hop::packed_backward_query_wgmma<DCH, kBF16, kConvert, kCausal>,
                                                 p, plan, seq, &hop::BwdArgs::dQ, nullptr,
@@ -1210,10 +1491,11 @@ cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequence
   });
 }
 
-cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, cudaStream_t stream) {
+cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                            cudaStream_t stream) {
   if (cudaError_t e = check_backward(p)) return e;
   const bool convert = p.prec[sdO] != p.prec[sQ];
-  const WgmmaPlan plan = plan_for(MFA_BACKWARD_KEY_VALUE, p, seq, convert);
+  const WgmmaPlan plan = plan_for(MFA_BACKWARD_KEY_VALUE, p, seq, band, convert);
   AttentionParams q = p;
   if (plan.convert_dO_first) {
     const uint64_t elements = static_cast<uint64_t>(p.batch) * p.R * p.D;
@@ -1227,6 +1509,11 @@ cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequ
   return hop::dispatch(q, convert && !plan.convert_dO_first, [&](auto dch, auto bf16, auto cvt, auto causal) {
     constexpr uint32_t DCH = decltype(dch)::value;
     constexpr bool kBF16 = decltype(bf16)::value, kConvert = decltype(cvt)::value, kCausal = decltype(causal)::value;
+    if (band)
+      return hop::launch_backward<hop::KVCfg<DCH>>(
+          hop::band_backward_key_value_wgmma<DCH, kBF16, kConvert>,
+          hop::band_backward_key_value_packed_wgmma<DCH, kBF16, kConvert>, q, plan, seq, &hop::BwdArgs::dV,
+          &hop::BwdArgs::dK, static_cast<size_t>(q.batch / q.group) * q.C * q.D, stream, *band);
     return hop::launch_backward<hop::KVCfg<DCH>>(
         hop::attention_backward_key_value_wgmma<DCH, kBF16, kConvert, kCausal>,
         hop::packed_backward_key_value_wgmma<DCH, kBF16, kConvert, kCausal>, q, plan, seq, &hop::BwdArgs::dV,

@@ -123,6 +123,8 @@ struct AttentionDescriptor {  // AttentionDescriptor.swift:10-27
 using SequenceTable = mfa_sequence_table_t;
 // {count, max_row, row_offsets, column_lengths, page_table, page_stride, page_size}: a paged K/V cache, int32 device tables
 using PagedKV = mfa_paged_kv_t;
+// {left, right}: a sliding window of keys around the bottom-right aligned diagonal, -1 = unbounded on that side
+using AttentionWindow = mfa_attention_window_t;
 
 class AttentionKernel {  // AttentionKernel.swift:11-50
  public:
@@ -133,6 +135,18 @@ class AttentionKernel {  // AttentionKernel.swift:11-50
     mfa_attention_descriptor_t d = descriptor.c();
     const mfa_attention_kernel_t *out = nullptr;
     check(mfa_attention_kernel_cache_fetch(&d, static_cast<mfa_kernel_type_t>(type), &out));
+    handle_ = const_cast<mfa_attention_kernel_t *>(out);
+  }
+  // a sliding window {left, right} (mfa_attention_kernel_create_windowed / _cache_fetch_windowed): with delta = C - R,
+  // query row i sees key j iff i + delta - left <= j <= i + delta + right, -1 leaving a side unbounded
+  AttentionKernel(const AttentionKernelDescriptor &descriptor, const AttentionWindow &window) {
+    check(mfa_attention_kernel_create_windowed(&descriptor.c, &window, &handle_));
+  }
+  AttentionKernel(const AttentionDescriptor &descriptor, AttentionKernelType type, const AttentionWindow &window)
+      : owned_(false) {
+    mfa_attention_descriptor_t d = descriptor.c();
+    const mfa_attention_kernel_t *out = nullptr;
+    check(mfa_attention_kernel_cache_fetch_windowed(&d, static_cast<mfa_kernel_type_t>(type), &window, &out));
     handle_ = const_cast<mfa_attention_kernel_t *>(out);
   }
   ~AttentionKernel() { if (owned_) mfa_attention_kernel_destroy(handle_); }

@@ -331,6 +331,25 @@ public final class AttentionKernel {
     handle = out!
     owned = false
   }
+  /// A sliding window (left, right): with delta = column - row, query row i sees key j iff
+  /// i + delta - left <= j <= i + delta + right, -1 leaving a side unbounded (mfa_attention_kernel_create_windowed).
+  public init(descriptor: AttentionKernelDescriptor, window: (left: Int32, right: Int32)) {
+    var kd = descriptor.c
+    var w = mfa_attention_window_t(left: window.left, right: window.right)
+    var out: OpaquePointer?
+    check(mfa_attention_kernel_create_windowed(&kd, &w, &out))
+    handle = out!
+    owned = true
+  }
+  /// The cached kernel object of (descriptor, type, window) (mfa_attention_kernel_cache_fetch_windowed).
+  public init(cached descriptor: AttentionDescriptor, type: AttentionKernelType, window: (left: Int32, right: Int32)) {
+    var d = descriptor.c
+    var w = mfa_attention_window_t(left: window.left, right: window.right)
+    var out: OpaquePointer?
+    check(mfa_attention_kernel_cache_fetch_windowed(&d, mfa_kernel_type_t(type.rawValue), &w, &out))
+    handle = out!
+    owned = false
+  }
   deinit { if owned { mfa_attention_kernel_destroy(handle) } }
 
   public var blockDimensions: (parallelization: UInt16, traversal: UInt16, head: UInt16) {
