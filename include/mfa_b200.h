@@ -409,6 +409,68 @@ MFA_API int mfa_attention_kernel_create_windowed(const mfa_attention_kernel_desc
                                                  const mfa_attention_window_t *window, mfa_attention_kernel_t **out);
 
 /* ------------------------------------------------------------------------------------------ */
+/* Split-KV decode (library extension; forward only)                                          */
+/* ------------------------------------------------------------------------------------------ */
+/** A forward over packed sequences or a paged cache whose key range may be split across CTAs, FlashAttention's
+ *  flash_attn_with_kvcache(..., num_splits=).  A decode step has few query rows per sequence, so the unsplit grid of
+ *  _sequences / _paged (one CTA per 128-row query tile, head and sequence) can leave most SMs idle while each CTA walks
+ *  every key; the split grid gives each tile `splits` CTAs, each of which walks one key range and leaves a partial
+ *  output that a second launch merges.
+ *
+ *  Buffer layouts, table contracts, window handling, empty rows (O = 0, L = +inf), rows outside every sequence (never
+ *  written), the clamping of table contents and the isolation of NaN outside a sequence's keys are exactly those of
+ *  mfa_attention_kernel_encode_sequences / _paged, and every check those calls make is made identically.  Beyond them,
+ *  MFA_ERROR_INVALID_ARGUMENT, naming the field, for a NULL split, num_splits above 16, a backward kernel type
+ *  ("only the forward"), and, in mfa_attention_kernel_split_plan, both or neither table.
+ *
+ *  The plan reads only host values: the kernel, the constants, the table's host fields and the hint.
+ *    splits          num_splits when it is 1..16.  For 0: when the unsplit grid (tiles x batch_count x count) is at
+ *                    most half the SMs, the most ranges up to SMs / grid and the parameter-table row's maximum (at most
+ *                    16) whose ranges keep the row's minimum of key blocks (ceil(K / traversal block), K = the hint or
+ *                    the table's bound, and for a windowed kernel at most the blocks the band of one tile meets); a
+ *                    row whose minimum is 0 never splits.  On the device each tile's visible key blocks of its own
+ *                    sequence are cut by ceiling into that many ranges; a range may be empty.
+ *    heads_per_tile  kv_group when 2 <= kv_group <= 128 and max_row < 128 on the tensor cores (a tile then holds
+ *                    floor(128 / kv_group) query rows of each query head of one K/V head, which reads each K/V block
+ *                    once for the group instead of once per head), else 1.  The unsplit grid counts
+ *                    ceil(max_row / rows per head) tiles x batch_count / heads_per_tile heads x count.
+ *  A plan of one split and one head per tile launches the kernels of _sequences / _paged: the result, launches and
+ *  grid are theirs, bit for bit.  One split with packed heads gives the same bits too (each row's arithmetic is that
+ *  of the unpacked tile) in one launch.
+ *  A split plan launches the split kernel and a merge (plus the operand staging of a packed call, as _sequences does).
+ *  Split partials live in the per-(device, stream) workspace of the fixed-length split forward: encode a new size once
+ *  outside a CUDA-graph capture first.  MFA_BACKEND_SIMT_FP32 accepts these calls and always plans one split, whatever
+ *  num_splits says (its fixed-length calls do not split either). */
+typedef struct mfa_split_kv {
+  uint32_t num_splits; /* 0: the library's plan (above); 1..16: exactly this many key ranges per tile */
+  uint32_t max_column; /* planning hint only: a bound on every Cs.  0 = the table's bound (max_column of a sequence
+                          table; page_stride * P of a paged call).  Never a correctness contract: the key ranges are
+                          cut on the device from each sequence's real Cs. */
+} mfa_split_kv_t;
+
+typedef struct mfa_split_plan {
+  uint32_t splits;         /* key ranges per tile (1 = not split) */
+  uint32_t heads_per_tile; /* 1, or kv_group when the query heads of one K/V head share a tile */
+  uint32_t grid_size;      /* CTAs of the attention kernel */
+  uint32_t launch_count;   /* kernels one encode launches */
+} mfa_split_plan_t;
+
+MFA_API int mfa_attention_kernel_encode_sequences_split(const mfa_attention_kernel_t *kernel,
+                                                        const mfa_function_constants_t *constants,
+                                                        const mfa_sequence_table_t *sequences,
+                                                        const mfa_split_kv_t *split,
+                                                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
+MFA_API int mfa_attention_kernel_encode_paged_split(const mfa_attention_kernel_t *kernel,
+                                                    const mfa_function_constants_t *constants,
+                                                    const mfa_paged_kv_t *paged, const mfa_split_kv_t *split,
+                                                    void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
+/** The plan the two calls above follow; exactly one of sequences / paged non-NULL. */
+MFA_API int mfa_attention_kernel_split_plan(const mfa_attention_kernel_t *kernel,
+                                            const mfa_function_constants_t *constants,
+                                            const mfa_sequence_table_t *sequences, const mfa_paged_kv_t *paged,
+                                            const mfa_split_kv_t *split, mfa_split_plan_t *out);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Kernel cache keyed by descriptor                                                            */
 /* ------------------------------------------------------------------------------------------ */
 /** The analogue of the reference's pipeline cache (GEMMKernel.register(descriptor:) / pipelineCache[descriptor],

@@ -119,6 +119,22 @@ class PagedKV(ctypes.Structure):
                          int(page_stride), int(page_size))
 
 
+class SplitKV(ctypes.Structure):
+    """mfa_split_kv_t: a split-KV forward over packed sequences or a paged cache (FlashAttention's num_splits).
+    num_splits 0 lets the library plan; 1..16 is taken as given.  max_column: a planning hint bounding every
+    sequence's keys (0 = the table's bound), never a correctness contract."""
+    _fields_ = [("num_splits", ctypes.c_uint32), ("max_column", ctypes.c_uint32)]
+
+    def __init__(self, num_splits=0, max_column=0):
+        super().__init__(int(num_splits), int(max_column))
+
+
+class SplitPlan(ctypes.Structure):
+    """mfa_split_plan_t: key ranges per tile, query heads per tile, CTAs of the attention kernel, kernels launched."""
+    _fields_ = [("splits", ctypes.c_uint32), ("heads_per_tile", ctypes.c_uint32), ("grid_size", ctypes.c_uint32),
+                ("launch_count", ctypes.c_uint32)]
+
+
 class _CWindow(ctypes.Structure):
     _fields_ = [("left", ctypes.c_int32), ("right", ctypes.c_int32)]
 
@@ -179,6 +195,15 @@ def _load():
                                                          c.POINTER(PagedKV), c.POINTER(c.c_uint32)]
     lib.mfa_attention_kernel_launch_count_paged.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
                                                             c.POINTER(PagedKV), c.POINTER(c.c_uint32)]
+    lib.mfa_attention_kernel_encode_sequences_split.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                                c.POINTER(SequenceTable), c.POINTER(SplitKV),
+                                                                c.POINTER(c.c_void_p * MFA_BUFFER_COUNT), c.c_void_p]
+    lib.mfa_attention_kernel_encode_paged_split.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                            c.POINTER(PagedKV), c.POINTER(SplitKV),
+                                                            c.POINTER(c.c_void_p * MFA_BUFFER_COUNT), c.c_void_p]
+    lib.mfa_attention_kernel_split_plan.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                    c.POINTER(SequenceTable), c.POINTER(PagedKV), c.POINTER(SplitKV),
+                                                    c.POINTER(SplitPlan)]
     lib.mfa_attention_kernel_cache_fetch.argtypes = [c.POINTER(_CDescriptor), c.c_int, c.POINTER(c.c_void_p)]
     lib.mfa_attention_kernel_create_windowed.argtypes = [c.POINTER(_CKernelDescriptor), c.POINTER(_CWindow),
                                                          c.POINTER(c.c_void_p)]
@@ -634,19 +659,43 @@ class AttentionKernel:
         """Stands in for createSource() (AttentionKernel+Source.swift:11-55): the kernels are AOT-compiled."""
         return _lib.mfa_attention_kernel_source_name(self._handle).decode()
 
+    def splitPlan(self, constants: FunctionConstantValues, sequences: Optional[SequenceTable] = None,
+                  paged: Optional[PagedKV] = None, split: Optional[SplitKV] = None) -> SplitPlan:
+        """mfa_attention_kernel_split_plan: what encode(..., split=split) with this table launches.  Exactly one of
+        sequences / paged."""
+        out = SplitPlan()
+        _check(_lib.mfa_attention_kernel_split_plan(self._handle, ctypes.byref(constants._c),
+                                                    ctypes.byref(sequences) if sequences is not None else None,
+                                                    ctypes.byref(paged) if paged is not None else None,
+                                                    ctypes.byref(split) if split is not None else None,
+                                                    ctypes.byref(out)))
+        return out
+
     def encode(self, constants: FunctionConstantValues, buffers: Dict[AttentionOperand, int],
-               stream: int = 0, sequences: Optional[SequenceTable] = None, paged: Optional[PagedKV] = None) -> None:
+               stream: int = 0, sequences: Optional[SequenceTable] = None, paged: Optional[PagedKV] = None,
+               split: Optional[SplitKV] = None) -> None:
         """buffers: {AttentionOperand: device pointer}; stream: cudaStream_t as int (0 = default).  sequences: packed
         variable-length sequences over the rows of every problem (mfa_attention_kernel_encode_sequences).  paged: the
-        forward over a paged K/V cache, K and V pointing at the page pools (mfa_attention_kernel_encode_paged)."""
+        forward over a paged K/V cache, K and V pointing at the page pools (mfa_attention_kernel_encode_paged).
+        split: the split-KV forward over sequences= or paged= (mfa_attention_kernel_encode_sequences_split / _paged_split)."""
         _one_table(sequences, paged)
+        if split is not None and sequences is None and paged is None:
+            raise MFAError(-2, "split= needs sequences= or paged=: the fixed-length forward plans its own split.")
         arr = (ctypes.c_void_p * MFA_BUFFER_COUNT)()
         for op, ptr in buffers.items():
             binding = AttentionOperand(op).bufferBinding
             if binding is None:
                 raise MFAError(-2, f"Operand {AttentionOperand(op).name} has no buffer binding.")
             arr[binding] = ptr
-        if paged is not None:
+        if split is not None and paged is not None:
+            _check(_lib.mfa_attention_kernel_encode_paged_split(self._handle, ctypes.byref(constants._c),
+                                                                ctypes.byref(paged), ctypes.byref(split),
+                                                                ctypes.byref(arr), ctypes.c_void_p(stream)))
+        elif split is not None:
+            _check(_lib.mfa_attention_kernel_encode_sequences_split(self._handle, ctypes.byref(constants._c),
+                                                                    ctypes.byref(sequences), ctypes.byref(split),
+                                                                    ctypes.byref(arr), ctypes.c_void_p(stream)))
+        elif paged is not None:
             _check(_lib.mfa_attention_kernel_encode_paged(self._handle, ctypes.byref(constants._c), ctypes.byref(paged),
                                                           ctypes.byref(arr), ctypes.c_void_p(stream)))
         elif sequences is None:
@@ -661,5 +710,6 @@ class AttentionKernel:
 __all__ = [
     "AttentionDescriptor", "AttentionKernelDescriptor", "AttentionKernel", "AttentionKernelType",
     "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError", "SequenceTable", "PagedKV",
+    "SplitKV", "SplitPlan",
     "library_path", "version", "setParameterTable", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
 ]

@@ -249,9 +249,32 @@ static Sequences grid_of(const PagedKV &pk) {
   return Sequences{pk.row_offsets, nullptr, pk.rows, 0, pk.count, pk.max_row, 1};
 }
 
-// encode() of problems of the full R x C shape (seq == nullptr) or of packed sequences
+// A split-KV request (mfa_split_kv_t), after the checks the host can make; the table's checks come first
+constexpr uint32_t kMaxKeySplits = 16;
+static int split_of(const mfa_attention_kernel *k, const mfa_split_kv_t *s) {
+  if (!s) return fail(MFA_ERROR_INVALID_ARGUMENT, "Split-KV: NULL split.");
+  if (k->type != MFA_FORWARD)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Split-KV: only the forward kernel splits its key range.");
+  if (s->num_splits > kMaxKeySplits)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Split-KV: num_splits " + std::to_string(s->num_splits) + " is above " +
+                                                std::to_string(kMaxKeySplits) + ".");
+  return MFA_SUCCESS;
+}
+// The key bound a split plan cuts: the hint, or the table's bound (capped so that block counts cannot overflow)
+static uint32_t key_bound_of(const mfa_split_kv_t &s, const Sequences *seq, const PagedKV *pk) {
+  const uint32_t bound = s.max_column ? s.max_column : (seq ? seq->max_column : pk->max_keys);
+  return bound < 0x7fffffffu ? bound : 0x7fffffffu;
+}
+
+// encode() of problems of the full R x C shape (seq == nullptr) or of packed sequences; split: the split-KV forward
 static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, const Sequences *seq,
-                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
+                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, const mfa_split_kv_t *split = nullptr);
+static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
+                      const PagedKV *pk, const mfa_split_kv_t &split, mfa_split_plan_t *out);
+// encode() of a paged cache; split_call: the split-KV entry point, whose request `split` is checked after the table
+static int encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
+                        const mfa_paged_kv_t *table, bool split_call, const mfa_split_kv_t *split,
+                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
 
 }  // namespace mfa
 
@@ -492,26 +515,24 @@ int mfa_attention_kernel_launch_count_paged(const mfa_attention_kernel_t *kernel
   return MFA_SUCCESS;
 }
 
+int mfa_attention_kernel_split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                                    const mfa_sequence_table_t *sequences, const mfa_paged_kv_t *paged,
+                                    const mfa_split_kv_t *split, mfa_split_plan_t *out) {
+  if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  if ((sequences != nullptr) == (paged != nullptr))
+    return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Split-KV: pass exactly one of sequences and paged (") +
+                                                (sequences ? "both" : "neither") + " given).");
+  Sequences seq;
+  PagedKV pk;
+  int status = sequences ? sequences_of(kernel, c, sequences, &seq) : paged_of(kernel, c, paged, &pk);
+  if (status != MFA_SUCCESS || (status = split_of(kernel, split)) != MFA_SUCCESS) return status;
+  return split_plan(kernel, c, sequences ? &seq : nullptr, paged ? &pk : nullptr, *split, out);
+}
+
 int mfa_attention_kernel_encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
                                       const mfa_paged_kv_t *table, void *const buffers[MFA_BUFFER_COUNT],
                                       void *cuda_stream) {
-  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
-  PagedKV pk;
-  int status = paged_of(kernel, constants, table, &pk);
-  if (status != MFA_SUCCESS) return status;
-  if ((status = check_device()) != MFA_SUCCESS) return status;
-  AttentionParams p;
-  if ((status = build_params(kernel, constants, buffers, p)) != MFA_SUCCESS) return status;
-  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  Band storage;
-  const Band *band = band_of(kernel, p.R, pk.max_keys, &storage);
-  const cudaError_t e = kernel->backend == MFA_BACKEND_TCGEN05 ? launch_wgmma_forward_paged(p, pk, band, stream)
-                                                              : launch_simt_forward_paged(p, pk, band, stream);
-  if (e != cudaSuccess)
-    return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " (paged K/V) failed: " +
-                                    cudaGetErrorString(e) + " " + last_launch_detail());
-  return MFA_SUCCESS;
+  return encode_paged(kernel, constants, table, false, nullptr, buffers, cuda_stream);
 }
 
 int mfa_attention_kernel_encode_sequences(const mfa_attention_kernel_t *kernel,
@@ -524,11 +545,97 @@ int mfa_attention_kernel_encode_sequences(const mfa_attention_kernel_t *kernel,
   return status != MFA_SUCCESS ? status : encode(kernel, constants, &seq, buffers, cuda_stream);
 }
 
+int mfa_attention_kernel_encode_paged_split(const mfa_attention_kernel_t *kernel,
+                                            const mfa_function_constants_t *constants, const mfa_paged_kv_t *table,
+                                            const mfa_split_kv_t *split, void *const buffers[MFA_BUFFER_COUNT],
+                                            void *cuda_stream) {
+  return encode_paged(kernel, constants, table, true, split, buffers, cuda_stream);
+}
+
+int mfa_attention_kernel_encode_sequences_split(const mfa_attention_kernel_t *kernel,
+                                                const mfa_function_constants_t *constants,
+                                                const mfa_sequence_table_t *table, const mfa_split_kv_t *split,
+                                                void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
+  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
+  Sequences seq;
+  int status = sequences_of(kernel, constants, table, &seq);
+  if (status != MFA_SUCCESS || (status = split_of(kernel, split)) != MFA_SUCCESS) return status;
+  return encode(kernel, constants, &seq, buffers, cuda_stream, split);
+}
+
 }  // extern "C"
 
 namespace mfa {
+// The plan of a split-KV call over packed sequences (seq) or a paged cache (pk): wgmma_plan_split per batch slice on
+// the tensor cores (a paged call is one slice), one split on the SIMT family
+static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
+                      const PagedKV *pk, const mfa_split_kv_t &split, mfa_split_plan_t *out) {
+  *out = mfa_split_plan_t{1, 1, 0, 0};
+  if (kernel->backend != MFA_BACKEND_TCGEN05) {
+    int status;
+    if (pk) {
+      const Sequences grid = grid_of(*pk);
+      status = grid_size(kernel, c, &grid, &out->grid_size);
+      out->launch_count = 1;
+    } else if ((status = grid_size(kernel, c, seq, &out->grid_size)) == MFA_SUCCESS) {
+      status = launch_count(kernel, c, seq, &out->launch_count);
+    }
+    return status;
+  }
+  const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
+  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, staged = __builtin_popcount(staged_operands(kernel));
+  uint32_t group = 1;
+  const int status = kv_group_of(c, &group);
+  if (status != MFA_SUCCESS) return status;
+  const uint32_t sm_count = device_sm_count(current_device());
+  Band storage;
+  const Band *band = band_of(kernel, c->row, pk ? pk->max_keys : c->column, &storage);
+  const uint32_t key_bound = key_bound_of(split, seq, pk);
+  const uint32_t max_row = pk ? pk->max_row : seq->max_row, count = pk ? pk->count : seq->count;
+  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t h0, uint32_t batch) -> int {
+    const WgmmaPlan plan = wgmma_plan_split(Dp, max_row, key_bound, count, batch, group, d.split_min_blocks,
+                                            d.split_max ? d.split_max : 1, split.num_splits, sm_count, band);
+    if (h0 == 0) {
+      out->splits = plan.splits;
+      out->heads_per_tile = plan.heads_per_tile;
+    }
+    out->grid_size += plan.grid.x * plan.grid.y * plan.grid.z;
+    out->launch_count += (pk ? 0 : staged) + plan.launches;
+    return MFA_SUCCESS;
+  });
+}
+
+static int encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
+                        const mfa_paged_kv_t *table, bool split_call, const mfa_split_kv_t *split,
+                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
+  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
+  PagedKV pk;
+  int status = paged_of(kernel, constants, table, &pk);
+  if (status != MFA_SUCCESS) return status;
+  if (split_call && (status = split_of(kernel, split)) != MFA_SUCCESS) return status;
+  if ((status = check_device()) != MFA_SUCCESS) return status;
+  AttentionParams p;
+  if ((status = build_params(kernel, constants, buffers, p)) != MFA_SUCCESS) return status;
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  Band storage;
+  const Band *band = band_of(kernel, p.R, pk.max_keys, &storage);
+  cudaError_t e;
+  if (kernel->backend != MFA_BACKEND_TCGEN05)
+    e = launch_simt_forward_paged(p, pk, band, stream);
+  else if (split)
+    e = launch_wgmma_forward_split(p, nullptr, &pk, band, split->num_splits, key_bound_of(*split, nullptr, &pk), stream);
+  else
+    e = launch_wgmma_forward_paged(p, pk, band, stream);
+  if (e != cudaSuccess)
+    return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " (paged K/V) failed: " +
+                                    cudaGetErrorString(e) + " " + last_launch_detail());
+  return MFA_SUCCESS;
+}
+
 static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, const Sequences *seq,
-                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
+                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, const mfa_split_kv_t *split) {
   int status = check_device();
   if (status != MFA_SUCCESS) return status;
   AttentionParams p;
@@ -589,7 +696,11 @@ static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_const
     }
     if (kernel->backend == MFA_BACKEND_TCGEN05) {
       switch (kernel->type) {
-        case MFA_FORWARD: e = launch_wgmma_forward(q, seq, band, stream); break;
+        case MFA_FORWARD:
+          e = split ? launch_wgmma_forward_split(q, seq, nullptr, band, split->num_splits,
+                                                 key_bound_of(*split, seq, nullptr), stream)
+                    : launch_wgmma_forward(q, seq, band, stream);
+          break;
         case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, seq, band, stream); break;
         default: e = launch_wgmma_backward_key_value(q, seq, band, stream); break;
       }

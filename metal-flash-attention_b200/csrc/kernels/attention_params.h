@@ -125,6 +125,10 @@ cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequ
 // paged K/V: the forward only, unsplit, grid (tiles of max_row, batch, count)
 cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
                                        cudaStream_t stream);
+// split-KV forward of packed sequences (seq) or a paged cache (pk), exactly one non-null: the plan of
+// wgmma_plan_split; one split runs launch_wgmma_forward / launch_wgmma_forward_paged unchanged
+cudaError_t launch_wgmma_forward_split(const AttentionParams &p, const Sequences *seq, const PagedKV *pk,
+                                       const Band *band, uint32_t num_splits, uint32_t key_bound, cudaStream_t stream);
 
 // How the launcher of kernel `type` (mfa_kernel_type_t) runs one problem of padded head dimension D; every field is
 // derived from the kernels' compile-time configurations.  R, C and batch do not affect the geometry fields.
@@ -135,6 +139,7 @@ struct WgmmaPlan {
   uint32_t blocks_per_split, splits;   // traversal blocks per CTA; ranges of the traversal axis (1 = not split)
   bool convert_dO_first;               // dK/dV: the BF16 dO is converted to FP16 in a pass of its own
   uint32_t launches;                   // kernels the launcher issues
+  uint32_t heads_per_tile;             // split-KV packed / paged forward: query heads per tile (1 elsewhere)
 };
 // batch = query problems, group = query problems per K/V problem (only the dK/dV plan, whose CTAs own K/V tiles,
 // depends on it).  band: a sliding window (host-resolved, as launched), whose width in traversal blocks, not the whole
@@ -145,6 +150,16 @@ WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batc
 // longest sequence, heads, count); the dO-conversion choice counts every CTA of that grid
 WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t max_column, uint32_t count,
                                uint32_t batch, uint32_t group, bool convert_dO, uint32_t sm_count);
+// The plan of a split-KV packed or paged forward (mfa_split_plan_t): grid (tiles of max_row x splits, batch, count).
+// key_bound bounds every sequence's keys (the caller's hint, or the table's bound); num_splits 0 lets the parameter-table
+// row's tuning columns choose, as choose_splits does, over ceil(key_bound / BN) blocks (a window's band width when
+// narrower); n >= 1 is taken as given.  Every value is host-visible, so launcher, split_plan, grid size and launch
+// count agree.  heads_per_tile: the group (2..128) when max_row < 128, so that a tile holds m = 128 / group rows of
+// each query head of a K/V head instead of padding rows; grid (ceil(max_row / m) x splits, batch / heads_per_tile,
+// count).
+WgmmaPlan wgmma_plan_split(uint32_t D, uint32_t max_row, uint32_t key_bound, uint32_t count, uint32_t batch,
+                           uint32_t group, uint32_t min_blocks, uint32_t max_splits, uint32_t num_splits,
+                           uint32_t sm_count, const Band *band);
 
 // operand staging for the tensor-core family (pad_head.cu): a [batch][seq][D] (or, transposed, [batch][D][seq]) operand
 // is copied to row-major [batch][seq][Dp] with zero padding columns, and an FP32 output computed in that form is copied

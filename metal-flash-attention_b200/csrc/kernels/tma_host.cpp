@@ -47,10 +47,10 @@ namespace {
 enum MapLayout : uint32_t { kMatrix = 0, kPagePool = 1 };
 struct MapKey {
   const void *base;
-  uint32_t seq, D, batch, boxCols, boxRows, dtype, layout;
+  uint32_t seq, D, batch, boxCols, boxRows, boxDepth, dtype, layout;
   bool operator==(const MapKey &o) const {
     return base == o.base && seq == o.seq && D == o.D && batch == o.batch && boxCols == o.boxCols &&
-           boxRows == o.boxRows && dtype == o.dtype && layout == o.layout;
+           boxRows == o.boxRows && boxDepth == o.boxDepth && dtype == o.dtype && layout == o.layout;
   }
 };
 struct MapEntry {
@@ -68,13 +68,13 @@ uint32_t map_slot(const MapKey &k) {
 }
 }  // namespace
 
-// kMatrix: [batch][seq][D], boxes of boxCols x boxRows x 1.  kPagePool: [seq][batch][D] (seq pool rows of `batch`
+// kMatrix: [batch][seq][D], boxes of boxCols x boxRows x boxDepth (boxDepth consecutive problems).  kPagePool: [seq][batch][D] (seq pool rows of `batch`
 // heads each), dims {D, batch, seq}, boxes of boxCols x 1 x boxRows: one head of boxRows consecutive rows, which lands
 // in shared memory as the same [boxRows][boxCols] tile.
 static cudaError_t encode(CUtensorMap *map, CUtensorMapDataType dtype, uint32_t elemBytes, const void *base,
                           uint32_t seq, uint32_t D, uint32_t batch, uint32_t boxCols, uint32_t boxRows,
-                          MapLayout layout) {
-  const MapKey key{base, seq, D, batch, boxCols, boxRows, static_cast<uint32_t>(dtype), layout};
+                          MapLayout layout, uint32_t boxDepth = 1) {
+  const MapKey key{base, seq, D, batch, boxCols, boxRows, boxDepth, static_cast<uint32_t>(dtype), layout};
   MapEntry &entry = g_map_cache[map_slot(key)];
   if (entry.valid && entry.key == key) {
     *map = entry.map;
@@ -93,7 +93,7 @@ static cudaError_t encode(CUtensorMap *map, CUtensorMapDataType dtype, uint32_t 
   const bool pool = layout == kPagePool;
   cuuint64_t dims[3] = {D, pool ? batch : seq, pool ? seq : batch};
   cuuint64_t strides[2] = {row, (pool ? batch : seq) * row};
-  cuuint32_t box[3] = {boxCols, pool ? 1 : boxRows, pool ? boxRows : 1};
+  cuuint32_t box[3] = {boxCols, pool ? 1 : boxRows, pool ? boxRows : boxDepth};
   cuuint32_t elemStrides[3] = {1, 1, 1};
   CUresult r = fn(map, dtype, 3, const_cast<void *>(base), dims, strides, box, elemStrides, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -109,9 +109,9 @@ static cudaError_t encode(CUtensorMap *map, CUtensorMapDataType dtype, uint32_t 
 }
 
 cudaError_t make_tensor_map_16bit(CUtensorMap *map, const void *base, uint32_t seq, uint32_t D, uint32_t batch,
-                                  uint32_t box_rows) {
+                                  uint32_t box_rows, uint32_t box_depth) {
   // BF16 and FP16 move identically through TMA; the 16-bit "type" only matters for OOB fill (zeros).
-  return encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, seq, D, batch, 64, box_rows, kMatrix);
+  return encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, seq, D, batch, 64, box_rows, kMatrix, box_depth);
 }
 
 cudaError_t make_tensor_map_page_pool(CUtensorMap *map, const void *base, uint32_t rows, uint32_t heads, uint32_t D,

@@ -26,7 +26,9 @@
 //
 // Packed sequences (the packed_* entry points, kVarlen in the shared bodies): grid.z is the sequence; a CTA takes its
 // sequence's rows from the offset tables, leaves when its tile starts past the sequence's end, works on the sequence's
-// R, C and delta, and zeroes the rows of its last streamed block that belong to the next sequence.  Never split.
+// R, C and delta, and zeroes the rows of its last streamed block that belong to the next sequence.  Unsplit, except in
+// the split_forward_* kernels (kSplit): there grid.x is tiles x splits, each CTA walks one ceiling-cut range of its
+// tile's visible key blocks, and merge_sequence_splits merges the partials of the sequence's rows.
 //
 // Paged K/V (the paged_* forward, KVLayout::kPaged in forward_body): queries packed as above, keys and values in pools
 // [pages][P][kv_heads][D] read through a 3-D tensor map {D, kv_heads, pool rows} with boxes of 64 x 1 x min(P, BN), so
@@ -327,6 +329,23 @@ __device__ __forceinline__ void mask_outside_band(float (&s)[NR], int row, int c
       if (c < first[1] || c > last[1]) s[4 * i + 2 + e] = -INFINITY;
     }
 }
+// mask_outside_band of S for a thread whose two rows are the query rows row0 and row1 (not row0 + 8: a tile that
+// packs several query heads, forward_body's kSplit)
+template <int NR>
+__device__ __forceinline__ void mask_rows_outside_band(float (&s)[NR], int row0, int row1, int col0, int64_t lower,
+                                                       int64_t upper) {
+  const int first0 = clamp_column(row0 + lower), last0 = clamp_column(row0 + upper);
+  const int first1 = clamp_column(row1 + lower), last1 = clamp_column(row1 + upper);
+  const int c0 = col0 + 2 * static_cast<int>(threadIdx.x % 4);
+#pragma unroll
+  for (int i = 0; i < NR / 4; ++i)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int c = c0 + 8 * i + e;
+      if (c < first0 || c > last0) s[4 * i + e] = -INFINITY;
+      if (c < first1 || c > last1) s[4 * i + 2 + e] = -INFINITY;
+    }
+}
 // Sliding window: whether a block of keys [key_first, key_last] x queries [query_first, query_last] crosses an edge of
 // the band (64-bit, as mask_outside_band)
 __device__ __forceinline__ bool crosses_band(int key_first, int key_last, int query_first, int query_last,
@@ -357,12 +376,8 @@ struct SplitArgs {
 // O[row][4 quad ..] and L[row] from the partials of every split (row = head * R + r): one thread per (row, 4 columns).
 // Causal: a split that saw no key of a row left L = -inf (weight 0); a row that no split saw gets O = 0, L = +inf.
 template <bool kCausal>
-__global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O, void *L, int l_prec, uint64_t rows_total,
-                                                    uint32_t D) {
-  const uint64_t idx = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const uint64_t row = idx / (D / 4);
-  if (row >= rows_total) return;
-  const uint32_t quad = static_cast<uint32_t>(idx % (D / 4));
+__device__ __forceinline__ void merge_row(const SplitArgs &sp, float *O, void *L, int l_prec, uint64_t rows_total,
+                                          uint32_t D, uint64_t row, uint32_t quad) {
   float lmax = -INFINITY;
   for (uint32_t s = 0; s < sp.splits; ++s) lmax = fmaxf(lmax, __ldcg(sp.L_part + s * rows_total + row));
   const float lref = kCausal && lmax == -INFINITY ? 0.f : lmax;
@@ -381,6 +396,28 @@ __global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O
   const float inv = empty ? 0.f : 1.0f / denom;
   *reinterpret_cast<float4 *>(O + row * D + 4 * quad) = make_float4(acc.x * inv, acc.y * inv, acc.z * inv, acc.w * inv);
   if (quad == 0) store_stat(L, row, l_prec, empty ? INFINITY : lmax + log2f(denom));
+}
+template <bool kCausal>
+__global__ void __launch_bounds__(128) merge_splits(const SplitArgs sp, float *O, void *L, int l_prec, uint64_t rows_total,
+                                                    uint32_t D) {
+  const uint64_t idx = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const uint64_t row = idx / (D / 4);
+  if (row >= rows_total) return;
+  merge_row<kCausal>(sp, O, L, l_prec, rows_total, D, row, static_cast<uint32_t>(idx % (D / 4)));
+}
+
+// merge_splits of a split packed or paged forward: grid (row chunks of the longest sequence, heads, sequences); the
+// sequence's rows come from row_offsets, clamped into [0, R] as the forward clamps them, and only rows inside the
+// sequence are written.  Always empty-aware: a sequence without keys, or a row whose band misses a chunk, leaves
+// L = -inf partials without a causal mask.
+__global__ void __launch_bounds__(128) merge_sequence_splits(const SplitArgs sp, float *O, void *L, int l_prec,
+                                                             uint32_t R, uint32_t D, const int32_t *row_offsets) {
+  uint32_t q0;
+  const uint32_t rows = sequence_rows(row_offsets, blockIdx.z, R, &q0);
+  const uint64_t idx = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x, r = idx / (D / 4);
+  if (r >= rows) return;
+  merge_row<true>(sp, O, L, l_prec, static_cast<uint64_t>(sp.batch) * R, D, static_cast<uint64_t>(blockIdx.y) * R + q0 + r,
+                  static_cast<uint32_t>(idx % (D / 4)));
 }
 
 // kPar / kTrav: rows of the parallelization / traversal axis per CTA / per pipeline stage; kQueryBoxRows /
@@ -471,23 +508,33 @@ __device__ __forceinline__ void load_paged_kv_band(uint8_t *dst, uint32_t kv_byt
 
 // The body of the forward kernels.  R, C: the rows of each problem's buffers (paged: C is unused).  kPacked / kPaged:
 // the CTA works on sequence blockIdx.z, whose span replaces R, C and delta in the ranges and masks and offsets every
-// query row, and zeroes the rows of its last key block past the sequence's keys; never split.
+// query row, and zeroes the rows of its last key block past the sequence's keys.
 // kBand: the sliding window `band` (with kCausal set).
-template <uint32_t DCH, bool kBF16, bool kCausal, KVLayout kLayout, bool kBand = false>
+// kSplit (packed / paged only): blockIdx.x is tile * sp.splits + split; the CTA takes chunk `split` of ceil(n / splits)
+// blocks of the n key blocks its tile sees in its own sequence, and leaves a partial (an empty chunk: O = 0, L = -inf)
+// at [split][head][packed row] of the workspace for merge_sequence_splits (one split: O and L themselves).  Its tile
+// holds m = kTileM / hpt query rows of each of the hpt query heads blockIdx.y * hpt + [0, hpt) (hpt = 1, or the K/V
+// group): tile row t is head blockIdx.y * hpt + t / m, query row tile * m + t % m; rows hpt * m .. kTileM - 1 are never
+// stored.  Each row is masked with its own query row, so its arithmetic is that of the unpacked tile.
+template <uint32_t DCH, bool kBF16, bool kCausal, KVLayout kLayout, bool kBand = false, bool kSplit = false>
 __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUtensorMap &mapK, const CUtensorMap &mapV,
                                              float *__restrict__ O, void *__restrict__ L, uint32_t R, uint32_t C,
                                              uint32_t D, float scale_log2, int l_prec, const SplitArgs &sp, int delta,
                                              uint32_t group, const Sequences &seq, const PagedKV &pk,
-                                             const Band &band = Band{}) {
+                                             const Band &band = Band{}, uint32_t hpt = 1) {
   constexpr bool kVarlen = kLayout != KVLayout::kFixed;
+  static_assert(!kSplit || kVarlen, "the fixed-length forward splits through blockIdx.z");
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
   const Ring<typename Cfg::Smem> ring(smem_raw);  // resident Q; step j: K and V of key block kb0 + j
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
+  const uint32_t tile = kSplit ? blockIdx.x / sp.splits : blockIdx.x;
   // (causal: unlike dQ, the forward gains nothing measurable from starting the tiles with the most key blocks first)
-  const uint32_t head = blockIdx.y, row_base = blockIdx.x * Cfg::kTileM;
-  const uint32_t kv_head = head / group;  // grouped K/V: the query heads of a group read one K/V head
+  const uint32_t tile_rows = kSplit ? Cfg::kTileM / hpt : Cfg::kTileM;  // query rows of each head in the tile (m)
+  const uint32_t head = blockIdx.y, row_base = tile * tile_rows;
+  // grouped K/V: the query heads of a group read one K/V head (kSplit: the tile's heads start at head * hpt)
+  const uint32_t kv_head = (kSplit ? head * hpt : head) / group;
   SequenceSpan span{0, R, 0, C};
   uint32_t kb0, per_split;
   if constexpr (kVarlen) {
@@ -501,14 +548,21 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
     per_split = sp.blocks_per_split;
   }
   uint32_t blocks;
-  if constexpr (kBand) {
+  if constexpr (kSplit) {
+    // the visible blocks [first, end) of the tile in its sequence, cut by ceiling (a chunk may hold no block)
+    const int2 range = kBand ? band_key_blocks<BN>(row_base, tile_rows, span.R, span.C, delta, band)
+                             : make_int2(0, static_cast<int>(key_blocks<BN, kCausal>(row_base, tile_rows, span.R,
+                                                                                     span.C, delta, 0, per_split)));
+    const uint32_t n = static_cast<uint32_t>(max(range.y - range.x, 0));
+    blocks = band_split(range, blockIdx.x % sp.splits, (n + sp.splits - 1) / sp.splits, &kb0);
+  } else if constexpr (kBand) {
     blocks = band_split(band_key_blocks<BN>(row_base, Cfg::kTileM, span.R, span.C, delta, band),
                         kVarlen ? 0u : blockIdx.z, per_split, &kb0);
   } else {
     blocks = key_blocks<BN, kCausal>(row_base, Cfg::kTileM, span.R, span.C, delta, kb0, per_split);
   }
   // window: the keys [band_lo, band_hi] some row of the tile sees, clamped into [-1, C]
-  const int64_t band_last = static_cast<int64_t>(min(row_base + Cfg::kTileM, span.R)) - 1;
+  const int64_t band_last = static_cast<int64_t>(min(row_base + tile_rows, span.R)) - 1;
   const int band_lo = kBand ? static_cast<int>(max(static_cast<int64_t>(row_base) + delta - band.left, int64_t(-1))) : 0;
   const int band_hi = kBand ? static_cast<int>(min(band_last + delta + band.right, static_cast<int64_t>(span.C))) : 0;
 
@@ -534,13 +588,21 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   }
   ring.init();
   ring.start(
-      [&](uint8_t *dst, uint64_t *bar) { load_tile<DCH, Cfg::kTileM>(dst, &mapQ, bar, span.q0 + row_base, head); },
+      [&](uint8_t *dst, uint64_t *bar) {
+        // (kSplit: boxes of m rows x hpt heads; the rows past hpt * m are never loaded, their bytes completed by hand)
+        load_tile<DCH, Cfg::kTileM>(dst, &mapQ, bar, span.q0 + row_base, kSplit ? head * hpt : head);
+        if (kSplit && hpt * tile_rows < Cfg::kTileM) mbar_complete_tx(bar, (Cfg::kTileM - hpt * tile_rows) * 128 * DCH);
+      },
       blocks, load_kv);
 
   const uint32_t sQ = smem_u32(ring.base);
   float o[NO / 2];
   zero(o);
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  // kSplit: the tile rows of this thread (the second is 8 below the first) and their query rows
+  const uint32_t trow0 = wg * kRows + frag_row(t);
+  const int qrow0 = static_cast<int>(row_base + trow0 % tile_rows);
+  const int qrow1 = static_cast<int>(row_base + (trow0 + 8) % tile_rows);
   ring.wait_resident();
   for (uint32_t j = 0; j < blocks; ++j) {
     ring.wait(j);
@@ -556,9 +618,9 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
         fence_proxy_async_smem();
         __syncthreads();
       }
-    } else if (kVarlen && ((kBand ? kb0 : 0) + j + 1) * BN > span.C) {
+    } else if (kVarlen && ((kBand || kSplit ? kb0 : 0) + j + 1) * BN > span.C) {
       // the sequence's last key block: the next sequence's keys and values (packed), or whatever the page holds past C
-      const uint32_t kb = (kBand ? kb0 : 0) + j;
+      const uint32_t kb = (kBand || kSplit ? kb0 : 0) + j;
       zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j), span.C - kb * BN);
       zero_rows<DCH, BN, Cfg::kThreads>(ring.stage(j) + Cfg::kKVBytes, span.C - kb * BN);
       fence_proxy_async_smem();
@@ -575,7 +637,15 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
 
     // keys past C: -inf before the row max
     if ((kb0 + j + 1) * BN > span.C) mask_past_edge(sc, (kb0 + j) * BN, span.C);
-    if constexpr (kBand) {
+    if constexpr (kSplit) {
+      // each row against its own query row: causal is the band (-inf, delta]
+      const int key0 = static_cast<int>((kb0 + j) * BN);
+      const int64_t lower = kBand ? static_cast<int64_t>(delta) - band.left : -(int64_t(1) << 40);
+      const int64_t upper = static_cast<int64_t>(delta) + (kBand ? band.right : 0);
+      if ((kBand || kCausal) && crosses_band(key0, key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base),
+                                             static_cast<int>(row_base + tile_rows) - 1, lower, upper))
+        mask_rows_outside_band(sc, qrow0, qrow1, key0, lower, upper);
+    } else if constexpr (kBand) {
       const int key0 = static_cast<int>((kb0 + j) * BN), row = static_cast<int>(row_base + wg * kRows + frag_row(t));
       const int64_t lower = static_cast<int64_t>(delta) - band.left, upper = static_cast<int64_t>(delta) + band.right;
       if (crosses_band(key0, key0 + static_cast<int>(BN) - 1, static_cast<int>(row_base),
@@ -644,6 +714,29 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  if constexpr (kSplit) {
+    // each of this thread's two rows at its own (head, query row); one split: O and L, else the partial of this range
+    const uint32_t split = blockIdx.x % sp.splits;
+#pragma unroll
+    for (uint32_t h = 0; h < 2; ++h) {
+      const uint32_t trow = trow0 + 8 * h, r = row_base + trow % tile_rows, qh = head * hpt + trow / tile_rows;
+      if (trow >= hpt * tile_rows || r >= span.R) continue;
+      const float l = h ? l1 : l0, mrow = h ? m1 : m0, inv = l == 0.f ? 0.f : 1.0f / l;
+      const size_t row = (sp.splits == 1 ? static_cast<size_t>(qh) : static_cast<size_t>(split) * sp.batch + qh) * R +
+                         span.q0 + r;
+      float *out = (sp.splits == 1 ? O : sp.O_part) + row * D;
+#pragma unroll
+      for (int i = 0; i < NO / 8; ++i) {
+        const uint32_t col = 8 * i + 2 * (t % 4);
+        if (col < D)
+          *reinterpret_cast<float2 *>(out + col) = make_float2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+      }
+      if (t % 4 == 0)
+        store_stat(sp.splits == 1 ? L : sp.L_part, row, sp.splits == 1 ? l_prec : FP32,
+                   l == 0.f ? (sp.splits == 1 ? INFINITY : -INFINITY) : mrow + log2f(l));
+    }
+    return;
+  }
   const uint32_t row0 = row_base + wg * kRows;
   // unsplit: O and L straight to the caller; split: the normalised partial of this key range
   const size_t slice = static_cast<size_t>(blockIdx.z) * sp.batch + head;
@@ -725,6 +818,47 @@ __global__ void __launch_bounds__(2 * kWG, 1)
   const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
   forward_body<DCH, kBF16, true, KVLayout::kPaged, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, unsplit, 0,
                                                          group, Sequences{}, pk, band);
+}
+
+// Split-KV packed and paged forwards (kSplit): grid (tiles of the longest query sequence x sp.splits, heads / hpt,
+// sequences), hpt query heads per tile; with more than one split the partials are merged by merge_sequence_splits.
+// Windowed twins with a band.
+template <uint32_t DCH, bool kBF16, bool kCausal>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    split_forward_packed_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                               const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
+                               uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, uint32_t group,
+                               const Sequences seq, const SplitArgs sp, uint32_t hpt) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPacked, false, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec,
+                                                                    sp, 0, group, seq, PagedKV{}, Band{}, hpt);
+}
+template <uint32_t DCH, bool kBF16, bool kCausal>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    split_forward_paged_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                              const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
+                              uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk,
+                              const SplitArgs sp, uint32_t hpt) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged, false, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec,
+                                                                   sp, 0, group, Sequences{}, pk, Band{}, hpt);
+}
+template <uint32_t DCH, bool kBF16>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    split_forward_packed_band_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                    const __grid_constant__ CUtensorMap mapV, float *__restrict__ O,
+                                    void *__restrict__ L, uint32_t R, uint32_t C, uint32_t D, float scale_log2,
+                                    int l_prec, uint32_t group, const Sequences seq, const Band band,
+                                    const SplitArgs sp, uint32_t hpt) {
+  forward_body<DCH, kBF16, true, KVLayout::kPacked, true, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, sp,
+                                                                0, group, seq, PagedKV{}, band, hpt);
+}
+template <uint32_t DCH, bool kBF16>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    split_forward_paged_band_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                   const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
+                                   uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group,
+                                   const PagedKV pk, const Band band, const SplitArgs sp, uint32_t hpt) {
+  forward_body<DCH, kBF16, true, KVLayout::kPaged, true, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, sp, 0,
+                                                               group, Sequences{}, pk, band, hpt);
 }
 
 // ================================================================================================ backward dQ
@@ -1151,6 +1285,19 @@ static uint32_t choose_splits(uint32_t items, uint32_t total_blocks, uint32_t sm
   return best;
 }
 
+// choose_splits of a split packed or paged forward, whose kernels cut each tile's visible key blocks by ceiling on the
+// device: the bound need not divide evenly, and every range but the last has at least min_blocks of `total_blocks`
+static uint32_t choose_key_splits(uint64_t items, uint32_t total_blocks, uint32_t sm_count, uint32_t min_blocks,
+                                  uint32_t max_splits) {
+  if (items * 2 > sm_count || min_blocks == 0) return 1;
+  if (max_splits > 16) max_splits = 16;
+  const uint32_t target = sm_count / static_cast<uint32_t>(items);
+  uint32_t best = 1;
+  for (uint32_t s = 2; s <= target && s <= max_splits; ++s)
+    if (total_blocks / s >= min_blocks) best = s;
+  return best;
+}
+
 // Traversal blocks per CTA of a backward kernel: all of them, or (few CTAs for the SMs) ranges of at least min_blocks,
 // at most max_splits (<= 8) ranges
 static uint32_t choose_blocks_per_split(uint32_t ctas, uint32_t total_blocks, uint32_t sm_count, uint32_t min_blocks,
@@ -1279,6 +1426,62 @@ cudaError_t launch_forward_paged(const AttentionParams &p, const WgmmaPlan &plan
   return cudaGetLastError();
 }
 
+// Split-KV packed (seq) or paged (pk) forward of plan.splits key ranges and plan.heads_per_tile query heads per tile
+// (not both 1): with splits > 1 the split kernel writes partials [split][head][row] into the workspace and
+// merge_sequence_splits merges each sequence's rows into O and L; with one split it writes O and L itself.  Q is read in
+// boxes of m = kTileM / heads_per_tile rows x heads_per_tile heads.
+template <uint32_t DCH, bool kBF16, bool kCausal>
+cudaError_t launch_forward_split(const AttentionParams &p, const WgmmaPlan &plan, const Sequences *seq,
+                                 const PagedKV *pk, const Band *band, cudaStream_t stream) {
+  using Cfg = FwdCfg<DCH>;
+  constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
+  TensorMaps m;
+  cudaError_t e;
+  const uint32_t hpt = plan.heads_per_tile, box_rows = Cfg::kTileM / hpt;
+  if (pk) {
+    const uint32_t box = min(1u << pk->page_shift, Cfg::BN);
+    if ((e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, box_rows, hpt)) != cudaSuccess ||
+        (e = make_tensor_map_page_pool(&m.K, p.buf[sK], p.C, pk->kv_heads, p.D, box)) != cudaSuccess ||
+        (e = make_tensor_map_page_pool(&m.V, p.buf[sV], p.C, pk->kv_heads, p.D, box)) != cudaSuccess)
+      return e;
+  } else if ((e = make_maps<Cfg>(p, false, &m)) != cudaSuccess ||
+             (e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, box_rows, hpt)) != cudaSuccess) {
+    return e;
+  }
+  SplitArgs sp{0, plan.splits, p.batch, nullptr, nullptr};
+  const uint64_t rows_total = static_cast<uint64_t>(p.batch) * p.R;
+  const size_t o_elems = plan.splits * rows_total * p.D;
+  if (plan.splits > 1) {
+    void *ws = nullptr;
+    if ((e = workspace_for(current_device(), stream, (o_elems + plan.splits * rows_total) * sizeof(float), &ws)) !=
+        cudaSuccess)
+      return e;
+    sp.O_part = static_cast<float *>(ws);
+    sp.L_part = sp.O_part + o_elems;
+  }
+  float *O = static_cast<float *>(p.buf[sO]);
+  const int l_prec = p.prec[sL];
+  auto run = [&](auto kernel, const auto &...args) {
+    if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess) return e;
+    kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, O, p.buf[sL], args...);
+    return cudaGetLastError();
+  };
+  if (pk && band)
+    e = run(split_forward_paged_band_wgmma<DCH, kBF16>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, *band, sp, hpt);
+  else if (pk)
+    e = run(split_forward_paged_wgmma<DCH, kBF16, kCausal>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, sp, hpt);
+  else if (band)
+    e = run(split_forward_packed_band_wgmma<DCH, kBF16>, p.R, p.C, p.D, p.scale_log2, l_prec, p.group, *seq, *band, sp, hpt);
+  else
+    e = run(split_forward_packed_wgmma<DCH, kBF16, kCausal>, p.R, p.C, p.D, p.scale_log2, l_prec, p.group, *seq, sp, hpt);
+  if (e != cudaSuccess || plan.splits == 1) return e;
+  const uint32_t max_row = pk ? pk->max_row : seq->max_row;
+  const uint64_t threads = static_cast<uint64_t>(max_row) * (p.D / 4);
+  merge_sequence_splits<<<dim3(static_cast<uint32_t>((threads + 127) / 128), p.batch, plan.grid.z), 128, 0, stream>>>(
+      sp, O, p.buf[sL], l_prec, p.R, p.D, pk ? pk->row_offsets : seq->row_offsets);
+  return cudaGetLastError();
+}
+
 static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
   BwdArgs a;
   a.O = static_cast<const float *>(p.buf[sO]);
@@ -1361,6 +1564,7 @@ static cudaError_t dispatch(const AttentionParams &p, bool convert_dO, F f) {
 WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
                      uint32_t max_splits, bool convert_dO, uint32_t sm_count, const Band *band) {
   WgmmaPlan p{};
+  p.heads_per_tile = 1;
   auto geometry = [&](auto cfg) {
     using Cfg = decltype(cfg);
     p.threads = Cfg::kThreads;
@@ -1419,6 +1623,21 @@ WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t 
   return p;
 }
 
+WgmmaPlan wgmma_plan_split(uint32_t D, uint32_t max_row, uint32_t key_bound, uint32_t count, uint32_t batch,
+                           uint32_t group, uint32_t min_blocks, uint32_t max_splits, uint32_t num_splits,
+                           uint32_t sm_count, const Band *band) {
+  // unsplit, blocks_per_split is the key-block bound of one tile (a window's band width when narrower)
+  WgmmaPlan p = wgmma_plan(MFA_FORWARD, D, max_row, key_bound, batch, 1, 0, 1, false, sm_count, band);
+  // a group's query heads share a tile when an unpacked tile would be partly empty
+  p.heads_per_tile = group >= 2 && group <= p.par && max_row < p.par ? group : 1;
+  const uint32_t rows = p.par / p.heads_per_tile, tiles = (max_row + rows - 1) / rows;
+  const uint64_t items = static_cast<uint64_t>(tiles) * (batch / p.heads_per_tile) * count;
+  p.splits = num_splits ? num_splits : hop::choose_key_splits(items, p.blocks_per_split, sm_count, min_blocks, max_splits);
+  p.grid = dim3(tiles * p.splits, batch / p.heads_per_tile, count);
+  p.launches = 1 + (p.splits > 1 ? 1 : 0);
+  return p;
+}
+
 static bool row_major_16bit(const AttentionParams &p) {
   for (int s = 0; s < kSlots; ++s)
     if (p.transposed[s]) return false;
@@ -1458,6 +1677,23 @@ cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &
                                               device_sm_count(current_device()));
   return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
     return hop::launch_forward_paged<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, pk,
+                                                                                                            band, stream);
+  });
+}
+
+cudaError_t launch_wgmma_forward_split(const AttentionParams &p, const Sequences *seq, const PagedKV *pk,
+                                       const Band *band, uint32_t num_splits, uint32_t key_bound, cudaStream_t stream) {
+  const WgmmaPlan plan = wgmma_plan_split(p.D, pk ? pk->max_row : seq->max_row, key_bound, pk ? pk->count : seq->count,
+                                          p.batch, p.group, p.split_min_blocks, p.split_max, num_splits,
+                                          device_sm_count(current_device()), band);
+  if (plan.splits == 1 && plan.heads_per_tile == 1)
+    return pk ? launch_wgmma_forward_paged(p, *pk, band, stream) : launch_wgmma_forward(p, seq, band, stream);
+  if (!row_major_16bit(p) || p.prec[sO] != FP32) {
+    set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
+    return cudaErrorInvalidValue;
+  }
+  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
+    return hop::launch_forward_split<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, seq, pk,
                                                                                                             band, stream);
   });
 }

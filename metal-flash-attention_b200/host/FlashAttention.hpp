@@ -125,6 +125,10 @@ using SequenceTable = mfa_sequence_table_t;
 using PagedKV = mfa_paged_kv_t;
 // {left, right}: a sliding window of keys around the bottom-right aligned diagonal, -1 = unbounded on that side
 using AttentionWindow = mfa_attention_window_t;
+// {num_splits, max_column}: a split-KV forward (0 = the library's plan; max_column a planning hint, 0 = the table's bound)
+using SplitKV = mfa_split_kv_t;
+// {splits, heads_per_tile, grid_size, launch_count}: what a split-KV encode launches
+using SplitPlan = mfa_split_plan_t;
 
 class AttentionKernel {  // AttentionKernel.swift:11-50
  public:
@@ -194,6 +198,23 @@ class AttentionKernel {  // AttentionKernel.swift:11-50
   void encode(const mfa_function_constants_t &constants, const PagedKV &paged,
               const std::array<void *, MFA_BUFFER_COUNT> &buffers, void *cudaStream = nullptr) const {
     check(mfa_attention_kernel_encode_paged(handle_, &constants, &paged, buffers.data(), cudaStream));
+  }
+  // the split-KV forward over packed sequences or a paged cache (library extension, mfa_split_kv_t)
+  SplitPlan splitPlan(const mfa_function_constants_t &constants, const SequenceTable &sequences,
+                      const SplitKV &split) const {
+    SplitPlan v; check(mfa_attention_kernel_split_plan(handle_, &constants, &sequences, nullptr, &split, &v)); return v;
+  }
+  SplitPlan splitPlan(const mfa_function_constants_t &constants, const PagedKV &paged, const SplitKV &split) const {
+    SplitPlan v; check(mfa_attention_kernel_split_plan(handle_, &constants, nullptr, &paged, &split, &v)); return v;
+  }
+  void encode(const mfa_function_constants_t &constants, const SequenceTable &sequences, const SplitKV &split,
+              const std::array<void *, MFA_BUFFER_COUNT> &buffers, void *cudaStream = nullptr) const {
+    check(mfa_attention_kernel_encode_sequences_split(handle_, &constants, &sequences, &split, buffers.data(),
+                                                      cudaStream));
+  }
+  void encode(const mfa_function_constants_t &constants, const PagedKV &paged, const SplitKV &split,
+              const std::array<void *, MFA_BUFFER_COUNT> &buffers, void *cudaStream = nullptr) const {
+    check(mfa_attention_kernel_encode_paged_split(handle_, &constants, &paged, &split, buffers.data(), cudaStream));
   }
  private:
   mfa_attention_kernel_t *handle_ = nullptr;

@@ -461,7 +461,64 @@ public final class AttentionKernel {
     var paged = paged
     check(mfa_attention_kernel_encode_paged(handle, &constants, &paged, &table, stream))
   }
+
+  // ---- library extension: the split-KV forward over packed sequences or a paged cache (mfa_split_kv_t)
+  public func splitPlan(constants: mfa_function_constants_t, sequences: SequenceTable, split: SplitKV) -> SplitPlan {
+    var constants = constants
+    var sequences = sequences
+    var split = split
+    var out = SplitPlan()
+    check(mfa_attention_kernel_split_plan(handle, &constants, &sequences, nil, &split, &out))
+    return out
+  }
+  public func splitPlan(constants: mfa_function_constants_t, paged: PagedKV, split: SplitKV) -> SplitPlan {
+    var constants = constants
+    var paged = paged
+    var split = split
+    var out = SplitPlan()
+    check(mfa_attention_kernel_split_plan(handle, &constants, nil, &paged, &split, &out))
+    return out
+  }
+  /// The forward `encode` over `sequences` whose key range may be split across CTAs (`split`).
+  public func encode(constants: mfa_function_constants_t, sequences: SequenceTable, split: SplitKV,
+                     buffers: [AttentionOperand: UnsafeMutableRawPointer],
+                     stream: UnsafeMutableRawPointer? = nil) {
+    var table = [UnsafeMutableRawPointer?](repeating: nil, count: Int(MFA_BUFFER_COUNT))
+    for (operand, pointer) in buffers {
+      guard let binding = operand.bufferBinding else { fatalError("Operand \(operand) has no buffer binding.") }
+      table[Int(binding)] = pointer
+    }
+    var constants = constants
+    var sequences = sequences
+    var split = split
+    check(mfa_attention_kernel_encode_sequences_split(handle, &constants, &sequences, &split, &table, stream))
+  }
+  /// The forward `encode` over a paged K/V cache whose key range may be split across CTAs (`split`).
+  public func encode(constants: mfa_function_constants_t, paged: PagedKV, split: SplitKV,
+                     buffers: [AttentionOperand: UnsafeMutableRawPointer],
+                     stream: UnsafeMutableRawPointer? = nil) {
+    var table = [UnsafeMutableRawPointer?](repeating: nil, count: Int(MFA_BUFFER_COUNT))
+    for (operand, pointer) in buffers {
+      guard let binding = operand.bufferBinding else { fatalError("Operand \(operand) has no buffer binding.") }
+      table[Int(binding)] = pointer
+    }
+    var constants = constants
+    var paged = paged
+    var split = split
+    check(mfa_attention_kernel_encode_paged_split(handle, &constants, &paged, &split, &table, stream))
+  }
 }
+
+/// library extension: a split-KV forward.  `numSplits` 0 lets the library plan, 1...16 is taken as given;
+/// `maxColumn` is a planning hint bounding every sequence's keys (0 = the table's bound).
+public typealias SplitKV = mfa_split_kv_t
+extension mfa_split_kv_t {
+  public init(numSplits: UInt32 = 0, maxColumn: UInt32 = 0) {
+    self.init(num_splits: numSplits, max_column: maxColumn)
+  }
+}
+/// library extension: what a split-KV encode launches (splits, heads_per_tile, grid_size, launch_count).
+public typealias SplitPlan = mfa_split_plan_t
 
 /// library extension: packed variable-length sequences.  `rowOffsets` / `columnOffsets` are DEVICE pointers to
 /// `count + 1` Int32 entries each; `maxRow` / `maxColumn` are at least every sequence's query / key length.
