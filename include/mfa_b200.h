@@ -471,6 +471,41 @@ MFA_API int mfa_attention_kernel_split_plan(const mfa_attention_kernel_t *kernel
                                             const mfa_split_kv_t *split, mfa_split_plan_t *out);
 
 /* ------------------------------------------------------------------------------------------ */
+/* FP8 K/V cache (library extension; paged forward only)                                       */
+/* ------------------------------------------------------------------------------------------ */
+/** A paged forward (above) whose K and V pools hold one OCP FP8 E4M3 byte per element (torch.float8_e4m3fn: no
+ *  infinities, NaN = 0x7F / 0xFF), [num_pages][P][H / G][D] bytes, the cache vLLM, SGLang, FlashInfer and
+ *  TensorRT-LLM keep with kv_cache_dtype="fp8".  Key row i of K/V head kv stands for k_scale[kv] * e4m3(byte), and
+ *  likewise for V with v_scale.  Q is FP16 or BF16 as the descriptor says; O is FP32 and L in the descriptor's precision.
+ *
+ *  The kernels dequantize on load: each FP8 value is converted exactly to Q's 16-bit type in shared memory, and the
+ *  products, softmax and outputs are those of the 16-bit paged kernels.  k_scale[kv] multiplies the softmax scale and
+ *  v_scale[kv] the output's normalisation, so with NULL scales, or scales that are powers of two, O and L equal bit for
+ *  bit those of mfa_attention_kernel_encode_paged (split == NULL) or _paged_split (the same split) over the 16-bit pools
+ *  holding the dequantized values.  Every guarantee of those calls holds unchanged: per-sequence causal alignment,
+ *  grouped K/V, windows (pages outside the band are never read), split plans and packed query heads, empty rows
+ *  (O = 0, L = +inf), the clamping of table contents, rows outside every sequence never written, pool contents past
+ *  Cs never reaching an output (NaN bytes included), and graph replay as the cache grows.
+ *
+ *  The plan does not depend on the K/V element type: mfa_attention_kernel_grid_size_paged and _launch_count_paged
+ *  describe an FP8 call with split == NULL, and mfa_attention_kernel_split_plan one with a split.
+ *
+ *  Every check of _paged (and, with a split, of _paged_split) is made identically.  Beyond them the host returns
+ *  MFA_ERROR_INVALID_ARGUMENT, naming the field, before any device work for: a NULL fp8; a kernel on
+ *  MFA_BACKEND_SIMT_FP32 ("FP8 K/V needs the tensor-core family"); a head dimension that is not a multiple of 16 (TMA
+ *  reads 1-byte rows at 16-byte strides). */
+typedef struct mfa_fp8_kv {
+  const float *k_scale; /* device, batch_count / kv_group entries (one per K/V head), read at launch; NULL: every 1 */
+  const float *v_scale; /* the same for V */
+} mfa_fp8_kv_t;
+/** split == NULL: as mfa_attention_kernel_encode_paged; else as mfa_attention_kernel_encode_paged_split. */
+MFA_API int mfa_attention_kernel_encode_paged_fp8(const mfa_attention_kernel_t *kernel,
+                                                  const mfa_function_constants_t *constants,
+                                                  const mfa_paged_kv_t *paged, const mfa_split_kv_t *split,
+                                                  const mfa_fp8_kv_t *fp8, void *const buffers[MFA_BUFFER_COUNT],
+                                                  void *cuda_stream);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Kernel cache keyed by descriptor                                                            */
 /* ------------------------------------------------------------------------------------------ */
 /** The analogue of the reference's pipeline cache (GEMMKernel.register(descriptor:) / pipelineCache[descriptor],

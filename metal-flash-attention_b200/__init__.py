@@ -135,6 +135,16 @@ class SplitPlan(ctypes.Structure):
                 ("launch_count", ctypes.c_uint32)]
 
 
+class FP8KV(ctypes.Structure):
+    """mfa_fp8_kv_t: the K and V pools of a paged call hold FP8 E4M3 bytes (torch.float8_e4m3fn viewed as uint8), key
+    row i of K/V head kv standing for k_scale[kv] * e4m3(byte) (v_scale for V).  k_scale / v_scale: float32 DEVICE
+    pointers with one entry per K/V head, read at launch; 0 means every scale is 1."""
+    _fields_ = [("k_scale", ctypes.c_void_p), ("v_scale", ctypes.c_void_p)]
+
+    def __init__(self, k_scale=0, v_scale=0):
+        super().__init__(k_scale or None, v_scale or None)
+
+
 class _CWindow(ctypes.Structure):
     _fields_ = [("left", ctypes.c_int32), ("right", ctypes.c_int32)]
 
@@ -201,6 +211,9 @@ def _load():
     lib.mfa_attention_kernel_encode_paged_split.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
                                                             c.POINTER(PagedKV), c.POINTER(SplitKV),
                                                             c.POINTER(c.c_void_p * MFA_BUFFER_COUNT), c.c_void_p]
+    lib.mfa_attention_kernel_encode_paged_fp8.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
+                                                          c.POINTER(PagedKV), c.POINTER(SplitKV), c.POINTER(FP8KV),
+                                                          c.POINTER(c.c_void_p * MFA_BUFFER_COUNT), c.c_void_p]
     lib.mfa_attention_kernel_split_plan.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
                                                     c.POINTER(SequenceTable), c.POINTER(PagedKV), c.POINTER(SplitKV),
                                                     c.POINTER(SplitPlan)]
@@ -673,21 +686,31 @@ class AttentionKernel:
 
     def encode(self, constants: FunctionConstantValues, buffers: Dict[AttentionOperand, int],
                stream: int = 0, sequences: Optional[SequenceTable] = None, paged: Optional[PagedKV] = None,
-               split: Optional[SplitKV] = None) -> None:
+               split: Optional[SplitKV] = None, fp8: Optional[FP8KV] = None) -> None:
         """buffers: {AttentionOperand: device pointer}; stream: cudaStream_t as int (0 = default).  sequences: packed
         variable-length sequences over the rows of every problem (mfa_attention_kernel_encode_sequences).  paged: the
         forward over a paged K/V cache, K and V pointing at the page pools (mfa_attention_kernel_encode_paged).
-        split: the split-KV forward over sequences= or paged= (mfa_attention_kernel_encode_sequences_split / _paged_split)."""
+        split: the split-KV forward over sequences= or paged= (mfa_attention_kernel_encode_sequences_split / _paged_split).
+        fp8: the pools of paged= hold FP8 E4M3 bytes with per-K/V-head scales, with or without split=
+        (mfa_attention_kernel_encode_paged_fp8)."""
         _one_table(sequences, paged)
         if split is not None and sequences is None and paged is None:
             raise MFAError(-2, "split= needs sequences= or paged=: the fixed-length forward plans its own split.")
+        if fp8 is not None and paged is None:
+            raise MFAError(-2, "fp8= needs paged=: FP8 K/V is read from a paged cache only.")
         arr = (ctypes.c_void_p * MFA_BUFFER_COUNT)()
         for op, ptr in buffers.items():
             binding = AttentionOperand(op).bufferBinding
             if binding is None:
                 raise MFAError(-2, f"Operand {AttentionOperand(op).name} has no buffer binding.")
             arr[binding] = ptr
-        if split is not None and paged is not None:
+        if fp8 is not None:
+            _check(_lib.mfa_attention_kernel_encode_paged_fp8(self._handle, ctypes.byref(constants._c),
+                                                              ctypes.byref(paged),
+                                                              ctypes.byref(split) if split is not None else None,
+                                                              ctypes.byref(fp8), ctypes.byref(arr),
+                                                              ctypes.c_void_p(stream)))
+        elif split is not None and paged is not None:
             _check(_lib.mfa_attention_kernel_encode_paged_split(self._handle, ctypes.byref(constants._c),
                                                                 ctypes.byref(paged), ctypes.byref(split),
                                                                 ctypes.byref(arr), ctypes.c_void_p(stream)))
@@ -710,6 +733,6 @@ class AttentionKernel:
 __all__ = [
     "AttentionDescriptor", "AttentionKernelDescriptor", "AttentionKernel", "AttentionKernelType",
     "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError", "SequenceTable", "PagedKV",
-    "SplitKV", "SplitPlan",
+    "SplitKV", "SplitPlan", "FP8KV",
     "library_path", "version", "setParameterTable", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
 ]

@@ -260,6 +260,21 @@ static int split_of(const mfa_attention_kernel *k, const mfa_split_kv_t *s) {
                                                 std::to_string(kMaxKeySplits) + ".");
   return MFA_SUCCESS;
 }
+// An FP8 K/V request (mfa_fp8_kv_t), after the checks the host can make; the table's and the split's checks come first
+// (paged_of rejects every kernel but the forward)
+static int fp8_of(const mfa_attention_kernel *k, const mfa_fp8_kv_t *f, Fp8KV *out) {
+  if (!f) return fail(MFA_ERROR_INVALID_ARGUMENT, "FP8 K/V: NULL fp8.");
+  if (k->backend != MFA_BACKEND_TCGEN05)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "FP8 K/V needs the tensor-core family (MFA_BACKEND_TCGEN05); this kernel "
+                                            "is on MFA_BACKEND_SIMT_FP32.");
+  if (k->descriptor.head_dimension % 16 != 0)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "FP8 K/V needs a head dimension that is a multiple of 16 (head " +
+                                                std::to_string(k->descriptor.head_dimension) +
+                                                "): TMA reads the pools' 1-byte rows at 16-byte strides.");
+  *out = Fp8KV{f->k_scale, f->v_scale};
+  return MFA_SUCCESS;
+}
+
 // The key bound a split plan cuts: the hint, or the table's bound (capped so that block counts cannot overflow)
 static uint32_t key_bound_of(const mfa_split_kv_t &s, const Sequences *seq, const PagedKV *pk) {
   const uint32_t bound = s.max_column ? s.max_column : (seq ? seq->max_column : pk->max_keys);
@@ -271,10 +286,12 @@ static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_const
                   void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, const mfa_split_kv_t *split = nullptr);
 static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
                       const PagedKV *pk, const mfa_split_kv_t &split, mfa_split_plan_t *out);
-// encode() of a paged cache; split_call: the split-KV entry point, whose request `split` is checked after the table
+// encode() of a paged cache; split_call: the split-KV entry point, whose request `split` is checked after the table;
+// fp8_call: the FP8 K/V entry point (split optional), whose request `fp8` is checked after both
 static int encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
                         const mfa_paged_kv_t *table, bool split_call, const mfa_split_kv_t *split,
-                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
+                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, bool fp8_call = false,
+                        const mfa_fp8_kv_t *fp8 = nullptr);
 
 }  // namespace mfa
 
@@ -552,6 +569,13 @@ int mfa_attention_kernel_encode_paged_split(const mfa_attention_kernel_t *kernel
   return encode_paged(kernel, constants, table, true, split, buffers, cuda_stream);
 }
 
+int mfa_attention_kernel_encode_paged_fp8(const mfa_attention_kernel_t *kernel,
+                                          const mfa_function_constants_t *constants, const mfa_paged_kv_t *table,
+                                          const mfa_split_kv_t *split, const mfa_fp8_kv_t *fp8,
+                                          void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
+  return encode_paged(kernel, constants, table, split != nullptr, split, buffers, cuda_stream, true, fp8);
+}
+
 int mfa_attention_kernel_encode_sequences_split(const mfa_attention_kernel_t *kernel,
                                                 const mfa_function_constants_t *constants,
                                                 const mfa_sequence_table_t *table, const mfa_split_kv_t *split,
@@ -608,13 +632,16 @@ static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_c
 
 static int encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
                         const mfa_paged_kv_t *table, bool split_call, const mfa_split_kv_t *split,
-                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
+                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, bool fp8_call,
+                        const mfa_fp8_kv_t *fp8) {
   if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
   PagedKV pk;
   int status = paged_of(kernel, constants, table, &pk);
   if (status != MFA_SUCCESS) return status;
   if (split_call && (status = split_of(kernel, split)) != MFA_SUCCESS) return status;
+  Fp8KV scales{};
+  if (fp8_call && (status = fp8_of(kernel, fp8, &scales)) != MFA_SUCCESS) return status;
   if ((status = check_device()) != MFA_SUCCESS) return status;
   AttentionParams p;
   if ((status = build_params(kernel, constants, buffers, p)) != MFA_SUCCESS) return status;
@@ -622,14 +649,18 @@ static int encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function
   Band storage;
   const Band *band = band_of(kernel, p.R, pk.max_keys, &storage);
   cudaError_t e;
-  if (kernel->backend != MFA_BACKEND_TCGEN05)
+  if (fp8_call)
+    e = launch_wgmma_forward_paged_fp8(p, pk, band, scales, split != nullptr, split ? split->num_splits : 1,
+                                       split ? key_bound_of(*split, nullptr, &pk) : pk.max_keys, stream);
+  else if (kernel->backend != MFA_BACKEND_TCGEN05)
     e = launch_simt_forward_paged(p, pk, band, stream);
   else if (split)
     e = launch_wgmma_forward_split(p, nullptr, &pk, band, split->num_splits, key_bound_of(*split, nullptr, &pk), stream);
   else
     e = launch_wgmma_forward_paged(p, pk, band, stream);
   if (e != cudaSuccess)
-    return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " (paged K/V) failed: " +
+    return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name +
+                                    (fp8_call ? " (paged FP8 K/V) failed: " : " (paged K/V) failed: ") +
                                     cudaGetErrorString(e) + " " + last_launch_detail());
   return MFA_SUCCESS;
 }

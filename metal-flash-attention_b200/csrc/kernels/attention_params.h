@@ -101,6 +101,13 @@ struct Band {
   int32_t left, right;
 };
 
+// FP8 K/V (mfa_fp8_kv_t): the K and V pools of a paged call hold OCP E4M3 bytes, and key row i of K/V head kv stands
+// for k_scale[kv] * e4m3(byte) (v_scale for V).  Device arrays of batch / group entries, read by the kernels at launch;
+// NULL: every scale is 1.
+struct Fp8KV {
+  const float *k_scale, *v_scale;
+};
+
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
 // seq: packed sequences, or nullptr for problems of the full R x C shape; band: a sliding window, or nullptr
 cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream);
@@ -129,6 +136,12 @@ cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &
 // wgmma_plan_split; one split runs launch_wgmma_forward / launch_wgmma_forward_paged unchanged
 cudaError_t launch_wgmma_forward_split(const AttentionParams &p, const Sequences *seq, const PagedKV *pk,
                                        const Band *band, uint32_t num_splits, uint32_t key_bound, cudaStream_t stream);
+// paged forward over FP8 E4M3 pools (K and V buffers hold bytes; Q's 16-bit type is what they are converted to): split,
+// the plan of wgmma_plan_split for num_splits / key_bound; unsplit, one split and one head per tile, the grid of
+// launch_wgmma_forward_paged.  Always the split paged kernels' FP8 twins.
+cudaError_t launch_wgmma_forward_paged_fp8(const AttentionParams &p, const PagedKV &pk, const Band *band,
+                                           const Fp8KV &fp8, bool split, uint32_t num_splits, uint32_t key_bound,
+                                           cudaStream_t stream);
 
 // How the launcher of kernel `type` (mfa_kernel_type_t) runs one problem of padded head dimension D; every field is
 // derived from the kernels' compile-time configurations.  R, C and batch do not affect the geometry fields.

@@ -102,6 +102,33 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
+// four OCP E4M3 bytes (byte 0 lowest) -> two f16x2 registers (byte 0 in the low half of .x); exact, NaN stays NaN
+__device__ __forceinline__ uint2 e4m3x4_to_f16x4(uint32_t bytes) {
+  uint2 r;
+  asm("{\n"
+      ".reg .b16 lo, hi;\n"
+      "mov.b32 {lo, hi}, %2;\n"
+      "cvt.rn.f16x2.e4m3x2 %0, lo;\n"
+      "cvt.rn.f16x2.e4m3x2 %1, hi;\n"
+      "}\n"
+      : "=r"(r.x), "=r"(r.y)
+      : "r"(bytes));
+  return r;
+}
+// f16x2 -> bf16x2 through FP32: exact for every value an E4M3 byte holds (at most 4 significant bits, exponent in
+// [-9, 8])
+__device__ __forceinline__ uint32_t f16x2_to_bf16x2(uint32_t h) {
+  float lo, hi;
+  asm("{\n"
+      ".reg .b16 a, b;\n"
+      "mov.b32 {a, b}, %2;\n"
+      "cvt.f32.f16 %0, a;\n"
+      "cvt.f32.f16 %1, b;\n"
+      "}\n"
+      : "=f"(lo), "=f"(hi)
+      : "r"(h));
+  return pack_bf16x2(lo, hi);
+}
 
 }  // namespace ptx
 }  // namespace mfa

@@ -73,7 +73,8 @@ uint32_t map_slot(const MapKey &k) {
 // in shared memory as the same [boxRows][boxCols] tile.
 static cudaError_t encode(CUtensorMap *map, CUtensorMapDataType dtype, uint32_t elemBytes, const void *base,
                           uint32_t seq, uint32_t D, uint32_t batch, uint32_t boxCols, uint32_t boxRows,
-                          MapLayout layout, uint32_t boxDepth = 1) {
+                          MapLayout layout, uint32_t boxDepth = 1,
+                          CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   const MapKey key{base, seq, D, batch, boxCols, boxRows, boxDepth, static_cast<uint32_t>(dtype), layout};
   MapEntry &entry = g_map_cache[map_slot(key)];
   if (entry.valid && entry.key == key) {
@@ -96,7 +97,7 @@ static cudaError_t encode(CUtensorMap *map, CUtensorMapDataType dtype, uint32_t 
   cuuint32_t box[3] = {boxCols, pool ? 1 : boxRows, pool ? boxRows : boxDepth};
   cuuint32_t elemStrides[3] = {1, 1, 1};
   CUresult r = fn(map, dtype, 3, const_cast<void *>(base), dims, strides, box, elemStrides, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_launch_detail("cuTensorMapEncodeTiled failed with CUresult %d (seq=%u D=%u batch=%u box=%ux%u)", (int)r, seq, D,
                       batch, boxCols, boxRows);
@@ -117,6 +118,13 @@ cudaError_t make_tensor_map_16bit(CUtensorMap *map, const void *base, uint32_t s
 cudaError_t make_tensor_map_page_pool(CUtensorMap *map, const void *base, uint32_t rows, uint32_t heads, uint32_t D,
                                       uint32_t box_rows) {
   return encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, rows, D, heads, 64, box_rows, kPagePool);
+}
+
+cudaError_t make_tensor_map_page_pool_8bit(CUtensorMap *map, const void *base, uint32_t rows, uint32_t heads,
+                                           uint32_t D, uint32_t box_rows) {
+  // (the key's data type tells these maps from the 16-bit ones, so the swizzle needs no key field of its own)
+  return encode(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, base, rows, D, heads, 64, box_rows, kPagePool, 1,
+                CU_TENSOR_MAP_SWIZZLE_NONE);
 }
 
 }  // namespace mfa

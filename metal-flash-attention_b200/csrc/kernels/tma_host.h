@@ -19,6 +19,11 @@ cudaError_t make_tensor_map_16bit(CUtensorMap *map, const void *base, uint32_t s
 cudaError_t make_tensor_map_page_pool(CUtensorMap *map, const void *base, uint32_t rows, uint32_t heads, uint32_t D,
                                       uint32_t box_rows);
 
+// The same pool of 1-byte elements (FP8 K/V): boxes of 64 (D) x 1 (head) x box_rows bytes, unswizzled, landing as a
+// dense [box_rows][64]-byte tile.  D must be a multiple of 16 (16-byte row pitch).
+cudaError_t make_tensor_map_page_pool_8bit(CUtensorMap *map, const void *base, uint32_t rows, uint32_t heads,
+                                           uint32_t D, uint32_t box_rows);
+
 void set_launch_detail(const char *fmt, ...);
 
 }  // namespace mfa

@@ -428,6 +428,16 @@ struct FwdCfg {
   static constexpr uint32_t kPar = kTileM, kTrav = BN, kQueryBoxRows = kTileM, kKeyBoxRows = BN;
   static constexpr uint32_t kQBytes = DCH * kTileM * 128, kKVBytes = DCH * BN * 128;
   using Smem = SmemLayout<kQBytes, kKVBytes>;  // resident Q; stage: K, V
+  // FP8 K/V: resident Q; a ring stage holds the FP8 K and V blocks as TMA lands them, [chunk][BN][64] bytes each,
+  // unswizzled; after the two stages, one converted stage of 16-bit K and V tiles laid out as Smem's; the same bytes
+  static constexpr uint32_t kFp8Bytes = DCH * BN * 64;
+  struct Fp8Smem {
+    static constexpr uint32_t kResidentBytes = kQBytes, kStageBytes = 2 * kFp8Bytes;
+    static constexpr uint32_t kConvertedOffset = kQBytes + 2 * kStageBytes;
+    static constexpr uint32_t kBarOffset = kConvertedOffset + 2 * kKVBytes;
+    static constexpr uint32_t kSmemBytes = 1024 + kBarOffset + kBarBytes;
+  };
+  static_assert(Fp8Smem::kSmemBytes == Smem::kSmemBytes, "FP8 K/V keeps the 16-bit kernels' shared memory");
 };
 
 // Where the forward's keys come from: every problem's [C][D] rows (kFixed), a packed sequence's rows of them
@@ -438,8 +448,8 @@ enum class KVLayout { kFixed, kPacked, kPaged };
 // `box` rows each (min(P, BN)).  P >= BN: one box per chunk and tensor, at the block's page.  P < BN: the page ids of
 // every box are read first, so that their loads overlap, then each box is issued for K and V.  Boxes that start at or
 // past the sequence's C never read the page table: they load pool row 0, and the caller zeroes every row past C before
-// the MMAs.
-template <uint32_t DCH, uint32_t BN>
+// the MMAs.  ROW: bytes of one tile row of a chunk (128: 64 16-bit elements; 64: 64 FP8 bytes).
+template <uint32_t DCH, uint32_t BN, uint32_t ROW = 128>
 __device__ __forceinline__ void load_paged_kv(uint8_t *dst, uint32_t kv_bytes, const CUtensorMap *mapK,
                                               const CUtensorMap *mapV, uint64_t *bar, const PagedKV &pk,
                                               const int32_t *table, uint32_t block, uint32_t box, uint32_t C,
@@ -448,8 +458,8 @@ __device__ __forceinline__ void load_paged_kv(uint8_t *dst, uint32_t kv_bytes, c
     const uint32_t row = paged_row(pk, table, block * BN);
 #pragma unroll
     for (uint32_t c = 0; c < DCH; ++c) {
-      tma_load_3d(dst + c * BN * 128, mapK, bar, c * 64, kv_head, row);
-      tma_load_3d(dst + kv_bytes + c * BN * 128, mapV, bar, c * 64, kv_head, row);
+      tma_load_3d(dst + c * BN * ROW, mapK, bar, c * 64, kv_head, row);
+      tma_load_3d(dst + kv_bytes + c * BN * ROW, mapV, bar, c * 64, kv_head, row);
     }
     return;
   }
@@ -465,8 +475,8 @@ __device__ __forceinline__ void load_paged_kv(uint8_t *dst, uint32_t kv_bytes, c
     if (i * box >= BN) break;
 #pragma unroll
     for (uint32_t c = 0; c < DCH; ++c) {
-      tma_load_3d(dst + c * BN * 128 + i * box * 128, mapK, bar, c * 64, kv_head, rows[i]);
-      tma_load_3d(dst + kv_bytes + c * BN * 128 + i * box * 128, mapV, bar, c * 64, kv_head, rows[i]);
+      tma_load_3d(dst + c * BN * ROW + i * box * ROW, mapK, bar, c * 64, kv_head, rows[i]);
+      tma_load_3d(dst + kv_bytes + c * BN * ROW + i * box * ROW, mapV, bar, c * 64, kv_head, rows[i]);
     }
   }
 }
@@ -482,7 +492,7 @@ __device__ __forceinline__ uint2 band_boxes(uint32_t block, uint32_t BN, uint32_
 // load_paged_kv of a windowed tile: only the boxes band_boxes names are issued, so the page-table entries and pages of
 // the others are never read; the bytes they would have brought are completed on `bar` by hand, and the caller zeroes
 // their rows
-template <uint32_t DCH, uint32_t BN>
+template <uint32_t DCH, uint32_t BN, uint32_t ROW = 128>
 __device__ __forceinline__ void load_paged_kv_band(uint8_t *dst, uint32_t kv_bytes, const CUtensorMap *mapK,
                                                    const CUtensorMap *mapV, uint64_t *bar, const PagedKV &pk,
                                                    const int32_t *table, uint32_t block, uint32_t box, int lo, int hi,
@@ -494,15 +504,46 @@ __device__ __forceinline__ void load_paged_kv_band(uint8_t *dst, uint32_t kv_byt
   for (uint32_t i = 0; i < kMaxBoxes; ++i)
     rows[i] = i >= kept.x && i < kept.y ? paged_row(pk, table, block * BN + i * box) : 0u;
   const uint32_t skipped = BN / box - (kept.y - kept.x);
-  if (skipped) mbar_complete_tx(bar, skipped * box * 128 * DCH * 2);
+  if (skipped) mbar_complete_tx(bar, skipped * box * ROW * DCH * 2);
 #pragma unroll
   for (uint32_t i = 0; i < kMaxBoxes; ++i) {
     if (i < kept.x || i >= kept.y) continue;
 #pragma unroll
     for (uint32_t c = 0; c < DCH; ++c) {
-      tma_load_3d(dst + c * BN * 128 + i * box * 128, mapK, bar, c * 64, kv_head, rows[i]);
-      tma_load_3d(dst + kv_bytes + c * BN * 128 + i * box * 128, mapV, bar, c * 64, kv_head, rows[i]);
+      tma_load_3d(dst + c * BN * ROW + i * box * ROW, mapK, bar, c * 64, kv_head, rows[i]);
+      tma_load_3d(dst + kv_bytes + c * BN * ROW + i * box * ROW, mapV, bar, c * 64, kv_head, rows[i]);
     }
+  }
+}
+
+// FP8 K/V: the landed block at src (FP8 K then V, [chunk][BN][64] bytes each) converted into the 16-bit K and V tiles
+// at dst ([chunk][BN][64] elements, 128-byte swizzled, as TMA writes them for the 16-bit kernels).  Rows outside
+// [first, end) -- past the sequence's keys, or in boxes that were not issued -- are written as zeros instead: a masked
+// product is 0 x x, which is NaN when x is not finite.  The caller fences and synchronises.
+template <uint32_t DCH, uint32_t BN, uint32_t kThreads, bool kBF16>
+__device__ __forceinline__ void convert_fp8_kv(const uint8_t *src, uint8_t *dst, uint32_t first, uint32_t end) {
+  // 16-byte units of the landed block: i = ((tensor * DCH + chunk) * BN + row) * 4 + quarter, at byte 16 i; its 16
+  // elements go to 16-byte units 2 quarter and 2 quarter + 1 of line i / 4 of dst, each XORed with row % 8
+  constexpr uint32_t kUnits = 2 * DCH * BN * 4;
+  static_assert(kUnits % kThreads == 0, "every thread converts the same number of units");
+#pragma unroll 4
+  for (uint32_t i = threadIdx.x; i < kUnits; i += kThreads) {
+    const uint32_t row = (i / 4) % BN, quarter = i % 4;
+    uint4 lo = make_uint4(0u, 0u, 0u, 0u), hi = lo;
+    if (row >= first && row < end) {
+      const uint4 v = *reinterpret_cast<const uint4 *>(src + 16 * i);
+      const uint2 a = e4m3x4_to_f16x4(v.x), b = e4m3x4_to_f16x4(v.y), c = e4m3x4_to_f16x4(v.z),
+                  d = e4m3x4_to_f16x4(v.w);
+      lo = make_uint4(a.x, a.y, b.x, b.y);
+      hi = make_uint4(c.x, c.y, d.x, d.y);
+      if constexpr (kBF16) {
+        lo = make_uint4(f16x2_to_bf16x2(lo.x), f16x2_to_bf16x2(lo.y), f16x2_to_bf16x2(lo.z), f16x2_to_bf16x2(lo.w));
+        hi = make_uint4(f16x2_to_bf16x2(hi.x), f16x2_to_bf16x2(hi.y), f16x2_to_bf16x2(hi.z), f16x2_to_bf16x2(hi.w));
+      }
+    }
+    uint8_t *line = dst + (i / 4) * 128;
+    *reinterpret_cast<uint4 *>(line + ((2 * quarter) ^ (row % 8)) * 16) = lo;
+    *reinterpret_cast<uint4 *>(line + ((2 * quarter + 1) ^ (row % 8)) * 16) = hi;
   }
 }
 
@@ -516,18 +557,24 @@ __device__ __forceinline__ void load_paged_kv_band(uint8_t *dst, uint32_t kv_byt
 // holds m = kTileM / hpt query rows of each of the hpt query heads blockIdx.y * hpt + [0, hpt) (hpt = 1, or the K/V
 // group): tile row t is head blockIdx.y * hpt + t / m, query row tile * m + t % m; rows hpt * m .. kTileM - 1 are never
 // stored.  Each row is masked with its own query row, so its arithmetic is that of the unpacked tile.
-template <uint32_t DCH, bool kBF16, bool kCausal, KVLayout kLayout, bool kBand = false, bool kSplit = false>
+// kFp8 (kSplit paged only): the pools hold E4M3 bytes (mapK / mapV are 8-bit page-pool maps).  The ring lands each FP8
+// block (Cfg::Fp8Smem); the threads convert it into the one 16-bit stage, zeroing the rows the 16-bit path zeroes, and
+// the MMAs read that stage.  fp8.k_scale[kv_head] multiplies scale_log2, fp8.v_scale[kv_head] the epilogue's 1 / l.
+template <uint32_t DCH, bool kBF16, bool kCausal, KVLayout kLayout, bool kBand = false, bool kSplit = false,
+          bool kFp8 = false>
 __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUtensorMap &mapK, const CUtensorMap &mapV,
                                              float *__restrict__ O, void *__restrict__ L, uint32_t R, uint32_t C,
                                              uint32_t D, float scale_log2, int l_prec, const SplitArgs &sp, int delta,
                                              uint32_t group, const Sequences &seq, const PagedKV &pk,
-                                             const Band &band = Band{}, uint32_t hpt = 1) {
+                                             const Band &band = Band{}, uint32_t hpt = 1, const Fp8KV &fp8 = Fp8KV{}) {
   constexpr bool kVarlen = kLayout != KVLayout::kFixed;
   static_assert(!kSplit || kVarlen, "the fixed-length forward splits through blockIdx.z");
+  static_assert(!kFp8 || (kSplit && kLayout == KVLayout::kPaged), "FP8 K/V is a split paged forward");
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
-  const Ring<typename Cfg::Smem> ring(smem_raw);  // resident Q; step j: K and V of key block kb0 + j
+  using Smem = std::conditional_t<kFp8, typename Cfg::Fp8Smem, typename Cfg::Smem>;
+  const Ring<Smem> ring(smem_raw);  // resident Q; step j: K and V of key block kb0 + j
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   const uint32_t tile = kSplit ? blockIdx.x / sp.splits : blockIdx.x;
   // (causal: unlike dQ, the forward gains nothing measurable from starting the tiles with the most key blocks first)
@@ -535,6 +582,11 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   const uint32_t head = blockIdx.y, row_base = tile * tile_rows;
   // grouped K/V: the query heads of a group read one K/V head (kSplit: the tile's heads start at head * hpt)
   const uint32_t kv_head = (kSplit ? head * hpt : head) / group;
+  float v_scale = 1.f;
+  if constexpr (kFp8) {
+    if (fp8.k_scale) scale_log2 *= __ldg(fp8.k_scale + kv_head);
+    if (fp8.v_scale) v_scale = __ldg(fp8.v_scale + kv_head);
+  }
   SequenceSpan span{0, R, 0, C};
   uint32_t kb0, per_split;
   if constexpr (kVarlen) {
@@ -571,7 +623,12 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
                                                      : nullptr;
   const uint32_t box = kLayout == KVLayout::kPaged ? min(1u << pk.page_shift, BN) : BN;
   auto load_kv = [&](uint32_t j, uint8_t *dst, uint64_t *bar) {
-    if constexpr (kLayout == KVLayout::kPaged && kBand) {
+    if constexpr (kFp8 && kBand) {
+      load_paged_kv_band<DCH, BN, 64>(dst, Cfg::kFp8Bytes, &mapK, &mapV, bar, pk, table, kb0 + j, box, band_lo,
+                                      min(band_hi, static_cast<int>(span.C) - 1), kv_head);
+    } else if constexpr (kFp8) {
+      load_paged_kv<DCH, BN, 64>(dst, Cfg::kFp8Bytes, &mapK, &mapV, bar, pk, table, kb0 + j, box, span.C, kv_head);
+    } else if constexpr (kLayout == KVLayout::kPaged && kBand) {
       load_paged_kv_band<DCH, BN>(dst, Cfg::kKVBytes, &mapK, &mapV, bar, pk, table, kb0 + j, box, band_lo,
                                   min(band_hi, static_cast<int>(span.C) - 1), kv_head);
     } else if constexpr (kLayout == KVLayout::kPaged) {
@@ -606,7 +663,20 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   ring.wait_resident();
   for (uint32_t j = 0; j < blocks; ++j) {
     ring.wait(j);
-    if constexpr (kLayout == KVLayout::kPaged && kBand) {
+    if constexpr (kFp8) {
+      // the rows [first, end) of the block that hold keys to use: below C, and (window) in the boxes that were issued
+      uint32_t first = 0, end = min(BN, span.C - (kb0 + j) * BN);
+      if constexpr (kBand) {
+        const uint2 kept = band_boxes(kb0 + j, BN, box, band_lo, min(band_hi, static_cast<int>(span.C) - 1));
+        first = kept.x * box;
+        end = min(kept.y * box, end);
+      }
+      convert_fp8_kv<DCH, BN, Cfg::kThreads, kBF16>(ring.stage(j), ring.base + Cfg::Fp8Smem::kConvertedOffset, first, end);
+      fence_proxy_async_smem();
+      __syncthreads();
+      // the landed block is spent: its stage takes step j + 2 while this block's MMAs run
+      if (tid == 0 && j + 2 < blocks) ring.load(j + 2, j & 1, load_kv);
+    } else if constexpr (kLayout == KVLayout::kPaged && kBand) {
       // the rows of the boxes that were not issued, and those past C
       const uint2 kept = band_boxes(kb0 + j, BN, box, band_lo, min(band_hi, static_cast<int>(span.C) - 1));
       const uint32_t first = kept.x * box, end = min(kept.y * box, span.C - (kb0 + j) * BN);
@@ -626,7 +696,7 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
       fence_proxy_async_smem();
       __syncthreads();
     }
-    const uint32_t sK = smem_u32(ring.stage(j)), sV = sK + Cfg::kKVBytes;
+    const uint32_t sK = smem_u32(kFp8 ? ring.base + Cfg::Fp8Smem::kConvertedOffset : ring.stage(j)), sV = sK + Cfg::kKVBytes;
     float sc[BN / 2];
     zero(sc);
     wgmma_fence();
@@ -707,7 +777,10 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(o);
-    ring.release_and_refill(j, blocks, load_kv);
+    if constexpr (kFp8)
+      __syncthreads();  // every warpgroup is done with the converted stage: the next block may overwrite it
+    else
+      ring.release_and_refill(j, blocks, load_kv);
   }
 
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
@@ -721,7 +794,9 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
     for (uint32_t h = 0; h < 2; ++h) {
       const uint32_t trow = trow0 + 8 * h, r = row_base + trow % tile_rows, qh = head * hpt + trow / tile_rows;
       if (trow >= hpt * tile_rows || r >= span.R) continue;
-      const float l = h ? l1 : l0, mrow = h ? m1 : m0, inv = l == 0.f ? 0.f : 1.0f / l;
+      const float l = h ? l1 : l0, mrow = h ? m1 : m0;
+      // (FP8: times the V scale, which scales O and not L; a power of two keeps the product exact)
+      const float inv = l == 0.f ? 0.f : (kFp8 ? (1.0f / l) * v_scale : 1.0f / l);
       const size_t row = (sp.splits == 1 ? static_cast<size_t>(qh) : static_cast<size_t>(split) * sp.batch + qh) * R +
                          span.q0 + r;
       float *out = (sp.splits == 1 ? O : sp.O_part) + row * D;
@@ -859,6 +934,27 @@ __global__ void __launch_bounds__(2 * kWG, 1)
                                    const PagedKV pk, const Band band, const SplitArgs sp, uint32_t hpt) {
   forward_body<DCH, kBF16, true, KVLayout::kPaged, true, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, sp, 0,
                                                                group, Sequences{}, pk, band, hpt);
+}
+
+// FP8 K/V: the two split paged forwards above over E4M3 pools with per-K/V-head scales (mapK / mapV: 8-bit page-pool
+// maps).  An unsplit call runs them with one split and one head per tile.
+template <uint32_t DCH, bool kBF16, bool kCausal>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    fp8_kv_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                         const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
+                         uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk,
+                         const SplitArgs sp, uint32_t hpt, const Fp8KV fp8) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged, false, true, true>(
+      mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, sp, 0, group, Sequences{}, pk, Band{}, hpt, fp8);
+}
+template <uint32_t DCH, bool kBF16>
+__global__ void __launch_bounds__(2 * kWG, 1)
+    fp8_kv_window_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                                const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
+                                uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk,
+                                const Band band, const SplitArgs sp, uint32_t hpt, const Fp8KV fp8) {
+  forward_body<DCH, kBF16, true, KVLayout::kPaged, true, true, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec,
+                                                                     sp, 0, group, Sequences{}, pk, band, hpt, fp8);
 }
 
 // ================================================================================================ backward dQ
@@ -1429,10 +1525,11 @@ cudaError_t launch_forward_paged(const AttentionParams &p, const WgmmaPlan &plan
 // Split-KV packed (seq) or paged (pk) forward of plan.splits key ranges and plan.heads_per_tile query heads per tile
 // (not both 1): with splits > 1 the split kernel writes partials [split][head][row] into the workspace and
 // merge_sequence_splits merges each sequence's rows into O and L; with one split it writes O and L itself.  Q is read in
-// boxes of m = kTileM / heads_per_tile rows x heads_per_tile heads.
+// boxes of m = kTileM / heads_per_tile rows x heads_per_tile heads.  fp8 (paged only): the pools hold E4M3 bytes, read
+// through 8-bit maps by the FP8 twins of the paged kernels.
 template <uint32_t DCH, bool kBF16, bool kCausal>
 cudaError_t launch_forward_split(const AttentionParams &p, const WgmmaPlan &plan, const Sequences *seq,
-                                 const PagedKV *pk, const Band *band, cudaStream_t stream) {
+                                 const PagedKV *pk, const Band *band, cudaStream_t stream, const Fp8KV *fp8 = nullptr) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
   TensorMaps m;
@@ -1440,9 +1537,10 @@ cudaError_t launch_forward_split(const AttentionParams &p, const WgmmaPlan &plan
   const uint32_t hpt = plan.heads_per_tile, box_rows = Cfg::kTileM / hpt;
   if (pk) {
     const uint32_t box = min(1u << pk->page_shift, Cfg::BN);
+    auto pool = fp8 ? make_tensor_map_page_pool_8bit : make_tensor_map_page_pool;
     if ((e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, box_rows, hpt)) != cudaSuccess ||
-        (e = make_tensor_map_page_pool(&m.K, p.buf[sK], p.C, pk->kv_heads, p.D, box)) != cudaSuccess ||
-        (e = make_tensor_map_page_pool(&m.V, p.buf[sV], p.C, pk->kv_heads, p.D, box)) != cudaSuccess)
+        (e = pool(&m.K, p.buf[sK], p.C, pk->kv_heads, p.D, box)) != cudaSuccess ||
+        (e = pool(&m.V, p.buf[sV], p.C, pk->kv_heads, p.D, box)) != cudaSuccess)
       return e;
   } else if ((e = make_maps<Cfg>(p, false, &m)) != cudaSuccess ||
              (e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, box_rows, hpt)) != cudaSuccess) {
@@ -1466,7 +1564,11 @@ cudaError_t launch_forward_split(const AttentionParams &p, const WgmmaPlan &plan
     kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, O, p.buf[sL], args...);
     return cudaGetLastError();
   };
-  if (pk && band)
+  if (fp8 && band)
+    e = run(fp8_kv_window_forward_wgmma<DCH, kBF16>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, *band, sp, hpt, *fp8);
+  else if (fp8)
+    e = run(fp8_kv_forward_wgmma<DCH, kBF16, kCausal>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, sp, hpt, *fp8);
+  else if (pk && band)
     e = run(split_forward_paged_band_wgmma<DCH, kBF16>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, *band, sp, hpt);
   else if (pk)
     e = run(split_forward_paged_wgmma<DCH, kBF16, kCausal>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, sp, hpt);
@@ -1695,6 +1797,28 @@ cudaError_t launch_wgmma_forward_split(const AttentionParams &p, const Sequences
   return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
     return hop::launch_forward_split<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, seq, pk,
                                                                                                             band, stream);
+  });
+}
+
+cudaError_t launch_wgmma_forward_paged_fp8(const AttentionParams &p, const PagedKV &pk, const Band *band,
+                                           const Fp8KV &fp8, bool split, uint32_t num_splits, uint32_t key_bound,
+                                           cudaStream_t stream) {
+  bool transposed = false;
+  for (int s = 0; s < kSlots; ++s) transposed = transposed || p.transposed[s];
+  if ((p.prec[sQ] != FP16 && p.prec[sQ] != BF16) || p.prec[sO] != FP32 || transposed || p.D % 16 != 0 ||
+      p.D > kWgmmaMaxHead) {
+    set_launch_detail("descriptor is outside the FP8 K/V forward kernels' domain");
+    return cudaErrorInvalidValue;
+  }
+  WgmmaPlan plan = wgmma_plan_split(p.D, pk.max_row, key_bound, pk.count, p.batch, p.group, p.split_min_blocks,
+                                    p.split_max, split ? num_splits : 1, device_sm_count(current_device()), band);
+  if (!split) {  // one split, one head per tile: the grid of the unsplit paged call
+    plan.heads_per_tile = 1;
+    plan.grid = dim3((pk.max_row + plan.par - 1) / plan.par, p.batch, pk.count);
+  }
+  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
+    return hop::launch_forward_split<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(
+        p, plan, nullptr, &pk, band, stream, &fp8);
   });
 }
 

@@ -129,6 +129,8 @@ using AttentionWindow = mfa_attention_window_t;
 using SplitKV = mfa_split_kv_t;
 // {splits, heads_per_tile, grid_size, launch_count}: what a split-KV encode launches
 using SplitPlan = mfa_split_plan_t;
+// {k_scale, v_scale}: FP8 E4M3 K/V pools with one FP32 scale per K/V head (device arrays, nullptr = 1)
+using FP8KV = mfa_fp8_kv_t;
 
 class AttentionKernel {  // AttentionKernel.swift:11-50
  public:
@@ -215,6 +217,11 @@ class AttentionKernel {  // AttentionKernel.swift:11-50
   void encode(const mfa_function_constants_t &constants, const PagedKV &paged, const SplitKV &split,
               const std::array<void *, MFA_BUFFER_COUNT> &buffers, void *cudaStream = nullptr) const {
     check(mfa_attention_kernel_encode_paged_split(handle_, &constants, &paged, &split, buffers.data(), cudaStream));
+  }
+  // the paged forward over FP8 E4M3 pools (library extension, mfa_fp8_kv_t); split == nullptr: unsplit, as encode(paged)
+  void encode(const mfa_function_constants_t &constants, const PagedKV &paged, const SplitKV *split, const FP8KV &fp8,
+              const std::array<void *, MFA_BUFFER_COUNT> &buffers, void *cudaStream = nullptr) const {
+    check(mfa_attention_kernel_encode_paged_fp8(handle_, &constants, &paged, split, &fp8, buffers.data(), cudaStream));
   }
  private:
   mfa_attention_kernel_t *handle_ = nullptr;

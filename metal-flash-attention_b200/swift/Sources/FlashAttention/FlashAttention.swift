@@ -507,6 +507,25 @@ public final class AttentionKernel {
     var split = split
     check(mfa_attention_kernel_encode_paged_split(handle, &constants, &paged, &split, &table, stream))
   }
+  /// The forward `encode` over a paged cache whose K and V pools hold FP8 E4M3 bytes with per-K/V-head scales
+  /// (`fp8`); `split` nil runs it unsplit, as `encode(constants:paged:buffers:)`.
+  public func encode(constants: mfa_function_constants_t, paged: PagedKV, split: SplitKV?, fp8: FP8KV,
+                     buffers: [AttentionOperand: UnsafeMutableRawPointer],
+                     stream: UnsafeMutableRawPointer? = nil) {
+    var table = [UnsafeMutableRawPointer?](repeating: nil, count: Int(MFA_BUFFER_COUNT))
+    for (operand, pointer) in buffers {
+      guard let binding = operand.bufferBinding else { fatalError("Operand \(operand) has no buffer binding.") }
+      table[Int(binding)] = pointer
+    }
+    var constants = constants
+    var paged = paged
+    var fp8 = fp8
+    if var split = split {
+      check(mfa_attention_kernel_encode_paged_fp8(handle, &constants, &paged, &split, &fp8, &table, stream))
+    } else {
+      check(mfa_attention_kernel_encode_paged_fp8(handle, &constants, &paged, nil, &fp8, &table, stream))
+    }
+  }
 }
 
 /// library extension: a split-KV forward.  `numSplits` 0 lets the library plan, 1...16 is taken as given;
@@ -550,5 +569,14 @@ extension mfa_function_constants_t {
   public var kvGroup: UInt32 {
     get { kv_group }
     set { kv_group = newValue }
+  }
+}
+
+/// library extension: FP8 E4M3 K/V pools of a paged forward, with one FP32 scale per K/V head in device memory
+/// (`kScale`, `vScale`: batch_count / kv_group entries each; nil means every scale is 1).
+public typealias FP8KV = mfa_fp8_kv_t
+extension mfa_fp8_kv_t {
+  public init(kScale: UnsafePointer<Float>? = nil, vScale: UnsafePointer<Float>? = nil) {
+    self.init(k_scale: kScale, v_scale: vScale)
   }
 }
