@@ -506,6 +506,50 @@ MFA_API int mfa_attention_kernel_encode_paged_fp8(const mfa_attention_kernel_t *
                                                   void *cuda_stream);
 
 /* ------------------------------------------------------------------------------------------ */
+/* Paged K/V append (library extension)                                                        */
+/* ------------------------------------------------------------------------------------------ */
+/** Writes a step's new keys and values into the page pools of a paged cache, through the table the paged forward reads
+ *  (vLLM's reshape_and_cache).  With the mfa_paged_kv_t of the step:
+ *    - sequence s owns new tokens [row_offsets[s], row_offsets[s + 1]) of k_new / v_new: Rs tokens;
+ *    - column_lengths[s] is Cs, the sequence's length with the new tokens included, as the forward reads it;
+ *    - new token i (0 <= i < Rs) becomes key p = Cs - Rs + i, pool row page_table[s][p / P] * P + p % P, every K/V head.
+ *  This is the bottom-right alignment of the forward: an append followed by a paged encode on one stream attends over
+ *  the cache with the step's tokens in it.
+ *
+ *  The kernel clamps as the forward does: row_offsets into [0, rows], Cs into [0, page_stride * P].  It never clamps a
+ *  write: a position p < 0 (Rs > Cs) or a page id outside [0, pool_rows / P) is skipped.  So the append never writes
+ *  outside k_pool / v_pool, nor a row the table does not name as one of the step's keys; tokens outside every sequence
+ *  are never read.  As for the forward, a sequence longer than max_row breaks the contract: its tokens past max_row
+ *  may be left unwritten.
+ *
+ *  fp8 == NULL: the pools hold `precision` elements ([num_pages][P][kv_heads][D]) and the append copies bit for bit.
+ *  fp8 != NULL: the pools hold E4M3 bytes, as mfa_attention_kernel_encode_paged_fp8 reads them: element x of K/V head
+ *  kv is stored as cvt.rn.satfinite.e4m3x2.f32(x / k_scale[kv]), x converted exactly to FP32 and / rounded to nearest
+ *  (v_scale for V; a NULL scale is 1).  Finite values beyond +-448 and +-inf become +-448; NaN stays NaN.  That is
+ *  torch's (x.float() / scale).clamp(-448, 448).to(torch.float8_e4m3fn), byte for byte.
+ *
+ *  One launch, no synchronisation, no allocation and no host read of device memory: the append can be captured into a
+ *  CUDA graph with the forward and replayed after column_lengths / page_table changed in place.  The host returns
+ *  MFA_ERROR_INVALID_ARGUMENT, naming the field, before any device work for: a NULL pointer (the table, its three
+ *  device arrays, append, k_new, v_new, k_pool, v_pool); count of 0 or above 65535; max_row of 0 or above rows; a
+ *  page_size that is not a power of two, is below 16, or does not divide pool_rows; page_stride of 0; kv_heads of 0;
+ *  head_dimension of 0 or above 512; token_stride below kv_heads * head_dimension; an unknown precision.  Off sm_90 it
+ *  returns MFA_ERROR_NO_DEVICE. */
+typedef struct mfa_paged_kv_append {
+  const void *k_new;       /* device: token t, K/V head kv, element d at element t * token_stride + kv * D + d */
+  const void *v_new;       /* device: the same layout and stride */
+  uint32_t rows;           /* T: tokens k_new / v_new hold (row_offsets are clamped into [0, T]) */
+  uint32_t token_stride;   /* elements from one token to the next, >= kv_heads * D; 0 = kv_heads * D */
+  uint32_t kv_heads;       /* Hkv >= 1 */
+  uint32_t head_dimension; /* D, 1..512 */
+  uint32_t pool_rows;      /* rows of each pool, num_pages * P: the forward's `column` */
+  uint32_t precision;      /* mfa_precision_t of k_new / v_new: MFA_FP32, MFA_FP16 or MFA_BF16 */
+} mfa_paged_kv_append_t;   /* 40 bytes */
+
+MFA_API int mfa_paged_kv_append(const mfa_paged_kv_t *paged, const mfa_paged_kv_append_t *append, void *k_pool,
+                                void *v_pool, const mfa_fp8_kv_t *fp8, void *cuda_stream);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Kernel cache keyed by descriptor                                                            */
 /* ------------------------------------------------------------------------------------------ */
 /** The analogue of the reference's pipeline cache (GEMMKernel.register(descriptor:) / pipelineCache[descriptor],

@@ -145,6 +145,21 @@ class FP8KV(ctypes.Structure):
         super().__init__(k_scale or None, v_scale or None)
 
 
+class PagedKVAppend(ctypes.Structure):
+    """mfa_paged_kv_append_t: the step's new tokens for appendPagedKV.  k_new / v_new: DEVICE pointers, token t's K/V
+    head kv at element t * token_stride + kv * head_dimension (token_stride 0: kv_heads * head_dimension, a contiguous
+    [rows][kv_heads][head_dimension] tensor); rows: tokens they hold; pool_rows: rows of each pool (num_pages *
+    page_size); precision: a GEMMOperandPrecision of k_new / v_new."""
+    _fields_ = [("k_new", ctypes.c_void_p), ("v_new", ctypes.c_void_p), ("rows", ctypes.c_uint32),
+                ("token_stride", ctypes.c_uint32), ("kv_heads", ctypes.c_uint32), ("head_dimension", ctypes.c_uint32),
+                ("pool_rows", ctypes.c_uint32), ("precision", ctypes.c_uint32)]
+
+    def __init__(self, k_new=0, v_new=0, rows=0, token_stride=0, kv_heads=0, head_dimension=0, pool_rows=0,
+                 precision=0):
+        super().__init__(k_new or None, v_new or None, int(rows), int(token_stride), int(kv_heads), int(head_dimension),
+                         int(pool_rows), int(precision))
+
+
 class _CWindow(ctypes.Structure):
     _fields_ = [("left", ctypes.c_int32), ("right", ctypes.c_int32)]
 
@@ -217,6 +232,8 @@ def _load():
     lib.mfa_attention_kernel_split_plan.argtypes = [c.c_void_p, c.POINTER(_CFunctionConstants),
                                                     c.POINTER(SequenceTable), c.POINTER(PagedKV), c.POINTER(SplitKV),
                                                     c.POINTER(SplitPlan)]
+    lib.mfa_paged_kv_append.argtypes = [c.POINTER(PagedKV), c.POINTER(PagedKVAppend), c.c_void_p, c.c_void_p,
+                                        c.POINTER(FP8KV), c.c_void_p]
     lib.mfa_attention_kernel_cache_fetch.argtypes = [c.POINTER(_CDescriptor), c.c_int, c.POINTER(c.c_void_p)]
     lib.mfa_attention_kernel_create_windowed.argtypes = [c.POINTER(_CKernelDescriptor), c.POINTER(_CWindow),
                                                          c.POINTER(c.c_void_p)]
@@ -276,6 +293,19 @@ def setParameterTable(type: "AttentionKernelType", text: Optional[str], transpos
     """mfa_set_parameter_table: replace (text) or restore (None) the tensor-core-family parameter table of `type`."""
     _check(_lib.mfa_set_parameter_table(int(type), int(bool(transposed)),
                                         None if text is None else text.encode()))
+
+
+def appendPagedKV(paged: PagedKV, append: PagedKVAppend, k_pool: int, v_pool: int, fp8: Optional[FP8KV] = None,
+                  stream: int = 0) -> None:
+    """mfa_paged_kv_append: writes the step's new keys and values into the page pools k_pool / v_pool (DEVICE pointers)
+    through the table of the step's paged forward.  New token i of sequence s becomes key column_lengths[s] - Rs + i.
+    fp8: the pools hold E4M3 bytes, each value divided by its K/V head's scale and saturated to +-448; None: the pools
+    hold append.precision elements, copied bit for bit.  One launch on `stream` (a cudaStream_t as int), capturable
+    into a CUDA graph."""
+    _check(_lib.mfa_paged_kv_append(ctypes.byref(paged) if paged is not None else None,
+                                    ctypes.byref(append) if append is not None else None,
+                                    ctypes.c_void_p(k_pool or None), ctypes.c_void_p(v_pool or None),
+                                    ctypes.byref(fp8) if fp8 is not None else None, ctypes.c_void_p(stream)))
 
 
 def library_path() -> str:
@@ -733,6 +763,6 @@ class AttentionKernel:
 __all__ = [
     "AttentionDescriptor", "AttentionKernelDescriptor", "AttentionKernel", "AttentionKernelType",
     "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError", "SequenceTable", "PagedKV",
-    "SplitKV", "SplitPlan", "FP8KV",
-    "library_path", "version", "setParameterTable", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
+    "SplitKV", "SplitPlan", "FP8KV", "PagedKVAppend",
+    "appendPagedKV", "library_path", "version", "setParameterTable", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
 ]

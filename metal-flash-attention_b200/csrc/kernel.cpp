@@ -196,6 +196,36 @@ static int sequences_of(const mfa_attention_kernel *k, const mfa_function_consta
   return MFA_SUCCESS;
 }
 
+// The launch form of a paged K/V table's own fields, after the checks the host can make without reading device memory,
+// shared by the forward and the append: the queries (new tokens) are `rows` rows of their buffer and the pools
+// `columns` rows.  rows_name / columns_name: what the messages call them.  kv_heads is left for the caller.
+static int paged_table_of(const mfa_paged_kv_t *t, uint32_t rows, uint32_t columns, const char *rows_name,
+                          const char *columns_name, PagedKV *out) {
+  if (!t->row_offsets || !t->column_lengths || !t->page_table)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Paged K/V: ") +
+                                                (!t->row_offsets ? "row_offsets" : !t->column_lengths ? "column_lengths"
+                                                                                                      : "page_table") +
+                                                " must not be NULL.");
+  if (t->count == 0 || t->count > kMaxSequences)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: count " + std::to_string(t->count) + " is outside [1, " +
+                                                std::to_string(kMaxSequences) + "].");
+  if (t->max_row == 0 || t->max_row > rows)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: max_row " + std::to_string(t->max_row) + " is outside [1, " +
+                                                rows_name + " = " + std::to_string(rows) + "].");
+  const uint32_t P = t->page_size;
+  if (P < 16 || (P & (P - 1)) != 0 || columns % P != 0)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: page_size " + std::to_string(P) +
+                                                " must be a power of two, at least 16, dividing " + columns_name + " = " +
+                                                std::to_string(columns) + ".");
+  if (t->page_stride == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: page_stride 0 must be at least 1.");
+  uint32_t shift = 0;
+  while ((1u << shift) < P) ++shift;
+  const uint64_t max_keys = static_cast<uint64_t>(t->page_stride) << shift;
+  *out = PagedKV{t->row_offsets, t->column_lengths, t->page_table, rows, columns / P, shift, t->page_stride,
+                 static_cast<uint32_t>(max_keys < 0x7fffffffu ? max_keys : 0x7fffffffu), 0, t->count, t->max_row};
+  return MFA_SUCCESS;
+}
+
 // The launch form of a paged K/V table, after the checks the host can make without reading device memory
 static int paged_of(const mfa_attention_kernel *k, const mfa_function_constants_t *c, const mfa_paged_kv_t *t,
                     PagedKV *out) {
@@ -211,36 +241,15 @@ static int paged_of(const mfa_attention_kernel *k, const mfa_function_constants_
   if (k->backend == MFA_BACKEND_TCGEN05 && k->descriptor.head_dimension % 8 != 0)
     return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V on MFA_BACKEND_TCGEN05 needs a head dimension that is a multiple "
                                             "of 8 (head " + std::to_string(k->descriptor.head_dimension) + ").");
-  if (!t->row_offsets || !t->column_lengths || !t->page_table)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Paged K/V: ") +
-                                                (!t->row_offsets ? "row_offsets" : !t->column_lengths ? "column_lengths"
-                                                                                                      : "page_table") +
-                                                " must not be NULL.");
-  if (t->count == 0 || t->count > kMaxSequences)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: count " + std::to_string(t->count) + " is outside [1, " +
-                                                std::to_string(kMaxSequences) + "].");
-  if (t->max_row == 0 || t->max_row > c->row)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: max_row " + std::to_string(t->max_row) +
-                                                " is outside [1, row = " + std::to_string(c->row) + "].");
-  const uint32_t P = t->page_size;
-  if (P < 16 || (P & (P - 1)) != 0 || c->column % P != 0)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: page_size " + std::to_string(P) +
-                                                " must be a power of two, at least 16, dividing column = " +
-                                                std::to_string(c->column) + ".");
-  if (t->page_stride == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: page_stride 0 must be at least 1.");
+  int status = paged_table_of(t, c->row, c->column, "row", "column", out);
+  if (status != MFA_SUCCESS) return status;
   const uint32_t batch = c->batch_count ? c->batch_count : 1;
   if (batch > kMaxBatchPerLaunch)
     return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V: batch_count " + std::to_string(batch) + " exceeds " +
                                                 std::to_string(kMaxBatchPerLaunch) + " (a paged call is one launch).");
   uint32_t group = 1;
-  const int status = kv_group_of(c, &group);
-  if (status != MFA_SUCCESS) return status;
-  uint32_t shift = 0;
-  while ((1u << shift) < P) ++shift;
-  const uint64_t max_keys = static_cast<uint64_t>(t->page_stride) << shift;
-  *out = PagedKV{t->row_offsets, t->column_lengths, t->page_table, c->row, c->column / P, shift, t->page_stride,
-                 static_cast<uint32_t>(max_keys < 0x7fffffffu ? max_keys : 0x7fffffffu), batch / group, t->count,
-                 t->max_row};
+  if ((status = kv_group_of(c, &group)) != MFA_SUCCESS) return status;
+  out->kv_heads = batch / group;
   return MFA_SUCCESS;
 }
 // The grid of a paged call is that of a packed call whose longest query sequence has max_row rows (a forward's grid
@@ -586,6 +595,47 @@ int mfa_attention_kernel_encode_sequences_split(const mfa_attention_kernel_t *ke
   int status = sequences_of(kernel, constants, table, &seq);
   if (status != MFA_SUCCESS || (status = split_of(kernel, split)) != MFA_SUCCESS) return status;
   return encode(kernel, constants, &seq, buffers, cuda_stream, split);
+}
+
+int mfa_paged_kv_append(const mfa_paged_kv_t *paged, const mfa_paged_kv_append_t *append, void *k_pool, void *v_pool,
+                        const mfa_fp8_kv_t *fp8, void *cuda_stream) {
+  if (!paged) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL paged K/V table.");
+  if (!append) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: NULL append.");
+  const mfa_paged_kv_append_t &a = *append;
+  if (!a.k_new || !a.v_new || !k_pool || !v_pool)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Paged K/V append: ") +
+                                                (!a.k_new ? "k_new" : !a.v_new ? "v_new" : !k_pool ? "k_pool" : "v_pool") +
+                                                " must not be NULL.");
+  PagedKV pk;
+  int status = paged_table_of(paged, a.rows, a.pool_rows, "rows", "pool_rows", &pk);
+  if (status != MFA_SUCCESS) return status;
+  if (a.kv_heads == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: kv_heads 0 must be at least 1.");
+  if (a.head_dimension == 0 || a.head_dimension > 512)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: head_dimension " + std::to_string(a.head_dimension) +
+                                                " is outside [1, 512].");
+  const uint64_t row_elements = static_cast<uint64_t>(a.kv_heads) * a.head_dimension;
+  if (a.token_stride != 0 && a.token_stride < row_elements)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: token_stride " + std::to_string(a.token_stride) +
+                                                " is below kv_heads * head_dimension = " + std::to_string(row_elements) +
+                                                ".");
+  if (row_elements > 0xffffffffu)  // (only reachable with token_stride 0: a nonzero stride bounds it)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: kv_heads * head_dimension = " +
+                                                std::to_string(row_elements) + " exceeds 2^32 - 1.");
+  if (a.precision > MFA_BF16)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: precision " + std::to_string(a.precision) +
+                                                " is not MFA_FP32, MFA_FP16 or MFA_BF16.");
+  if ((status = check_device()) != MFA_SUCCESS) return status;
+  pk.kv_heads = a.kv_heads;
+  const AppendSource src{a.k_new, a.v_new,
+                         a.token_stride ? a.token_stride : static_cast<uint32_t>(row_elements), a.head_dimension,
+                         static_cast<uint32_t>(row_elements), static_cast<uint8_t>(a.precision)};
+  Fp8KV scales{};
+  if (fp8) scales = Fp8KV{fp8->k_scale, fp8->v_scale};
+  const cudaError_t e = launch_paged_kv_append(pk, src, k_pool, v_pool, fp8 ? &scales : nullptr,
+                                               static_cast<cudaStream_t>(cuda_stream));
+  if (e != cudaSuccess)
+    return fail(MFA_ERROR_CUDA, std::string("launch of paged_kv_append failed: ") + cudaGetErrorString(e));
+  return MFA_SUCCESS;
 }
 
 }  // extern "C"

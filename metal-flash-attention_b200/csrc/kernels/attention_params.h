@@ -108,6 +108,20 @@ struct Fp8KV {
   const float *k_scale, *v_scale;
 };
 
+// Paged K/V append (mfa_paged_kv_append_t): the step's new tokens, token t's K/V head kv, element d at element
+// t * token_stride + kv * D + d of k / v, in `precision`
+struct AppendSource {
+  const void *k, *v;
+  uint32_t token_stride;   // elements, >= row_elements
+  uint32_t head_dimension; // D
+  uint32_t row_elements;   // kv_heads * D: the elements of one pool row
+  uint8_t precision;       // Prec
+};
+// The append of paged_kv_append.cu: one launch, grid (tokens of max_row, count).  fp8: the pools hold E4M3 bytes
+// quantized with its scales; nullptr: the pools hold `precision` elements, copied bit for bit
+cudaError_t launch_paged_kv_append(const PagedKV &pk, const AppendSource &src, void *k_pool, void *v_pool,
+                                   const Fp8KV *fp8, cudaStream_t stream);
+
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
 // seq: packed sequences, or nullptr for problems of the full R x C shape; band: a sliding window, or nullptr
 cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream);

@@ -131,6 +131,15 @@ using SplitKV = mfa_split_kv_t;
 using SplitPlan = mfa_split_plan_t;
 // {k_scale, v_scale}: FP8 E4M3 K/V pools with one FP32 scale per K/V head (device arrays, nullptr = 1)
 using FP8KV = mfa_fp8_kv_t;
+// {k_new, v_new, rows, token_stride, kv_heads, head_dimension, pool_rows, precision}: the new tokens of a paged K/V append
+using PagedKVAppend = mfa_paged_kv_append_t;
+
+// Writes a step's new keys and values into the page pools through the table of the step's paged forward (library
+// extension, mfa_paged_kv_append); fp8 == nullptr: the pools hold append.precision elements, copied bit for bit
+inline void appendPagedKV(const PagedKV &paged, const PagedKVAppend &append, void *kPool, void *vPool,
+                          const FP8KV *fp8 = nullptr, void *cudaStream = nullptr) {
+  check(mfa_paged_kv_append(&paged, &append, kPool, vPool, fp8, cudaStream));
+}
 
 class AttentionKernel {  // AttentionKernel.swift:11-50
  public:

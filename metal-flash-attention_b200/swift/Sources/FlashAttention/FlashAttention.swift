@@ -580,3 +580,30 @@ extension mfa_fp8_kv_t {
     self.init(k_scale: kScale, v_scale: vScale)
   }
 }
+
+/// library extension: the new tokens of a paged K/V append.  `kNew` / `vNew` are DEVICE pointers, token t's K/V head
+/// kv at element t * tokenStride + kv * headDimension (tokenStride 0: kvHeads * headDimension); `rows` is the tokens
+/// they hold, `poolRows` the rows of each pool (num_pages * page_size), `precision` the element type of kNew / vNew.
+public typealias PagedKVAppend = mfa_paged_kv_append_t
+extension mfa_paged_kv_append_t {
+  public init(kNew: UnsafeRawPointer, vNew: UnsafeRawPointer, rows: UInt32, tokenStride: UInt32 = 0, kvHeads: UInt32,
+              headDimension: UInt32, poolRows: UInt32, precision: GEMMOperandPrecision) {
+    self.init(k_new: kNew, v_new: vNew, rows: rows, token_stride: tokenStride, kv_heads: kvHeads,
+              head_dimension: headDimension, pool_rows: poolRows, precision: UInt32(precision.rawValue))
+  }
+}
+
+/// library extension: writes a step's new keys and values into the page pools through the table of the step's paged
+/// forward (new token i of sequence s becomes key columnLengths[s] - Rs + i).  `fp8` nil: the pools hold
+/// `append.precision` elements, copied bit for bit; otherwise E4M3 bytes, each value divided by its K/V head's scale and
+/// saturated to +-448.  One launch on `stream`, capturable into a CUDA graph with the forward.
+public func appendPagedKV(paged: PagedKV, append: PagedKVAppend, kPool: UnsafeMutableRawPointer,
+                          vPool: UnsafeMutableRawPointer, fp8: FP8KV? = nil, stream: UnsafeMutableRawPointer? = nil) {
+  var paged = paged
+  var append = append
+  if var fp8 = fp8 {
+    check(mfa_paged_kv_append(&paged, &append, kPool, vPool, &fp8, stream))
+  } else {
+    check(mfa_paged_kv_append(&paged, &append, kPool, vPool, nil, stream))
+  }
+}
