@@ -550,6 +550,54 @@ MFA_API int mfa_paged_kv_append(const mfa_paged_kv_t *paged, const mfa_paged_kv_
                                 void *v_pool, const mfa_fp8_kv_t *fp8, void *cuda_stream);
 
 /* ------------------------------------------------------------------------------------------ */
+/* Rotary append (library extension)                                                           */
+/* ------------------------------------------------------------------------------------------ */
+/** mfa_paged_kv_append with rotary position embedding (RoPE), FlashAttention's rotary_cos / rotary_sin of
+ *  flash_attn_with_kvcache: the step's queries and new keys are rotated at their cache positions, and the queries are
+ *  written in the paged forward's Q layout, in one launch.
+ *
+ *  New token i of sequence s sits at position p = Cs - Rs + i: the key mfa_paged_kv_append writes, with the same
+ *  clamping of query ranges and Cs.  With c = cos[p][j] and s = sin[p][j], each pair (x, y) of q (every query head) and
+ *  of k (every K/V head) becomes x' = x c - y s, y' = y c + x s: x, y converted exactly to FP32, each product and the
+ *  sum or difference rounded separately (no FMA), the result rounded to nearest-even to append->precision (FP32 stays
+ *  FP32).  Pairs are (j, j + r/2) (GPT-NeoX / Llama rotate_half) or, interleaved, (2j, 2j + 1) (GPT-J), for
+ *  0 <= j < r/2.  Elements d >= r and V pass through unchanged.  FP8 pools receive the rounded rotated k quantized
+ *  exactly as mfa_paged_kv_append quantizes a source value.  So k_pool / v_pool hold the bytes mfa_paged_kv_append
+ *  writes for rope(k_new) and v_new, and q_out holds rope(q_new) transposed to [query_heads][rows][D], with rope
+ *  torch's (x.float() * c - y.float() * s).to(dtype), op by op.
+ *
+ *  Row (h, q0 + i) of q_out is written iff p >= 0: rows of tokens with p < 0 (Rs > Cs) and rows outside every sequence
+ *  are never written.  A K/V row is written under mfa_paged_kv_append's rule.  Scaled RoPE variants (linear, NTK,
+ *  YaRN, Llama-3) live in the tables.  vLLM's cos_sin_cache [max_pos][r] (cos half, then sin half) is passed as
+ *  cos = base, sin = base + r/2, table_stride = r; FlashAttention's [seqlen][r/2] tables use table_stride 0.
+ *
+ *  No synchronisation, allocation or host read of device memory: the call captures into a CUDA graph with the split
+ *  forward and replays as column_lengths / page_table change in place.  q_new and q_out must not overlap.
+ *
+ *  Every check of mfa_paged_kv_append is made first, identically.  Beyond them the host returns
+ *  MFA_ERROR_INVALID_ARGUMENT, naming the field, before any device work for: a NULL rotary, q_new, q_out, cos or sin;
+ *  query_heads of 0 or not a multiple of kv_heads; query_heads * D above 2^32 - 1; a nonzero q_token_stride below
+ *  query_heads * D; rotary_dim of 0, odd or above D; a nonzero table_stride below r / 2; positions below
+ *  page_stride * page_size (so the kernel never reads past the tables); interleaved other than 0 or 1.  Off sm_90 it
+ *  returns MFA_ERROR_NO_DEVICE. */
+typedef struct mfa_rotary {
+  const void *q_new;       /* device: token t, query head h, element d at t * q_token_stride + h * D + d; append->precision */
+  void *q_out;             /* device: the paged forward's Q buffer, [query_heads][append->rows][D]; append->precision */
+  const float *cos;        /* device FP32: position p, frequency j (0 <= j < rotary_dim / 2) at p * table_stride + j */
+  const float *sin;        /* the same layout */
+  uint32_t query_heads;    /* H: a multiple of append->kv_heads (the forward's batch_count) */
+  uint32_t q_token_stride; /* elements from one token to the next, >= query_heads * D; 0 = query_heads * D */
+  uint32_t rotary_dim;     /* r: even, 2..D; elements d >= r pass through unchanged (partial rotary) */
+  uint32_t table_stride;   /* floats per table row, >= r / 2; 0 = r / 2 */
+  uint32_t positions;      /* rows of cos / sin: at least page_stride * page_size */
+  uint32_t interleaved;    /* 0: pairs (j, j + r/2) (GPT-NeoX / Llama rotate_half); 1: pairs (2j, 2j + 1) (GPT-J) */
+} mfa_rotary_t;            /* 56 bytes */
+
+MFA_API int mfa_paged_kv_append_rotary(const mfa_paged_kv_t *paged, const mfa_paged_kv_append_t *append,
+                                       const mfa_rotary_t *rotary, void *k_pool, void *v_pool,
+                                       const mfa_fp8_kv_t *fp8, void *cuda_stream);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Kernel cache keyed by descriptor                                                            */
 /* ------------------------------------------------------------------------------------------ */
 /** The analogue of the reference's pipeline cache (GEMMKernel.register(descriptor:) / pipelineCache[descriptor],

@@ -160,6 +160,24 @@ class PagedKVAppend(ctypes.Structure):
                          int(pool_rows), int(precision))
 
 
+class Rotary(ctypes.Structure):
+    """mfa_rotary_t: rotary position embedding for appendPagedKV(..., rotary=).  q_new: DEVICE pointer, token t's query
+    head h at element t * q_token_stride + h * D (0: query_heads * D, a contiguous [rows][query_heads][D] tensor), in
+    append.precision; q_out: the paged forward's Q buffer [query_heads][append.rows][D]; cos / sin: float32 DEVICE
+    tables, position p, frequency j < rotary_dim / 2 at p * table_stride + j (0: rotary_dim / 2); positions: their
+    rows, at least page_stride * page_size; interleaved: 0 pairs (j, j + r/2) (GPT-NeoX / Llama), 1 pairs (2j, 2j + 1)
+    (GPT-J)."""
+    _fields_ = [("q_new", ctypes.c_void_p), ("q_out", ctypes.c_void_p), ("cos", ctypes.c_void_p),
+                ("sin", ctypes.c_void_p), ("query_heads", ctypes.c_uint32), ("q_token_stride", ctypes.c_uint32),
+                ("rotary_dim", ctypes.c_uint32), ("table_stride", ctypes.c_uint32), ("positions", ctypes.c_uint32),
+                ("interleaved", ctypes.c_uint32)]
+
+    def __init__(self, q_new=0, q_out=0, cos=0, sin=0, query_heads=0, q_token_stride=0, rotary_dim=0, table_stride=0,
+                 positions=0, interleaved=0):
+        super().__init__(q_new or None, q_out or None, cos or None, sin or None, int(query_heads), int(q_token_stride),
+                         int(rotary_dim), int(table_stride), int(positions), int(interleaved))
+
+
 class _CWindow(ctypes.Structure):
     _fields_ = [("left", ctypes.c_int32), ("right", ctypes.c_int32)]
 
@@ -234,6 +252,8 @@ def _load():
                                                     c.POINTER(SplitPlan)]
     lib.mfa_paged_kv_append.argtypes = [c.POINTER(PagedKV), c.POINTER(PagedKVAppend), c.c_void_p, c.c_void_p,
                                         c.POINTER(FP8KV), c.c_void_p]
+    lib.mfa_paged_kv_append_rotary.argtypes = [c.POINTER(PagedKV), c.POINTER(PagedKVAppend), c.POINTER(Rotary),
+                                               c.c_void_p, c.c_void_p, c.POINTER(FP8KV), c.c_void_p]
     lib.mfa_attention_kernel_cache_fetch.argtypes = [c.POINTER(_CDescriptor), c.c_int, c.POINTER(c.c_void_p)]
     lib.mfa_attention_kernel_create_windowed.argtypes = [c.POINTER(_CKernelDescriptor), c.POINTER(_CWindow),
                                                          c.POINTER(c.c_void_p)]
@@ -296,16 +316,21 @@ def setParameterTable(type: "AttentionKernelType", text: Optional[str], transpos
 
 
 def appendPagedKV(paged: PagedKV, append: PagedKVAppend, k_pool: int, v_pool: int, fp8: Optional[FP8KV] = None,
-                  stream: int = 0) -> None:
+                  stream: int = 0, rotary: Optional[Rotary] = None) -> None:
     """mfa_paged_kv_append: writes the step's new keys and values into the page pools k_pool / v_pool (DEVICE pointers)
     through the table of the step's paged forward.  New token i of sequence s becomes key column_lengths[s] - Rs + i.
     fp8: the pools hold E4M3 bytes, each value divided by its K/V head's scale and saturated to +-448; None: the pools
     hold append.precision elements, copied bit for bit.  One launch on `stream` (a cudaStream_t as int), capturable
-    into a CUDA graph."""
-    _check(_lib.mfa_paged_kv_append(ctypes.byref(paged) if paged is not None else None,
-                                    ctypes.byref(append) if append is not None else None,
-                                    ctypes.c_void_p(k_pool or None), ctypes.c_void_p(v_pool or None),
-                                    ctypes.byref(fp8) if fp8 is not None else None, ctypes.c_void_p(stream)))
+    into a CUDA graph.
+    rotary (mfa_paged_kv_append_rotary): the queries and new keys are also rotated by RoPE at their cache positions,
+    and the queries written to rotary.q_out in the paged forward's [query_heads][rows][D] layout, in the same launch."""
+    args = (ctypes.byref(paged) if paged is not None else None, ctypes.byref(append) if append is not None else None)
+    tail = (ctypes.c_void_p(k_pool or None), ctypes.c_void_p(v_pool or None),
+            ctypes.byref(fp8) if fp8 is not None else None, ctypes.c_void_p(stream))
+    if rotary is None:
+        _check(_lib.mfa_paged_kv_append(*args, *tail))
+    else:
+        _check(_lib.mfa_paged_kv_append_rotary(*args, ctypes.byref(rotary), *tail))
 
 
 def library_path() -> str:
@@ -763,6 +788,6 @@ class AttentionKernel:
 __all__ = [
     "AttentionDescriptor", "AttentionKernelDescriptor", "AttentionKernel", "AttentionKernelType",
     "AttentionOperand", "GEMMOperandPrecision", "FunctionConstantValues", "Backend", "MFAError", "SequenceTable", "PagedKV",
-    "SplitKV", "SplitPlan", "FP8KV", "PagedKVAppend",
+    "SplitKV", "SplitPlan", "FP8KV", "PagedKVAppend", "Rotary",
     "appendPagedKV", "library_path", "version", "setParameterTable", "hostAlloc", "hostFree", "bindThreadToDevice", "releaseDeviceResources",
 ]

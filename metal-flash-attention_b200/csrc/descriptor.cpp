@@ -438,7 +438,7 @@ using namespace mfa;
 extern "C" {
 
 const char *mfa_last_error(void) { return g_last_error.c_str(); }
-const char *mfa_version(void) { return "mfa_b200 0.5 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family, grouped K/V, packed sequences, paged K/V, sliding window, split-KV decode, FP8 K/V, paged K/V append)"; }
+const char *mfa_version(void) { return "mfa_b200 0.5 (sm_90a; wgmma+TMA forward / dQ / dK-dV, SIMT FP32 family, grouped K/V, packed sequences, paged K/V, sliding window, split-KV decode, FP8 K/V, paged K/V append, rotary append)"; }
 
 int mfa_precision_size(mfa_precision_t precision) { return precision == MFA_FP32 ? 4 : 2; }
 const char *mfa_precision_name(mfa_precision_t precision) {

@@ -226,6 +226,41 @@ static int paged_table_of(const mfa_paged_kv_t *t, uint32_t rows, uint32_t colum
   return MFA_SUCCESS;
 }
 
+// The launch form of a paged K/V append (table and new tokens), after every check mfa_paged_kv_append makes before it
+// looks for a device
+static int append_of(const mfa_paged_kv_t *paged, const mfa_paged_kv_append_t *append, const void *k_pool,
+                     const void *v_pool, PagedKV *pk, AppendSource *src) {
+  if (!paged) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL paged K/V table.");
+  if (!append) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: NULL append.");
+  const mfa_paged_kv_append_t &a = *append;
+  if (!a.k_new || !a.v_new || !k_pool || !v_pool)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Paged K/V append: ") +
+                                                (!a.k_new ? "k_new" : !a.v_new ? "v_new" : !k_pool ? "k_pool" : "v_pool") +
+                                                " must not be NULL.");
+  const int status = paged_table_of(paged, a.rows, a.pool_rows, "rows", "pool_rows", pk);
+  if (status != MFA_SUCCESS) return status;
+  if (a.kv_heads == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: kv_heads 0 must be at least 1.");
+  if (a.head_dimension == 0 || a.head_dimension > 512)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: head_dimension " + std::to_string(a.head_dimension) +
+                                                " is outside [1, 512].");
+  const uint64_t row_elements = static_cast<uint64_t>(a.kv_heads) * a.head_dimension;
+  if (a.token_stride != 0 && a.token_stride < row_elements)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: token_stride " + std::to_string(a.token_stride) +
+                                                " is below kv_heads * head_dimension = " + std::to_string(row_elements) +
+                                                ".");
+  if (row_elements > 0xffffffffu)  // (only reachable with token_stride 0: a nonzero stride bounds it)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: kv_heads * head_dimension = " +
+                                                std::to_string(row_elements) + " exceeds 2^32 - 1.");
+  if (a.precision > MFA_BF16)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: precision " + std::to_string(a.precision) +
+                                                " is not MFA_FP32, MFA_FP16 or MFA_BF16.");
+  pk->kv_heads = a.kv_heads;
+  *src = AppendSource{a.k_new, a.v_new,
+                      a.token_stride ? a.token_stride : static_cast<uint32_t>(row_elements), a.head_dimension,
+                      static_cast<uint32_t>(row_elements), static_cast<uint8_t>(a.precision)};
+  return MFA_SUCCESS;
+}
+
 // The launch form of a paged K/V table, after the checks the host can make without reading device memory
 static int paged_of(const mfa_attention_kernel *k, const mfa_function_constants_t *c, const mfa_paged_kv_t *t,
                     PagedKV *out) {
@@ -599,42 +634,68 @@ int mfa_attention_kernel_encode_sequences_split(const mfa_attention_kernel_t *ke
 
 int mfa_paged_kv_append(const mfa_paged_kv_t *paged, const mfa_paged_kv_append_t *append, void *k_pool, void *v_pool,
                         const mfa_fp8_kv_t *fp8, void *cuda_stream) {
-  if (!paged) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL paged K/V table.");
-  if (!append) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: NULL append.");
-  const mfa_paged_kv_append_t &a = *append;
-  if (!a.k_new || !a.v_new || !k_pool || !v_pool)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Paged K/V append: ") +
-                                                (!a.k_new ? "k_new" : !a.v_new ? "v_new" : !k_pool ? "k_pool" : "v_pool") +
-                                                " must not be NULL.");
   PagedKV pk;
-  int status = paged_table_of(paged, a.rows, a.pool_rows, "rows", "pool_rows", &pk);
-  if (status != MFA_SUCCESS) return status;
-  if (a.kv_heads == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: kv_heads 0 must be at least 1.");
-  if (a.head_dimension == 0 || a.head_dimension > 512)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: head_dimension " + std::to_string(a.head_dimension) +
-                                                " is outside [1, 512].");
-  const uint64_t row_elements = static_cast<uint64_t>(a.kv_heads) * a.head_dimension;
-  if (a.token_stride != 0 && a.token_stride < row_elements)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: token_stride " + std::to_string(a.token_stride) +
-                                                " is below kv_heads * head_dimension = " + std::to_string(row_elements) +
-                                                ".");
-  if (row_elements > 0xffffffffu)  // (only reachable with token_stride 0: a nonzero stride bounds it)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: kv_heads * head_dimension = " +
-                                                std::to_string(row_elements) + " exceeds 2^32 - 1.");
-  if (a.precision > MFA_BF16)
-    return fail(MFA_ERROR_INVALID_ARGUMENT, "Paged K/V append: precision " + std::to_string(a.precision) +
-                                                " is not MFA_FP32, MFA_FP16 or MFA_BF16.");
-  if ((status = check_device()) != MFA_SUCCESS) return status;
-  pk.kv_heads = a.kv_heads;
-  const AppendSource src{a.k_new, a.v_new,
-                         a.token_stride ? a.token_stride : static_cast<uint32_t>(row_elements), a.head_dimension,
-                         static_cast<uint32_t>(row_elements), static_cast<uint8_t>(a.precision)};
+  AppendSource src;
+  int status = append_of(paged, append, k_pool, v_pool, &pk, &src);
+  if (status != MFA_SUCCESS || (status = check_device()) != MFA_SUCCESS) return status;
   Fp8KV scales{};
   if (fp8) scales = Fp8KV{fp8->k_scale, fp8->v_scale};
   const cudaError_t e = launch_paged_kv_append(pk, src, k_pool, v_pool, fp8 ? &scales : nullptr,
                                                static_cast<cudaStream_t>(cuda_stream));
   if (e != cudaSuccess)
     return fail(MFA_ERROR_CUDA, std::string("launch of paged_kv_append failed: ") + cudaGetErrorString(e));
+  return MFA_SUCCESS;
+}
+
+int mfa_paged_kv_append_rotary(const mfa_paged_kv_t *paged, const mfa_paged_kv_append_t *append,
+                               const mfa_rotary_t *rotary, void *k_pool, void *v_pool, const mfa_fp8_kv_t *fp8,
+                               void *cuda_stream) {
+  PagedKV pk;
+  AppendSource src;
+  int status = append_of(paged, append, k_pool, v_pool, &pk, &src);
+  if (status != MFA_SUCCESS) return status;
+  if (!rotary) return fail(MFA_ERROR_INVALID_ARGUMENT, "Rotary append: NULL rotary.");
+  const mfa_rotary_t &r = *rotary;
+  if (!r.q_new || !r.q_out || !r.cos || !r.sin)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, std::string("Rotary append: ") +
+                                                (!r.q_new ? "q_new" : !r.q_out ? "q_out" : !r.cos ? "cos" : "sin") +
+                                                " must not be NULL.");
+  if (r.query_heads == 0 || r.query_heads % pk.kv_heads != 0)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Rotary append: query_heads " + std::to_string(r.query_heads) +
+                                                " is not a positive multiple of kv_heads = " +
+                                                std::to_string(pk.kv_heads) + ".");
+  const uint64_t q_elements = static_cast<uint64_t>(r.query_heads) * src.head_dimension;
+  if (q_elements > 0xffffffffu)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Rotary append: query_heads * head_dimension = " +
+                                                std::to_string(q_elements) + " exceeds 2^32 - 1.");
+  if (r.q_token_stride != 0 && r.q_token_stride < q_elements)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Rotary append: q_token_stride " + std::to_string(r.q_token_stride) +
+                                                " is below query_heads * head_dimension = " +
+                                                std::to_string(q_elements) + ".");
+  if (r.rotary_dim == 0 || r.rotary_dim % 2 != 0 || r.rotary_dim > src.head_dimension)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Rotary append: rotary_dim " + std::to_string(r.rotary_dim) +
+                                                " must be even and in [2, head_dimension = " +
+                                                std::to_string(src.head_dimension) + "].");
+  if (r.table_stride != 0 && r.table_stride < r.rotary_dim / 2)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Rotary append: table_stride " + std::to_string(r.table_stride) +
+                                                " is below rotary_dim / 2 = " + std::to_string(r.rotary_dim / 2) + ".");
+  const uint64_t keys = static_cast<uint64_t>(paged->page_stride) * paged->page_size;
+  if (r.positions < keys)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Rotary append: positions " + std::to_string(r.positions) +
+                                                " is below page_stride * page_size = " + std::to_string(keys) + ".");
+  if (r.interleaved > 1)
+    return fail(MFA_ERROR_INVALID_ARGUMENT, "Rotary append: interleaved " + std::to_string(r.interleaved) +
+                                                " is not 0 or 1.");
+  if ((status = check_device()) != MFA_SUCCESS) return status;
+  const RotarySource rot{r.q_new, r.q_out, r.cos, r.sin, r.query_heads,
+                         r.q_token_stride ? r.q_token_stride : static_cast<uint32_t>(q_elements), r.rotary_dim,
+                         r.table_stride ? r.table_stride : r.rotary_dim / 2, r.interleaved != 0};
+  Fp8KV scales{};
+  if (fp8) scales = Fp8KV{fp8->k_scale, fp8->v_scale};
+  const cudaError_t e = launch_rotary_kv_append(pk, src, rot, k_pool, v_pool, fp8 ? &scales : nullptr,
+                                                static_cast<cudaStream_t>(cuda_stream));
+  if (e != cudaSuccess)
+    return fail(MFA_ERROR_CUDA, std::string("launch of rotary_kv_append failed: ") + cudaGetErrorString(e));
   return MFA_SUCCESS;
 }
 

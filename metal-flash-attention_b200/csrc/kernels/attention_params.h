@@ -122,6 +122,23 @@ struct AppendSource {
 cudaError_t launch_paged_kv_append(const PagedKV &pk, const AppendSource &src, void *k_pool, void *v_pool,
                                    const Fp8KV *fp8, cudaStream_t stream);
 
+// Rotary append (mfa_rotary_t): the step's queries, token t's query head h, element d at t * q_token_stride + h * D + d
+// of q, in the append's precision, rotated into q_out [query_heads][rows][D]; cos / sin FP32, position p, frequency j
+// at p * table_stride + j
+struct RotarySource {
+  const void *q;
+  void *q_out;
+  const float *cos, *sin;
+  uint32_t query_heads;
+  uint32_t q_token_stride;  // elements, >= query_heads * D
+  uint32_t rotary_dim;      // r: even, 2..D
+  uint32_t table_stride;    // floats, >= r / 2
+  bool interleaved;         // pairs (2j, 2j + 1), else (j, j + r / 2)
+};
+// The rotary append of rotary_append.cu: the append above, with q and k rotated at their cache positions, in one launch
+cudaError_t launch_rotary_kv_append(const PagedKV &pk, const AppendSource &src, const RotarySource &rot, void *k_pool,
+                                    void *v_pool, const Fp8KV *fp8, cudaStream_t stream);
+
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
 // seq: packed sequences, or nullptr for problems of the full R x C shape; band: a sliding window, or nullptr
 cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream);

@@ -140,6 +140,15 @@ inline void appendPagedKV(const PagedKV &paged, const PagedKVAppend &append, voi
                           const FP8KV *fp8 = nullptr, void *cudaStream = nullptr) {
   check(mfa_paged_kv_append(&paged, &append, kPool, vPool, fp8, cudaStream));
 }
+// {q_new, q_out, cos, sin, query_heads, q_token_stride, rotary_dim, table_stride, positions, interleaved}: rotary
+// position embedding of the queries and new keys of a paged K/V append
+using Rotary = mfa_rotary_t;
+// appendPagedKV with the queries and new keys rotated at their cache positions, and the queries written to rotary.q_out
+// in the paged forward's [query_heads][rows][D] layout (library extension, mfa_paged_kv_append_rotary)
+inline void appendPagedKV(const PagedKV &paged, const PagedKVAppend &append, const Rotary &rotary, void *kPool,
+                          void *vPool, const FP8KV *fp8 = nullptr, void *cudaStream = nullptr) {
+  check(mfa_paged_kv_append_rotary(&paged, &append, &rotary, kPool, vPool, fp8, cudaStream));
+}
 
 class AttentionKernel {  // AttentionKernel.swift:11-50
  public:

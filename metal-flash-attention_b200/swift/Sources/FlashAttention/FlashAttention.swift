@@ -607,3 +607,32 @@ public func appendPagedKV(paged: PagedKV, append: PagedKVAppend, kPool: UnsafeMu
     check(mfa_paged_kv_append(&paged, &append, kPool, vPool, nil, stream))
   }
 }
+
+/// library extension: rotary position embedding for a paged K/V append.  `qNew` is a DEVICE pointer, token t's query
+/// head h at element t * qTokenStride + h * headDimension (qTokenStride 0: queryHeads * headDimension), in the append's
+/// precision; `qOut` the paged forward's Q buffer [queryHeads][rows][headDimension]; `cos` / `sin` Float tables in device
+/// memory, position p, frequency j < rotaryDim / 2 at p * tableStride + j (tableStride 0: rotaryDim / 2), `positions`
+/// rows of them (at least pageStride * pageSize); `interleaved` pairs (2j, 2j + 1) (GPT-J), else (j, j + rotaryDim / 2).
+public typealias Rotary = mfa_rotary_t
+extension mfa_rotary_t {
+  public init(qNew: UnsafeRawPointer, qOut: UnsafeMutableRawPointer, cos: UnsafePointer<Float>,
+              sin: UnsafePointer<Float>, queryHeads: UInt32, qTokenStride: UInt32 = 0, rotaryDim: UInt32,
+              tableStride: UInt32 = 0, positions: UInt32, interleaved: Bool = false) {
+    self.init(q_new: qNew, q_out: qOut, cos: cos, sin: sin, query_heads: queryHeads, q_token_stride: qTokenStride,
+              rotary_dim: rotaryDim, table_stride: tableStride, positions: positions, interleaved: interleaved ? 1 : 0)
+  }
+}
+
+/// library extension: `appendPagedKV` with the queries and new keys rotated by RoPE at their cache positions, and the
+/// queries written to `rotary.qOut` in the paged forward's layout, in the same launch.
+public func appendPagedKV(paged: PagedKV, append: PagedKVAppend, rotary: Rotary, kPool: UnsafeMutableRawPointer,
+                          vPool: UnsafeMutableRawPointer, fp8: FP8KV? = nil, stream: UnsafeMutableRawPointer? = nil) {
+  var paged = paged
+  var append = append
+  var rotary = rotary
+  if var fp8 = fp8 {
+    check(mfa_paged_kv_append_rotary(&paged, &append, &rotary, kPool, vPool, &fp8, stream))
+  } else {
+    check(mfa_paged_kv_append_rotary(&paged, &append, &rotary, kPool, vPool, nil, stream))
+  }
+}

@@ -3,8 +3,9 @@
     python scripts/sass_diff.py                  # HEAD against the working tree
     python scripts/sass_diff.py --base HEAD~1    # the last commit's parent against the working tree
 
-Both trees compile wgmma_attention.cu and simt_attention.cu through the library's Makefile, with the build's flags,
-into temporary directories; nothing in the repository is written.  Functions are matched by mangled name.  The script
+Both trees compile the kernel sources in SOURCES through the library's Makefile, with the build's flags, into
+temporary directories; nothing in the repository is written.  A source the base does not have is compiled from the
+working tree alone and its functions are listed as new.  Functions are matched by mangled name.  The script
 prints every function whose SASS is not byte-identical, with its instruction count before and after, and fails (exit
 status 1) when a function appears or disappears, or when anything ptxas -v reports differs from the base: a function's
 registers, barriers, shared and constant memory, stack frame, spills or diagnostics (counted by code), or the
@@ -18,20 +19,28 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join("metal-flash-attention_b200", "csrc")
-SOURCES = ("kernels/wgmma_attention.cu", "kernels/simt_attention.cu")
+SOURCES = ("kernels/wgmma_attention.cu", "kernels/simt_attention.cu", "kernels/paged_append.cu",
+           "kernels/rotary_append.cu")
 CUOBJDUMP = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "cuobjdump")
 
 
 def compile_tree(tree, out):
-    """Object files of SOURCES compiled from `tree`'s Makefile into `out`: [(object, ptxas log)]"""
-    objs = [os.path.join(out, src.replace(".cu", ".o")) for src in SOURCES]
+    """Object files of the SOURCES `tree` has, compiled from its Makefile into `out`: {source: (object, ptxas log)}"""
+    present = [src for src in SOURCES if os.path.exists(os.path.join(tree, CSRC, src))]
+    objs = [os.path.join(out, src.replace(".cu", ".o")) for src in present]
     subprocess.check_call(["make", "-s", "-j", str(len(objs)), "-C", os.path.join(tree, CSRC), f"BUILD={out}", *objs])
-    return [(obj, obj + ".ptxas.log") for obj in objs]
+    return {src: (obj, obj + ".ptxas.log") for src, obj in zip(present, objs)}
+
+
+def anonymous(text):
+    """text with each anonymous namespace's per-compilation id removed: nvcc derives it from the compilation, so the
+    same source compiled in two trees names its functions differently"""
+    return re.sub(r"_GLOBAL__N__[0-9a-f]+_", "_GLOBAL__N__", text)
 
 
 def sass(obj):
     """{function: SASS text} of an object file"""
-    text = subprocess.check_output([CUOBJDUMP, "-sass", obj], text=True)
+    text = anonymous(subprocess.check_output([CUOBJDUMP, "-sass", obj], text=True))
     funcs, name = {}, None
     for line in text.splitlines():
         m = re.search(r"Function : (\S+)", line)
@@ -53,7 +62,7 @@ def ptxas_report(log):
     source edit).  Key None holds the lines that belong to no function, such as the gmem total."""
     report, name = {None: {}}, None
     with open(log) as f:
-        for line in f:
+        for line in map(anonymous, f):
             text = line.split(":", 1)[-1].strip()
             m = re.search(r"Compiling entry function '(\S+)'|Function properties for (\S+)", line)
             if m:
@@ -84,7 +93,11 @@ def main():
         subprocess.run(["tar", "-x", "-C", base_tree], input=archive, check=True)
         before = compile_tree(base_tree, os.path.join(tmp, "build_base"))
         after = compile_tree(ROOT, os.path.join(tmp, "build_tree"))
-        for src, (obj_a, log_a), (obj_b, log_b) in zip(SOURCES, before, after):
+        for src in SOURCES:
+            if src not in before:
+                print(f"{src}: new in the working tree, {len(sass(after[src][0]))} functions")
+                continue
+            (obj_a, log_a), (obj_b, log_b) = before[src], after[src]
             sa, sb = sass(obj_a), sass(obj_b)
             ra, rb = ptxas_report(log_a), ptxas_report(log_b)
             same = [f for f in sa if f in sb and sa[f] == sb[f]]
