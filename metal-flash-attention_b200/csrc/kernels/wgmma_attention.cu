@@ -123,7 +123,11 @@ struct SmemLayout {
 // with parity (n >> 1) & 1; bar[0] tracks the resident tiles.  Thread 0 issues every load; a load callback
 // load(n, dst, bar) issues the TMA loads of step n's two tiles into dst.  The callbacks are taken by reference: copying
 // the closures into these calls made ptxas schedule the dK/dV kernels differently (1-2 registers, more instructions).
-template <class Smem>
+//
+// kRelease: stages are freed through mbarriers instead of a CTA-wide barrier, so the two warpgroups drift apart and one's
+// softmax can run while the other's wgmmas hold the tensor cores.  Each warpgroup arrives on the empty barrier
+// bar[3 + s] of a stage it is done with (count 2); thread 0 waits on it before it refills the stage (refill).
+template <class Smem, bool kRelease = false>
 struct Ring {
   uint8_t *base;
   uint64_t *bar;
@@ -138,6 +142,8 @@ struct Ring {
   __device__ __forceinline__ void init() const {
     if (threadIdx.x == 0) {
       for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
+      if constexpr (kRelease)
+        for (int i = 3; i < 5; ++i) mbar_init(&bar[i], 2);  // one arrive per warpgroup
       fence_barrier_init();
     }
     __syncthreads();
@@ -163,6 +169,19 @@ struct Ring {
   __device__ __forceinline__ void release_and_refill(uint32_t n, uint32_t total, const Load &load) const {
     __syncthreads();
     if (threadIdx.x == 0 && n + 2 < total) this->load(n + 2, n & 1, load);
+  }
+  // kRelease: this warpgroup is done with step n (one thread: its wgmma_wait retired the warpgroup's wgmmas, and with
+  // them their reads of the stage)
+  __device__ __forceinline__ void release(uint32_t n) const {
+    if (threadIdx.x % kWG == 0) mbar_arrive(&bar[3 + (n & 1)]);
+  }
+  // kRelease, thread 0: step n + 2 into the stage of step n once both warpgroups have released it
+  template <class Load>
+  __device__ __forceinline__ void refill(uint32_t n, uint32_t total, const Load &load) const {
+    if (threadIdx.x == 0 && n + 2 < total) {
+      mbar_wait(&bar[3 + (n & 1)], (n >> 1) & 1);
+      this->load(n + 2, n & 1, load);
+    }
   }
 };
 
@@ -574,7 +593,9 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
   using Smem = std::conditional_t<kFp8, typename Cfg::Fp8Smem, typename Cfg::Smem>;
-  const Ring<Smem> ring(smem_raw);  // resident Q; step j: K and V of key block kb0 + j
+  // the unmasked fixed-length forward has no CTA-wide barrier in its key loop (Ring's kRelease)
+  constexpr bool kRelease = kLayout == KVLayout::kFixed && !kCausal;
+  const Ring<Smem, kRelease> ring(smem_raw);  // resident Q; step j: K and V of key block kb0 + j
   const uint32_t tid = threadIdx.x, wg = tid / kWG, t = tid % kWG;
   const uint32_t tile = kSplit ? blockIdx.x / sp.splits : blockIdx.x;
   // (causal: unlike dQ, the forward gains nothing measurable from starting the tiles with the most key blocks first)
@@ -702,6 +723,10 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
     wgmma_fence();
     mma_ss<DCH, BN, kBF16, Cfg::kTileM>(sc, sQ, wg * kRows, sK);
     wgmma_commit();
+    // kRelease: the stage of step j - 1 takes step j + 1 while this S product runs (thread 0 may wait there for the
+    // other warpgroup to release it)
+    if constexpr (kRelease)
+      if (j > 0) ring.refill(j - 1, blocks, load_kv);
     wgmma_wait<0>();
     fence_regs(sc);
 
@@ -779,6 +804,8 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
     fence_regs(o);
     if constexpr (kFp8)
       __syncthreads();  // every warpgroup is done with the converted stage: the next block may overwrite it
+    else if constexpr (kRelease)
+      ring.release(j);
     else
       ring.release_and_refill(j, blocks, load_kv);
   }
