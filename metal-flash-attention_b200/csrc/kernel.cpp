@@ -287,21 +287,22 @@ static int paged_of(const mfa_attention_kernel *k, const mfa_function_constants_
   out->kv_heads = batch / group;
   return MFA_SUCCESS;
 }
-// The grid of a paged call is that of a packed call whose longest query sequence has max_row rows (a forward's grid
-// does not depend on the keys)
-static Sequences grid_of(const PagedKV &pk) {
-  return Sequences{pk.row_offsets, nullptr, pk.rows, 0, pk.count, pk.max_row, 1};
-}
 
-// A split-KV request (mfa_split_kv_t), after the checks the host can make; the table's checks come first
+// A split-KV request (mfa_split_kv_t) of a call over call->seq or call->pk, after the checks the host can make; the
+// table's checks come first.  The key bound the plan cuts is the hint, or the table's bound (capped so that block counts
+// cannot overflow).
 constexpr uint32_t kMaxKeySplits = 16;
-static int split_of(const mfa_attention_kernel *k, const mfa_split_kv_t *s) {
+static int split_of(const mfa_attention_kernel *k, const mfa_split_kv_t *s, ForwardCall *call) {
   if (!s) return fail(MFA_ERROR_INVALID_ARGUMENT, "Split-KV: NULL split.");
   if (k->type != MFA_FORWARD)
     return fail(MFA_ERROR_INVALID_ARGUMENT, "Split-KV: only the forward kernel splits its key range.");
   if (s->num_splits > kMaxKeySplits)
     return fail(MFA_ERROR_INVALID_ARGUMENT, "Split-KV: num_splits " + std::to_string(s->num_splits) + " is above " +
                                                 std::to_string(kMaxKeySplits) + ".");
+  const uint32_t bound = s->max_column ? s->max_column : (call->seq ? call->seq->max_column : call->pk->max_keys);
+  call->split = true;
+  call->num_splits = s->num_splits;
+  call->key_bound = bound < 0x7fffffffu ? bound : 0x7fffffffu;
   return MFA_SUCCESS;
 }
 // An FP8 K/V request (mfa_fp8_kv_t), after the checks the host can make; the table's and the split's checks come first
@@ -319,23 +320,37 @@ static int fp8_of(const mfa_attention_kernel *k, const mfa_fp8_kv_t *f, Fp8KV *o
   return MFA_SUCCESS;
 }
 
-// The key bound a split plan cuts: the hint, or the table's bound (capped so that block counts cannot overflow)
-static uint32_t key_bound_of(const mfa_split_kv_t &s, const Sequences *seq, const PagedKV *pk) {
-  const uint32_t bound = s.max_column ? s.max_column : (seq ? seq->max_column : pk->max_keys);
-  return bound < 0x7fffffffu ? bound : 0x7fffffffu;
+// The plan of a forward call on the tensor cores, per batch slice (a paged call is one slice), with the kernel's window:
+// f(first problem of the slice, plan)
+template <class F>
+static int forward_plans(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, ForwardCall call,
+                         F f) {
+  const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
+  uint32_t group = 1;
+  const int status = kv_group_of(c, &group);
+  if (status != MFA_SUCCESS) return status;
+  Band band;
+  call.band = band_of(kernel, c->row, call.pk ? call.pk->max_keys : c->column, &band);
+  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, sm_count = device_sm_count(current_device());
+  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t h0, uint32_t batch) -> int {
+    f(h0, wgmma_forward_plan(Dp, c->row, c->column, batch, group, d.split_min_blocks, d.split_max ? d.split_max : 1,
+                             call, sm_count));
+    return MFA_SUCCESS;
+  });
 }
 
-// encode() of problems of the full R x C shape (seq == nullptr) or of packed sequences; split: the split-KV forward
-static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, const Sequences *seq,
-                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, const mfa_split_kv_t *split = nullptr);
-static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
-                      const PagedKV *pk, const mfa_split_kv_t &split, mfa_split_plan_t *out);
-// encode() of a paged cache; split_call: the split-KV entry point, whose request `split` is checked after the table;
-// fp8_call: the FP8 K/V entry point (split optional), whose request `fp8` is checked after both
-static int encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
-                        const mfa_paged_kv_t *table, bool split_call, const mfa_split_kv_t *split,
-                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, bool fp8_call = false,
-                        const mfa_fp8_kv_t *fp8 = nullptr);
+// The first checks of an encode over a sequence table or a paged cache, before the table's
+static int encode_arguments(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
+                            void *const buffers[MFA_BUFFER_COUNT]) {
+  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
+  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
+  return MFA_SUCCESS;
+}
+
+// encode() of any kernel type in the form `call` describes (the backward kernels take call.seq only); the kernel's
+// window is added to the call here
+static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, ForwardCall call,
+                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
 
 }  // namespace mfa
 
@@ -475,39 +490,50 @@ int mfa_attention_kernel_threadgroup_memory_allocation(const mfa_attention_kerne
 }
 
 namespace mfa {
-static int grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
+static int grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const ForwardCall &call,
                      uint32_t *out) {
+  if (kernel->backend == MFA_BACKEND_TCGEN05 && kernel->type == MFA_FORWARD) {
+    *out = 0;  // the CTAs of one key range
+    return forward_plans(kernel, c, call, [&](uint32_t, const WgmmaPlan &plan) {
+      *out += static_cast<uint32_t>(static_cast<uint64_t>(plan.grid.x) * plan.grid.y * plan.grid.z / plan.splits);
+    });
+  }
   // parallelization dimension: R for forward / backwardQuery, C for backwardKeyValue
   // (AttentionKernel.swift:197-204; dispatch: SquareAttentionTest.swift:328-339)
-  // (dK/dV: one CTA per K/V tile, which walks the query problems of its group; packed sequences: the tiles of the
-  // longest sequence, once per sequence)
+  // (dK/dV: one CTA per K/V tile, which walks the query problems of its group; packed sequences and paged calls: the
+  // tiles of the longest sequence, once per sequence)
   const bool key_value = kernel->type == MFA_BACKWARD_KEY_VALUE;
-  const uint32_t dim = key_value ? (seq ? seq->max_column : c->column) : (seq ? seq->max_row : c->row);
+  const Sequences *seq = call.seq;
+  const uint32_t dim = call.pk ? call.pk->max_row
+                               : (key_value ? (seq ? seq->max_column : c->column) : (seq ? seq->max_row : c->row));
+  const uint32_t count = call.pk ? call.pk->count : (seq ? seq->count : 1);
   const uint32_t batch = c->batch_count ? c->batch_count : 1;
   uint32_t group = 1;
   const int status = kv_group_of(c, &group);
   if (status != MFA_SUCCESS) return status;
-  *out = ((dim + kernel->par - 1) / kernel->par) * (key_value ? batch / group : batch) * (seq ? seq->count : 1);
+  *out = ((dim + kernel->par - 1) / kernel->par) * (key_value ? batch / group : batch) * count;
   return MFA_SUCCESS;
 }
 
-static int launch_count(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
-                        uint32_t *out) {
+static int launch_count(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                        const ForwardCall &call, uint32_t *out) {
   const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
   const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, staged = __builtin_popcount(staged_operands(kernel));
+  *out = 0;
+  if (kernel->backend == MFA_BACKEND_TCGEN05 && kernel->type == MFA_FORWARD)
+    return forward_plans(kernel, c, call, [&](uint32_t, const WgmmaPlan &plan) { *out += staged + plan.launches; });
   uint32_t group = 1;
   const int status = kv_group_of(c, &group);
   if (status != MFA_SUCCESS) return status;
   const uint32_t sm_count = kernel->backend == MFA_BACKEND_TCGEN05 ? device_sm_count(current_device()) : 0;
   const bool convert_dO = d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q];
   Band band;
-  *out = 0;
   return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t, uint32_t batch) -> int {
     if (kernel->backend != MFA_BACKEND_TCGEN05)
       *out += 1;
-    else if (seq)
-      *out += staged + wgmma_plan_sequences(kernel->type, Dp, seq->max_row, seq->max_column, seq->count, batch, group,
-                                            convert_dO, sm_count)
+    else if (call.seq)
+      *out += staged + wgmma_plan_sequences(kernel->type, Dp, call.seq->max_row, call.seq->max_column, call.seq->count,
+                                            batch, group, convert_dO, sm_count)
                            .launches;
     else
       *out += staged + wgmma_plan(kernel->type, Dp, c->row, c->column, batch, group, d.split_min_blocks, d.split_max,
@@ -516,20 +542,40 @@ static int launch_count(const mfa_attention_kernel_t *kernel, const mfa_function
     return MFA_SUCCESS;
   });
 }
+
+// The plan of a split-KV call: the forward plan's on the tensor cores, one split on the SIMT family
+static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const ForwardCall &call,
+                      mfa_split_plan_t *out) {
+  *out = mfa_split_plan_t{1, 1, 0, 0};
+  if (kernel->backend != MFA_BACKEND_TCGEN05) {
+    const int status = grid_size(kernel, c, call, &out->grid_size);
+    return status != MFA_SUCCESS ? status : launch_count(kernel, c, call, &out->launch_count);
+  }
+  const uint32_t staged = __builtin_popcount(staged_operands(kernel));
+  return forward_plans(kernel, c, call, [&](uint32_t h0, const WgmmaPlan &plan) {
+    if (h0 == 0) {
+      out->splits = plan.splits;
+      out->heads_per_tile = plan.heads_per_tile;
+    }
+    out->grid_size += plan.grid.x * plan.grid.y * plan.grid.z;
+    out->launch_count += staged + plan.launches;
+  });
+}
 }  // namespace mfa
 
 int mfa_attention_kernel_grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                    uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  return grid_size(kernel, c, nullptr, out);
+  return grid_size(kernel, c, ForwardCall{}, out);
 }
 
 int mfa_attention_kernel_grid_size_sequences(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                              const mfa_sequence_table_t *table, uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   Sequences seq;
+  ForwardCall call{&seq};
   const int status = sequences_of(kernel, c, table, &seq);
-  return status != MFA_SUCCESS ? status : grid_size(kernel, c, &seq, out);
+  return status != MFA_SUCCESS ? status : grid_size(kernel, c, call, out);
 }
 
 const char *mfa_attention_kernel_source_name(const mfa_attention_kernel_t *kernel) {
@@ -539,41 +585,40 @@ const char *mfa_attention_kernel_source_name(const mfa_attention_kernel_t *kerne
 int mfa_attention_kernel_launch_count(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                       uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  return launch_count(kernel, c, nullptr, out);
+  return launch_count(kernel, c, ForwardCall{}, out);
 }
 
 int mfa_attention_kernel_launch_count_sequences(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                                 const mfa_sequence_table_t *table, uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   Sequences seq;
+  ForwardCall call{&seq};
   const int status = sequences_of(kernel, c, table, &seq);
-  return status != MFA_SUCCESS ? status : launch_count(kernel, c, &seq, out);
+  return status != MFA_SUCCESS ? status : launch_count(kernel, c, call, out);
 }
 
 int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
                                 void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  return encode(kernel, constants, nullptr, buffers, cuda_stream);
+  return encode(kernel, constants, ForwardCall{}, buffers, cuda_stream);
 }
 
 int mfa_attention_kernel_grid_size_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                          const mfa_paged_kv_t *table, uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   PagedKV pk;
+  ForwardCall call{nullptr, &pk};
   const int status = paged_of(kernel, c, table, &pk);
-  if (status != MFA_SUCCESS) return status;
-  const Sequences seq = grid_of(pk);
-  return grid_size(kernel, c, &seq, out);
+  return status != MFA_SUCCESS ? status : grid_size(kernel, c, call, out);
 }
 
 int mfa_attention_kernel_launch_count_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                             const mfa_paged_kv_t *table, uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   PagedKV pk;
+  ForwardCall call{nullptr, &pk};
   const int status = paged_of(kernel, c, table, &pk);
-  if (status != MFA_SUCCESS) return status;
-  *out = 1;  // never staged (row-major, head % 8 == 0 on the tensor cores), never split, one batch slice
-  return MFA_SUCCESS;
+  return status != MFA_SUCCESS ? status : launch_count(kernel, c, call, out);
 }
 
 int mfa_attention_kernel_split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
@@ -585,51 +630,71 @@ int mfa_attention_kernel_split_plan(const mfa_attention_kernel_t *kernel, const 
                                                 (sequences ? "both" : "neither") + " given).");
   Sequences seq;
   PagedKV pk;
+  ForwardCall call{sequences ? &seq : nullptr, paged ? &pk : nullptr};
   int status = sequences ? sequences_of(kernel, c, sequences, &seq) : paged_of(kernel, c, paged, &pk);
-  if (status != MFA_SUCCESS || (status = split_of(kernel, split)) != MFA_SUCCESS) return status;
-  return split_plan(kernel, c, sequences ? &seq : nullptr, paged ? &pk : nullptr, *split, out);
+  if (status != MFA_SUCCESS || (status = split_of(kernel, split, &call)) != MFA_SUCCESS) return status;
+  return split_plan(kernel, c, call, out);
 }
 
 int mfa_attention_kernel_encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
                                       const mfa_paged_kv_t *table, void *const buffers[MFA_BUFFER_COUNT],
                                       void *cuda_stream) {
-  return encode_paged(kernel, constants, table, false, nullptr, buffers, cuda_stream);
+  PagedKV pk;
+  ForwardCall call{nullptr, &pk};
+  int status = encode_arguments(kernel, constants, buffers);
+  if (status != MFA_SUCCESS || (status = paged_of(kernel, constants, table, &pk)) != MFA_SUCCESS) return status;
+  return encode(kernel, constants, call, buffers, cuda_stream);
 }
 
 int mfa_attention_kernel_encode_sequences(const mfa_attention_kernel_t *kernel,
                                           const mfa_function_constants_t *constants, const mfa_sequence_table_t *table,
                                           void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
-  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
   Sequences seq;
-  const int status = sequences_of(kernel, constants, table, &seq);
-  return status != MFA_SUCCESS ? status : encode(kernel, constants, &seq, buffers, cuda_stream);
+  ForwardCall call{&seq};
+  int status = encode_arguments(kernel, constants, buffers);
+  if (status != MFA_SUCCESS || (status = sequences_of(kernel, constants, table, &seq)) != MFA_SUCCESS) return status;
+  return encode(kernel, constants, call, buffers, cuda_stream);
 }
 
 int mfa_attention_kernel_encode_paged_split(const mfa_attention_kernel_t *kernel,
                                             const mfa_function_constants_t *constants, const mfa_paged_kv_t *table,
                                             const mfa_split_kv_t *split, void *const buffers[MFA_BUFFER_COUNT],
                                             void *cuda_stream) {
-  return encode_paged(kernel, constants, table, true, split, buffers, cuda_stream);
+  PagedKV pk;
+  ForwardCall call{nullptr, &pk};
+  int status = encode_arguments(kernel, constants, buffers);
+  if (status != MFA_SUCCESS || (status = paged_of(kernel, constants, table, &pk)) != MFA_SUCCESS ||
+      (status = split_of(kernel, split, &call)) != MFA_SUCCESS)
+    return status;
+  return encode(kernel, constants, call, buffers, cuda_stream);
 }
 
 int mfa_attention_kernel_encode_paged_fp8(const mfa_attention_kernel_t *kernel,
                                           const mfa_function_constants_t *constants, const mfa_paged_kv_t *table,
                                           const mfa_split_kv_t *split, const mfa_fp8_kv_t *fp8,
                                           void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
-  return encode_paged(kernel, constants, table, split != nullptr, split, buffers, cuda_stream, true, fp8);
+  PagedKV pk;
+  Fp8KV scales;
+  ForwardCall call{nullptr, &pk, nullptr, &scales};
+  int status = encode_arguments(kernel, constants, buffers);
+  if (status != MFA_SUCCESS || (status = paged_of(kernel, constants, table, &pk)) != MFA_SUCCESS ||
+      (split && (status = split_of(kernel, split, &call)) != MFA_SUCCESS) ||
+      (status = fp8_of(kernel, fp8, &scales)) != MFA_SUCCESS)
+    return status;
+  return encode(kernel, constants, call, buffers, cuda_stream);
 }
 
 int mfa_attention_kernel_encode_sequences_split(const mfa_attention_kernel_t *kernel,
                                                 const mfa_function_constants_t *constants,
                                                 const mfa_sequence_table_t *table, const mfa_split_kv_t *split,
                                                 void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
-  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
   Sequences seq;
-  int status = sequences_of(kernel, constants, table, &seq);
-  if (status != MFA_SUCCESS || (status = split_of(kernel, split)) != MFA_SUCCESS) return status;
-  return encode(kernel, constants, &seq, buffers, cuda_stream, split);
+  ForwardCall call{&seq};
+  int status = encode_arguments(kernel, constants, buffers);
+  if (status != MFA_SUCCESS || (status = sequences_of(kernel, constants, table, &seq)) != MFA_SUCCESS ||
+      (status = split_of(kernel, split, &call)) != MFA_SUCCESS)
+    return status;
+  return encode(kernel, constants, call, buffers, cuda_stream);
 }
 
 int mfa_paged_kv_append(const mfa_paged_kv_t *paged, const mfa_paged_kv_append_t *append, void *k_pool, void *v_pool,
@@ -702,90 +767,18 @@ int mfa_paged_kv_append_rotary(const mfa_paged_kv_t *paged, const mfa_paged_kv_a
 }  // extern "C"
 
 namespace mfa {
-// The plan of a split-KV call over packed sequences (seq) or a paged cache (pk): wgmma_plan_split per batch slice on
-// the tensor cores (a paged call is one slice), one split on the SIMT family
-static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const Sequences *seq,
-                      const PagedKV *pk, const mfa_split_kv_t &split, mfa_split_plan_t *out) {
-  *out = mfa_split_plan_t{1, 1, 0, 0};
-  if (kernel->backend != MFA_BACKEND_TCGEN05) {
-    int status;
-    if (pk) {
-      const Sequences grid = grid_of(*pk);
-      status = grid_size(kernel, c, &grid, &out->grid_size);
-      out->launch_count = 1;
-    } else if ((status = grid_size(kernel, c, seq, &out->grid_size)) == MFA_SUCCESS) {
-      status = launch_count(kernel, c, seq, &out->launch_count);
-    }
-    return status;
-  }
-  const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
-  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, staged = __builtin_popcount(staged_operands(kernel));
-  uint32_t group = 1;
-  const int status = kv_group_of(c, &group);
-  if (status != MFA_SUCCESS) return status;
-  const uint32_t sm_count = device_sm_count(current_device());
-  Band storage;
-  const Band *band = band_of(kernel, c->row, pk ? pk->max_keys : c->column, &storage);
-  const uint32_t key_bound = key_bound_of(split, seq, pk);
-  const uint32_t max_row = pk ? pk->max_row : seq->max_row, count = pk ? pk->count : seq->count;
-  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t h0, uint32_t batch) -> int {
-    const WgmmaPlan plan = wgmma_plan_split(Dp, max_row, key_bound, count, batch, group, d.split_min_blocks,
-                                            d.split_max ? d.split_max : 1, split.num_splits, sm_count, band);
-    if (h0 == 0) {
-      out->splits = plan.splits;
-      out->heads_per_tile = plan.heads_per_tile;
-    }
-    out->grid_size += plan.grid.x * plan.grid.y * plan.grid.z;
-    out->launch_count += (pk ? 0 : staged) + plan.launches;
-    return MFA_SUCCESS;
-  });
-}
-
-static int encode_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
-                        const mfa_paged_kv_t *table, bool split_call, const mfa_split_kv_t *split,
-                        void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, bool fp8_call,
-                        const mfa_fp8_kv_t *fp8) {
-  if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  if (constants->row == 0 || constants->column == 0) return fail(MFA_ERROR_INVALID_ARGUMENT, "R and C must be at least 1.");
-  PagedKV pk;
-  int status = paged_of(kernel, constants, table, &pk);
-  if (status != MFA_SUCCESS) return status;
-  if (split_call && (status = split_of(kernel, split)) != MFA_SUCCESS) return status;
-  Fp8KV scales{};
-  if (fp8_call && (status = fp8_of(kernel, fp8, &scales)) != MFA_SUCCESS) return status;
-  if ((status = check_device()) != MFA_SUCCESS) return status;
-  AttentionParams p;
-  if ((status = build_params(kernel, constants, buffers, p)) != MFA_SUCCESS) return status;
-  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  Band storage;
-  const Band *band = band_of(kernel, p.R, pk.max_keys, &storage);
-  cudaError_t e;
-  if (fp8_call)
-    e = launch_wgmma_forward_paged_fp8(p, pk, band, scales, split != nullptr, split ? split->num_splits : 1,
-                                       split ? key_bound_of(*split, nullptr, &pk) : pk.max_keys, stream);
-  else if (kernel->backend != MFA_BACKEND_TCGEN05)
-    e = launch_simt_forward_paged(p, pk, band, stream);
-  else if (split)
-    e = launch_wgmma_forward_split(p, nullptr, &pk, band, split->num_splits, key_bound_of(*split, nullptr, &pk), stream);
-  else
-    e = launch_wgmma_forward_paged(p, pk, band, stream);
-  if (e != cudaSuccess)
-    return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name +
-                                    (fp8_call ? " (paged FP8 K/V) failed: " : " (paged K/V) failed: ") +
-                                    cudaGetErrorString(e) + " " + last_launch_detail());
-  return MFA_SUCCESS;
-}
-
-static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, const Sequences *seq,
-                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream, const mfa_split_kv_t *split) {
+static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, ForwardCall call,
+                  void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   int status = check_device();
   if (status != MFA_SUCCESS) return status;
   AttentionParams p;
   status = build_params(kernel, constants, buffers, p);
   if (status != MFA_SUCCESS) return status;
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  // (a paged call's keys are bounded by its table)
   Band storage;
-  const Band *band = band_of(kernel, p.R, p.C, &storage);
+  call.band = band_of(kernel, p.R, call.pk ? call.pk->max_keys : p.C, &storage);
+  const Sequences *seq = call.seq;
 
   // Tensor-core family: operands with D % 8 != 0 or a transposed layout are staged row-major with pad8(D) columns, the
   // kernels run at the padded head dimension (the softmax scale stays 1 / sqrt(D) of the true D), and the FP32 outputs
@@ -838,24 +831,21 @@ static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_const
     }
     if (kernel->backend == MFA_BACKEND_TCGEN05) {
       switch (kernel->type) {
-        case MFA_FORWARD:
-          e = split ? launch_wgmma_forward_split(q, seq, nullptr, band, split->num_splits,
-                                                 key_bound_of(*split, seq, nullptr), stream)
-                    : launch_wgmma_forward(q, seq, band, stream);
-          break;
-        case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, seq, band, stream); break;
-        default: e = launch_wgmma_backward_key_value(q, seq, band, stream); break;
+        case MFA_FORWARD: e = launch_wgmma_forward(q, call, stream); break;
+        case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, seq, call.band, stream); break;
+        default: e = launch_wgmma_backward_key_value(q, seq, call.band, stream); break;
       }
     } else {
       switch (kernel->type) {
-        case MFA_FORWARD: e = launch_simt_forward(q, seq, band, stream); break;
-        case MFA_BACKWARD_QUERY: e = launch_simt_backward_query(q, seq, band, stream); break;
-        default: e = launch_simt_backward_key_value(q, seq, band, stream); break;
+        case MFA_FORWARD: e = launch_simt_forward(q, call, stream); break;
+        case MFA_BACKWARD_QUERY: e = launch_simt_backward_query(q, seq, call.band, stream); break;
+        default: e = launch_simt_backward_key_value(q, seq, call.band, stream); break;
       }
     }
     if (e != cudaSuccess)
-      return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name + " failed: " + cudaGetErrorString(e) +
-                                      " " + last_launch_detail());
+      return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name +
+                                      (call.fp8 ? " (paged FP8 K/V)" : (call.pk ? " (paged K/V)" : "")) + " failed: " +
+                                      cudaGetErrorString(e) + " " + last_launch_detail());
     // (packed sequences: only the sequences' rows, which the kernels wrote; the caller's other rows stay as they are)
     for (int slot = 0; slot < kSlots && e == cudaSuccess; ++slot)
       if (user_out[slot] && seq)

@@ -139,41 +139,36 @@ struct RotarySource {
 cudaError_t launch_rotary_kv_append(const PagedKV &pk, const AppendSource &src, const RotarySource &rot, void *k_pool,
                                     void *v_pool, const Fp8KV *fp8, cudaStream_t stream);
 
+// The form of a forward call: fixed-length problems, or packed sequences (seq) or a paged cache (pk); a window; FP8 pools
+// (paged); a split-KV request of a packed or paged call (num_splits 0: the plan's choice; key_bound: every Cs's bound)
+struct ForwardCall {
+  const Sequences *seq = nullptr;
+  const PagedKV *pk = nullptr;
+  const Band *band = nullptr;
+  const Fp8KV *fp8 = nullptr;
+  bool split = false;
+  uint32_t num_splits = 0, key_bound = 0;
+};
+
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
-// seq: packed sequences, or nullptr for problems of the full R x C shape; band: a sliding window, or nullptr
-cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream);
+// The forward of call.seq, call.pk and call.band (a null one: absent), never split; FP8 K/V is not served here
+cudaError_t launch_simt_forward(const AttentionParams &p, const ForwardCall &call, cudaStream_t stream);
+// The backward: seq, packed sequences, or nullptr for problems of the full R x C shape; band, a window, or nullptr
 cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
                                        cudaStream_t stream);
 cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
                                            cudaStream_t stream);
-// paged K/V: the forward only, row-major operands
-cudaError_t launch_simt_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
-                                      cudaStream_t stream);
 void simt_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
                    uint32_t *head);
 
 // ---- tensor-core family (wgmma_attention.cu; the backend keeps its historical name "tcgen05" in the ABI) --------
 // 16-bit row-major operands with D % 8 == 0 and D <= kWgmmaMaxHead; kernel.cpp stages every other layout into that form.
 constexpr uint32_t kWgmmaMaxHead = 256;
-cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream);
+cudaError_t launch_wgmma_forward(const AttentionParams &p, const ForwardCall &call, cudaStream_t stream);
 cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
                                         cudaStream_t stream);
 cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
                                             cudaStream_t stream);
-// paged K/V: the forward only, unsplit, grid (tiles of max_row, batch, count)
-cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
-                                       cudaStream_t stream);
-// split-KV forward of packed sequences (seq) or a paged cache (pk), exactly one non-null: the plan of
-// wgmma_plan_split; one split runs launch_wgmma_forward / launch_wgmma_forward_paged unchanged
-cudaError_t launch_wgmma_forward_split(const AttentionParams &p, const Sequences *seq, const PagedKV *pk,
-                                       const Band *band, uint32_t num_splits, uint32_t key_bound, cudaStream_t stream);
-// paged forward over FP8 E4M3 pools (K and V buffers hold bytes; Q's 16-bit type is what they are converted to): split,
-// the plan of wgmma_plan_split for num_splits / key_bound; unsplit, one split and one head per tile, the grid of
-// launch_wgmma_forward_paged.  Always the split paged kernels' FP8 twins.
-cudaError_t launch_wgmma_forward_paged_fp8(const AttentionParams &p, const PagedKV &pk, const Band *band,
-                                           const Fp8KV &fp8, bool split, uint32_t num_splits, uint32_t key_bound,
-                                           cudaStream_t stream);
-
 // How the launcher of kernel `type` (mfa_kernel_type_t) runs one problem of padded head dimension D; every field is
 // derived from the kernels' compile-time configurations.  R, C and batch do not affect the geometry fields.
 struct WgmmaPlan {
@@ -204,6 +199,10 @@ WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t 
 WgmmaPlan wgmma_plan_split(uint32_t D, uint32_t max_row, uint32_t key_bound, uint32_t count, uint32_t batch,
                            uint32_t group, uint32_t min_blocks, uint32_t max_splits, uint32_t num_splits,
                            uint32_t sm_count, const Band *band);
+// The plan of a forward call, which its launcher and the host's counts follow: wgmma_plan for fixed-length problems,
+// wgmma_plan_split for split calls unless it plans one split and one head per tile, else wgmma_plan_sequences.
+WgmmaPlan wgmma_forward_plan(uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
+                             uint32_t max_splits, const ForwardCall &call, uint32_t sm_count);
 
 // operand staging for the tensor-core family (pad_head.cu): a [batch][seq][D] (or, transposed, [batch][D][seq]) operand
 // is copied to row-major [batch][seq][Dp] with zero padding columns, and an FP32 output computed in that form is copied

@@ -1111,29 +1111,25 @@ static dim3 simt_grid(uint32_t rows, uint32_t y, const Sequences *seq) {
   return dim3((rows + simt::kBlock - 1) / simt::kBlock, y, seq ? seq->count : 1);
 }
 
-cudaError_t launch_simt_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream) {
-  const dim3 grid = simt_grid(seq ? seq->max_row : p.R, p.batch, seq);
+cudaError_t launch_simt_forward(const AttentionParams &p, const ForwardCall &call, cudaStream_t stream) {
+  const Sequences *seq = call.seq;
+  const PagedKV *pk = call.pk;
+  const Band *band = call.band;
+  const uint32_t rows = pk ? pk->max_row : (seq ? seq->max_row : p.R);
+  const dim3 grid((rows + simt::kBlock - 1) / simt::kBlock, p.batch, pk ? pk->count : (seq ? seq->count : 1));
   return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
     constexpr int NCH = decltype(nch)::value;
     using simt::Layout;
+    if (band && pk)
+      return simt::launch(simt::simt_band_forward_kernel<NCH, Layout::kPaged>, grid, stream, p, Sequences{}, *pk, *band);
     if (band && seq)
       return simt::launch(simt::simt_band_forward_kernel<NCH, Layout::kPacked>, grid, stream, p, *seq, PagedKV{}, *band);
     if (band)
       return simt::launch(simt::simt_band_forward_kernel<NCH, Layout::kFixed>, grid, stream, p, Sequences{}, PagedKV{},
                           *band);
+    if (pk) return simt::launch(simt::simt_forward_kernel_paged<NCH>, grid, stream, p, *pk);
     if (seq) return simt::launch(simt::simt_forward_kernel_varlen<NCH>, grid, stream, p, *seq);
     return simt::launch(simt::simt_forward_kernel<NCH>, grid, stream, p);
-  });
-}
-
-cudaError_t launch_simt_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
-                                      cudaStream_t stream) {
-  const dim3 grid((pk.max_row + simt::kBlock - 1) / simt::kBlock, p.batch, pk.count);
-  return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
-    if (band)
-      return simt::launch(simt::simt_band_forward_kernel<decltype(nch)::value, simt::Layout::kPaged>, grid, stream, p,
-                          Sequences{}, pk, *band);
-    return simt::launch(simt::simt_forward_kernel_paged<decltype(nch)::value>, grid, stream, p, pk);
   });
 }
 

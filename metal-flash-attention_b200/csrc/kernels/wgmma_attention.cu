@@ -24,6 +24,9 @@
 // dK/dV grid's y axis is K/V heads, and a CTA walks the query blocks of every query head of its group, so dK and dV
 // are the group sums, accumulated in registers without atomics.
 //
+// Every forward entry point takes the three tensor maps and one FwdArgs (below), whose fields each form reads as it
+// needs; launch_forward picks the entry point of a call's form and fills FwdArgs once.
+//
 // Packed sequences (the packed_* entry points, kVarlen in the shared bodies): grid.z is the sequence; a CTA takes its
 // sequence's rows from the offset tables, leaves when its tile starts past the sequence's end, works on the sequence's
 // R, C and delta, and zeroes the rows of its last streamed block that belong to the next sequence.  Unsplit, except in
@@ -36,7 +39,7 @@
 // each at the pool row of its page; thread 0 reads the block's page ids just before it issues its boxes.
 //
 // Sliding window (the band_* entry points, kBand in the shared bodies; Band in attention_params.h): row i sees key j iff
-// i + delta - left <= j <= i + delta + right, with left and right runtime arguments, so one instantiation serves every
+// i + delta - left <= j <= i + delta + right, with left and right runtime values, so one instantiation serves every
 // window.  A CTA visits only the traversal blocks that meet its rows' (keys') band; only blocks that cross an edge of the
 // band are masked (mask_outside_band, whose edges are 64-bit: a side may be as large as INT32_MAX).  The bodies run with kCausal set, which brings the empty-row handling (reference value 0 for a
 // row without a key yet, L = -inf split partials, merge_splits<true>).  A fixed-length split range counts from the
@@ -566,9 +569,35 @@ __device__ __forceinline__ void convert_fp8_kv(const uint8_t *src, uint8_t *dst,
   }
 }
 
-// The body of the forward kernels.  R, C: the rows of each problem's buffers (paged: C is unused).  kPacked / kPaged:
-// the CTA works on sequence blockIdx.z, whose span replaces R, C and delta in the ranges and masks and offsets every
-// query row, and zeroes the rows of its last key block past the sequence's keys.
+// The arguments of every forward kernel but its tensor maps.  Each kernel reads the fields its form uses:
+//   O, L, l_prec   the outputs (O FP32 [batch][R][D], L [batch][R] in precision l_prec)
+//   R, C, D        the rows of each problem's buffers (paged: C is unused) and the head dimension
+//   delta          fixed-length problems: query row i sees key j iff j <= i + delta (C - R), the window's centre
+//   group          query heads per K/V head
+//   sp             the split of the key range and the workspace of its partials (the unsplit packed and paged kernels
+//                  ignore it: they are never split)
+//   hpt            split packed and paged kernels: query heads per tile
+//   seq, pk        the packed sequences or the paged cache
+//   band           the sliding window of the band_* kernels and their split and FP8 twins
+//   fp8            the scales of FP8 pools
+struct FwdArgs {
+  float *O;
+  void *L;
+  uint32_t R, C, D;
+  float scale_log2;
+  int l_prec, delta;
+  uint32_t group;
+  SplitArgs sp;
+  uint32_t hpt;
+  Sequences seq;
+  PagedKV pk;
+  Band band;
+  Fp8KV fp8;
+};
+
+// The body of the forward kernels.  kPacked / kPaged: the CTA works on sequence blockIdx.z, whose span replaces R, C
+// and delta in the ranges and masks and offsets every query row, and zeroes the rows of its last key block past the
+// sequence's keys.
 // kBand: the sliding window `band` (with kCausal set).
 // kSplit (packed / paged only): blockIdx.x is tile * sp.splits + split; the CTA takes chunk `split` of ceil(n / splits)
 // blocks of the n key blocks its tile sees in its own sequence, and leaves a partial (an empty chunk: O = 0, L = -inf)
@@ -582,13 +611,21 @@ __device__ __forceinline__ void convert_fp8_kv(const uint8_t *src, uint8_t *dst,
 template <uint32_t DCH, bool kBF16, bool kCausal, KVLayout kLayout, bool kBand = false, bool kSplit = false,
           bool kFp8 = false>
 __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUtensorMap &mapK, const CUtensorMap &mapV,
-                                             float *__restrict__ O, void *__restrict__ L, uint32_t R, uint32_t C,
-                                             uint32_t D, float scale_log2, int l_prec, const SplitArgs &sp, int delta,
-                                             uint32_t group, const Sequences &seq, const PagedKV &pk,
-                                             const Band &band = Band{}, uint32_t hpt = 1, const Fp8KV &fp8 = Fp8KV{}) {
+                                             const FwdArgs &a) {
   constexpr bool kVarlen = kLayout != KVLayout::kFixed;
   static_assert(!kSplit || kVarlen, "the fixed-length forward splits through blockIdx.z");
   static_assert(!kFp8 || (kSplit && kLayout == KVLayout::kPaged), "FP8 K/V is a split paged forward");
+  float *__restrict__ O = a.O;
+  void *__restrict__ L = a.L;
+  const uint32_t R = a.R, C = a.C, D = a.D, group = a.group, hpt = a.hpt;
+  const int l_prec = a.l_prec;
+  const Sequences &seq = a.seq;
+  const PagedKV &pk = a.pk;
+  const Band &band = a.band;
+  const Fp8KV &fp8 = a.fp8;
+  const SplitArgs sp = kVarlen && !kSplit ? SplitArgs{0, 1, 0, nullptr, nullptr} : a.sp;
+  float scale_log2 = a.scale_log2;
+  int delta = a.delta;
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -858,68 +895,49 @@ __device__ __forceinline__ void forward_body(const CUtensorMap &mapQ, const CUte
   }
 }
 
+// Fixed-length problems: grid (tiles, heads, splits); each split is one range of blocks_per_split key blocks, and
+// with more than one, merge_splits merges the partials
 template <uint32_t DCH, bool kBF16, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
     attention_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                            const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                            uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp,
-                            int delta, uint32_t group) {
-  forward_body<DCH, kBF16, kCausal, KVLayout::kFixed>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, sp, delta,
-                                                      group, Sequences{}, PagedKV{});
+                            const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kFixed>(mapQ, mapK, mapV, a);
 }
 
 // Packed sequences: grid (tiles of the longest sequence, heads, sequences)
 template <uint32_t DCH, bool kBF16, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
     packed_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                                   const __grid_constant__ CUtensorMap mapV, float *__restrict__ O,
-                                   void *__restrict__ L, uint32_t R, uint32_t C, uint32_t D, float scale_log2,
-                                   int l_prec, uint32_t group, const Sequences seq) {
-  const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
-  forward_body<DCH, kBF16, kCausal, KVLayout::kPacked>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, unsplit, 0,
-                                                       group, seq, PagedKV{});
+                         const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPacked>(mapQ, mapK, mapV, a);
 }
 
 // Paged K/V: grid (tiles of the longest query sequence, heads, sequences); mapK / mapV are page-pool maps
 template <uint32_t DCH, bool kBF16, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
     paged_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                        const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L, uint32_t R,
-                        uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk) {
-  const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
-  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, unsplit, 0,
-                                                      group, Sequences{}, pk);
+                        const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged>(mapQ, mapK, mapV, a);
 }
 
 // Sliding window: the three forward kernels above with a band, causal or not (a causal window is a band with right = 0)
 template <uint32_t DCH, bool kBF16>
 __global__ void __launch_bounds__(2 * kWG, 1)
     band_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                       const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L, uint32_t R,
-                       uint32_t C, uint32_t D, float scale_log2, int l_prec, const SplitArgs sp, int delta,
-                       uint32_t group, const Band band) {
-  forward_body<DCH, kBF16, true, KVLayout::kFixed, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, sp, delta,
-                                                         group, Sequences{}, PagedKV{}, band);
+                       const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, true, KVLayout::kFixed, true>(mapQ, mapK, mapV, a);
 }
 template <uint32_t DCH, bool kBF16>
 __global__ void __launch_bounds__(2 * kWG, 1)
     band_forward_packed_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                              const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                              uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, uint32_t group,
-                              const Sequences seq, const Band band) {
-  const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
-  forward_body<DCH, kBF16, true, KVLayout::kPacked, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, unsplit,
-                                                          0, group, seq, PagedKV{}, band);
+                              const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, true, KVLayout::kPacked, true>(mapQ, mapK, mapV, a);
 }
 template <uint32_t DCH, bool kBF16>
 __global__ void __launch_bounds__(2 * kWG, 1)
     band_forward_paged_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                             const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                             uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk,
-                             const Band band) {
-  const SplitArgs unsplit{0, 1, 0, nullptr, nullptr};
-  forward_body<DCH, kBF16, true, KVLayout::kPaged, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, unsplit, 0,
-                                                         group, Sequences{}, pk, band);
+                             const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, true, KVLayout::kPaged, true>(mapQ, mapK, mapV, a);
 }
 
 // Split-KV packed and paged forwards (kSplit): grid (tiles of the longest query sequence x sp.splits, heads / hpt,
@@ -928,39 +946,28 @@ __global__ void __launch_bounds__(2 * kWG, 1)
 template <uint32_t DCH, bool kBF16, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
     split_forward_packed_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                               const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                               uint32_t R, uint32_t C, uint32_t D, float scale_log2, int l_prec, uint32_t group,
-                               const Sequences seq, const SplitArgs sp, uint32_t hpt) {
-  forward_body<DCH, kBF16, kCausal, KVLayout::kPacked, false, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec,
-                                                                    sp, 0, group, seq, PagedKV{}, Band{}, hpt);
+                               const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPacked, false, true>(mapQ, mapK, mapV, a);
 }
+// (D <= 64, not causal: held to two CTAs per SM, which its 127 registers allowed when its arguments were separate
+// kernel parameters; read from one struct, ptxas would take 131 and one CTA.  It fits 128 without spilling.)
 template <uint32_t DCH, bool kBF16, bool kCausal>
-__global__ void __launch_bounds__(2 * kWG, 1)
+__global__ void __launch_bounds__(2 * kWG, DCH == 1 && !kCausal ? 2 : 1)
     split_forward_paged_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                              const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                              uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk,
-                              const SplitArgs sp, uint32_t hpt) {
-  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged, false, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec,
-                                                                   sp, 0, group, Sequences{}, pk, Band{}, hpt);
+                              const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged, false, true>(mapQ, mapK, mapV, a);
 }
 template <uint32_t DCH, bool kBF16>
 __global__ void __launch_bounds__(2 * kWG, 1)
     split_forward_packed_band_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                                    const __grid_constant__ CUtensorMap mapV, float *__restrict__ O,
-                                    void *__restrict__ L, uint32_t R, uint32_t C, uint32_t D, float scale_log2,
-                                    int l_prec, uint32_t group, const Sequences seq, const Band band,
-                                    const SplitArgs sp, uint32_t hpt) {
-  forward_body<DCH, kBF16, true, KVLayout::kPacked, true, true>(mapQ, mapK, mapV, O, L, R, C, D, scale_log2, l_prec, sp,
-                                                                0, group, seq, PagedKV{}, band, hpt);
+                                    const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, true, KVLayout::kPacked, true, true>(mapQ, mapK, mapV, a);
 }
 template <uint32_t DCH, bool kBF16>
 __global__ void __launch_bounds__(2 * kWG, 1)
     split_forward_paged_band_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                                   const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                                   uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group,
-                                   const PagedKV pk, const Band band, const SplitArgs sp, uint32_t hpt) {
-  forward_body<DCH, kBF16, true, KVLayout::kPaged, true, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, sp, 0,
-                                                               group, Sequences{}, pk, band, hpt);
+                                   const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, true, KVLayout::kPaged, true, true>(mapQ, mapK, mapV, a);
 }
 
 // FP8 K/V: the two split paged forwards above over E4M3 pools with per-K/V-head scales (mapK / mapV: 8-bit page-pool
@@ -968,20 +975,14 @@ __global__ void __launch_bounds__(2 * kWG, 1)
 template <uint32_t DCH, bool kBF16, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
     fp8_kv_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                         const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                         uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk,
-                         const SplitArgs sp, uint32_t hpt, const Fp8KV fp8) {
-  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged, false, true, true>(
-      mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec, sp, 0, group, Sequences{}, pk, Band{}, hpt, fp8);
+                         const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, kCausal, KVLayout::kPaged, false, true, true>(mapQ, mapK, mapV, a);
 }
 template <uint32_t DCH, bool kBF16>
 __global__ void __launch_bounds__(2 * kWG, 1)
     fp8_kv_window_forward_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                                const __grid_constant__ CUtensorMap mapV, float *__restrict__ O, void *__restrict__ L,
-                                uint32_t R, uint32_t D, float scale_log2, int l_prec, uint32_t group, const PagedKV pk,
-                                const Band band, const SplitArgs sp, uint32_t hpt, const Fp8KV fp8) {
-  forward_body<DCH, kBF16, true, KVLayout::kPaged, true, true, true>(mapQ, mapK, mapV, O, L, R, 0, D, scale_log2, l_prec,
-                                                                     sp, 0, group, Sequences{}, pk, band, hpt, fp8);
+                                const __grid_constant__ CUtensorMap mapV, const __grid_constant__ FwdArgs a) {
+  forward_body<DCH, kBF16, true, KVLayout::kPaged, true, true, true>(mapQ, mapK, mapV, a);
 }
 
 // ================================================================================================ backward dQ
@@ -1468,34 +1469,54 @@ static cudaError_t make_maps(const AttentionParams &p, bool with_dO, TensorMaps 
   return make_tensor_map_16bit(&m->V, p.buf[sV], p.C, p.D, kv_heads, Cfg::kKeyBoxRows);
 }
 
+// The forward kernel of a call's form.  Only the forms compiled above are reachable: the split kernels serve packed and
+// paged calls, the FP8 kernels paged ones.
+using ForwardKernel = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const FwdArgs);
 template <uint32_t DCH, bool kBF16, bool kCausal>
-cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, const Sequences *seq, const Band *band,
-                           cudaStream_t stream) {
+static ForwardKernel forward_kernel(KVLayout layout, bool band, bool split, bool fp8) {
+  if (fp8) return band ? fp8_kv_window_forward_wgmma<DCH, kBF16> : fp8_kv_forward_wgmma<DCH, kBF16, kCausal>;
+  if (split && layout == KVLayout::kPaged)
+    return band ? split_forward_paged_band_wgmma<DCH, kBF16> : split_forward_paged_wgmma<DCH, kBF16, kCausal>;
+  if (split) return band ? split_forward_packed_band_wgmma<DCH, kBF16> : split_forward_packed_wgmma<DCH, kBF16, kCausal>;
+  if (layout == KVLayout::kPaged) return band ? band_forward_paged_wgmma<DCH, kBF16> : paged_forward_wgmma<DCH, kBF16, kCausal>;
+  if (layout == KVLayout::kPacked)
+    return band ? band_forward_packed_wgmma<DCH, kBF16> : packed_forward_wgmma<DCH, kBF16, kCausal>;
+  return band ? band_forward_wgmma<DCH, kBF16> : attention_forward_wgmma<DCH, kBF16, kCausal>;
+}
+
+// A forward call of the form `call` on the grid of `plan`.  Q is read in boxes of kTileM / heads_per_tile rows x
+// heads_per_tile heads; K and V as problems of C rows in boxes of BN rows, or (paged) as page pools of C rows, 16-bit
+// or FP8, in boxes of min(P, BN) rows.  A packed or paged call runs the split kernels unless the plan has one split and
+// one head per tile (FP8: always).  With more than one split the kernel writes partials [split][head][row] into the
+// workspace, and merge_splits (fixed) or merge_sequence_splits (packed, paged) merges them into O and L.
+template <uint32_t DCH, bool kBF16, bool kCausal>
+static cudaError_t launch_forward(const AttentionParams &p, const ForwardCall &call, const WgmmaPlan &plan,
+                                  cudaStream_t stream) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
-  auto kernel = attention_forward_wgmma<DCH, kBF16, kCausal>;
-  TensorMaps m;
+  const KVLayout layout = call.pk ? KVLayout::kPaged : (call.seq ? KVLayout::kPacked : KVLayout::kFixed);
+  const bool split = layout != KVLayout::kFixed && (call.fp8 || plan.splits > 1 || plan.heads_per_tile > 1);
+  const ForwardKernel kernel = forward_kernel<DCH, kBF16, kCausal>(layout, call.band, split, call.fp8);
+  const uint32_t hpt = plan.heads_per_tile;
+  FwdArgs a{static_cast<float *>(p.buf[sO]), p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL], p.causal_offset,
+            p.group, SplitArgs{plan.blocks_per_split, plan.splits, p.batch, nullptr, nullptr}, hpt,
+            call.seq ? *call.seq : Sequences{}, call.pk ? *call.pk : PagedKV{}, call.band ? *call.band : Band{},
+            call.fp8 ? *call.fp8 : Fp8KV{}};
+  CUtensorMap mapQ, mapK, mapV;
   cudaError_t e;
-  if (seq && band) {
-    auto packed = band_forward_packed_wgmma<DCH, kBF16>;
-    if ((e = prepare(packed, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess) return e;
-    packed<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]),
-                                                             p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL],
-                                                             p.group, *seq, *band);
-    return cudaGetLastError();
-  }
-  if (seq) {  // packed sequences: unsplit
-    auto packed = packed_forward_wgmma<DCH, kBF16, kCausal>;
-    if ((e = prepare(packed, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess) return e;
-    packed<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]),
-                                                             p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL],
-                                                             p.group, *seq);
-    return cudaGetLastError();
-  }
-  if ((e = (band ? prepare(band_forward_wgmma<DCH, kBF16>, kSmemBytes) : prepare(kernel, kSmemBytes))) != cudaSuccess ||
-      (e = make_maps<Cfg>(p, false, &m)) != cudaSuccess)
+  if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess ||
+      (e = make_tensor_map_16bit(&mapQ, p.buf[sQ], p.R, p.D, p.batch, Cfg::kTileM / hpt, hpt)) != cudaSuccess)
     return e;
-  SplitArgs sp{plan.blocks_per_split, plan.splits, p.batch, nullptr, nullptr};
+  if (call.pk) {
+    const uint32_t box = min(1u << call.pk->page_shift, Cfg::BN);
+    auto pool = call.fp8 ? make_tensor_map_page_pool_8bit : make_tensor_map_page_pool;
+    if ((e = pool(&mapK, p.buf[sK], p.C, call.pk->kv_heads, p.D, box)) != cudaSuccess ||
+        (e = pool(&mapV, p.buf[sV], p.C, call.pk->kv_heads, p.D, box)) != cudaSuccess)
+      return e;
+  } else if ((e = make_tensor_map_16bit(&mapK, p.buf[sK], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess ||
+             (e = make_tensor_map_16bit(&mapV, p.buf[sV], p.C, p.D, p.batch / p.group, Cfg::BN)) != cudaSuccess) {
+    return e;
+  }
   const uint64_t rows_total = static_cast<uint64_t>(p.batch) * p.R;
   if (plan.splits > 1) {
     void *ws = nullptr;
@@ -1503,111 +1524,21 @@ cudaError_t launch_forward(const AttentionParams &p, const WgmmaPlan &plan, cons
     if ((e = workspace_for(current_device(), stream, (o_elems + plan.splits * rows_total) * sizeof(float), &ws)) !=
         cudaSuccess)
       return e;
-    sp.O_part = static_cast<float *>(ws);
-    sp.L_part = sp.O_part + o_elems;
+    a.sp.O_part = static_cast<float *>(ws);
+    a.sp.L_part = a.sp.O_part + o_elems;
   }
-  if (band)
-    band_forward_wgmma<DCH, kBF16><<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(
-        m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL], p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp,
-        p.causal_offset, p.group, *band);
-  else
-    kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL],
-                                                             p.R, p.C, p.D, p.scale_log2, p.prec[sL], sp,
-                                                             p.causal_offset, p.group);
+  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(mapQ, mapK, mapV, a);
   if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
-  const uint64_t threads = rows_total * (p.D / 4);
-  // (a window can leave a row without a key in a split, or in every split, as causal does)
-  auto merge = band ? merge_splits<true> : merge_splits<kCausal>;
-  merge<<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(sp, static_cast<float *>(p.buf[sO]), p.buf[sL],
-                                                                          p.prec[sL], rows_total, p.D);
-  return cudaGetLastError();
-}
-
-// Paged K/V: Q in the usual map, K and V as page pools of p.C rows, boxes of min(P, BN) rows
-template <uint32_t DCH, bool kBF16, bool kCausal>
-cudaError_t launch_forward_paged(const AttentionParams &p, const WgmmaPlan &plan, const PagedKV &pk, const Band *band,
-                                 cudaStream_t stream) {
-  using Cfg = FwdCfg<DCH>;
-  constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
-  auto kernel = paged_forward_wgmma<DCH, kBF16, kCausal>;
-  const uint32_t box = min(1u << pk.page_shift, Cfg::BN);
-  TensorMaps m;
-  cudaError_t e;
-  if ((e = (band ? prepare(band_forward_paged_wgmma<DCH, kBF16>, kSmemBytes) : prepare(kernel, kSmemBytes))) !=
-          cudaSuccess ||
-      (e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, Cfg::kQueryBoxRows)) != cudaSuccess ||
-      (e = make_tensor_map_page_pool(&m.K, p.buf[sK], p.C, pk.kv_heads, p.D, box)) != cudaSuccess ||
-      (e = make_tensor_map_page_pool(&m.V, p.buf[sV], p.C, pk.kv_heads, p.D, box)) != cudaSuccess)
-    return e;
-  if (band)
-    band_forward_paged_wgmma<DCH, kBF16><<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(
-        m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL], p.R, p.D, p.scale_log2, p.prec[sL], p.group, pk,
-        *band);
-  else
-    kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, static_cast<float *>(p.buf[sO]), p.buf[sL],
-                                                             p.R, p.D, p.scale_log2, p.prec[sL], p.group, pk);
-  return cudaGetLastError();
-}
-
-// Split-KV packed (seq) or paged (pk) forward of plan.splits key ranges and plan.heads_per_tile query heads per tile
-// (not both 1): with splits > 1 the split kernel writes partials [split][head][row] into the workspace and
-// merge_sequence_splits merges each sequence's rows into O and L; with one split it writes O and L itself.  Q is read in
-// boxes of m = kTileM / heads_per_tile rows x heads_per_tile heads.  fp8 (paged only): the pools hold E4M3 bytes, read
-// through 8-bit maps by the FP8 twins of the paged kernels.
-template <uint32_t DCH, bool kBF16, bool kCausal>
-cudaError_t launch_forward_split(const AttentionParams &p, const WgmmaPlan &plan, const Sequences *seq,
-                                 const PagedKV *pk, const Band *band, cudaStream_t stream, const Fp8KV *fp8 = nullptr) {
-  using Cfg = FwdCfg<DCH>;
-  constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
-  TensorMaps m;
-  cudaError_t e;
-  const uint32_t hpt = plan.heads_per_tile, box_rows = Cfg::kTileM / hpt;
-  if (pk) {
-    const uint32_t box = min(1u << pk->page_shift, Cfg::BN);
-    auto pool = fp8 ? make_tensor_map_page_pool_8bit : make_tensor_map_page_pool;
-    if ((e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, box_rows, hpt)) != cudaSuccess ||
-        (e = pool(&m.K, p.buf[sK], p.C, pk->kv_heads, p.D, box)) != cudaSuccess ||
-        (e = pool(&m.V, p.buf[sV], p.C, pk->kv_heads, p.D, box)) != cudaSuccess)
-      return e;
-  } else if ((e = make_maps<Cfg>(p, false, &m)) != cudaSuccess ||
-             (e = make_tensor_map_16bit(&m.Q, p.buf[sQ], p.R, p.D, p.batch, box_rows, hpt)) != cudaSuccess) {
-    return e;
+  if (layout == KVLayout::kFixed) {
+    const uint64_t threads = rows_total * (p.D / 4);
+    // (a window can leave a row without a key in a split, or in every split, as causal does)
+    auto merge = call.band ? merge_splits<true> : merge_splits<kCausal>;
+    merge<<<static_cast<uint32_t>((threads + 127) / 128), 128, 0, stream>>>(a.sp, a.O, a.L, a.l_prec, rows_total, p.D);
+  } else {
+    const uint64_t threads = static_cast<uint64_t>(call.pk ? call.pk->max_row : call.seq->max_row) * (p.D / 4);
+    merge_sequence_splits<<<dim3(static_cast<uint32_t>((threads + 127) / 128), p.batch, plan.grid.z), 128, 0, stream>>>(
+        a.sp, a.O, a.L, a.l_prec, p.R, p.D, call.pk ? call.pk->row_offsets : call.seq->row_offsets);
   }
-  SplitArgs sp{0, plan.splits, p.batch, nullptr, nullptr};
-  const uint64_t rows_total = static_cast<uint64_t>(p.batch) * p.R;
-  const size_t o_elems = plan.splits * rows_total * p.D;
-  if (plan.splits > 1) {
-    void *ws = nullptr;
-    if ((e = workspace_for(current_device(), stream, (o_elems + plan.splits * rows_total) * sizeof(float), &ws)) !=
-        cudaSuccess)
-      return e;
-    sp.O_part = static_cast<float *>(ws);
-    sp.L_part = sp.O_part + o_elems;
-  }
-  float *O = static_cast<float *>(p.buf[sO]);
-  const int l_prec = p.prec[sL];
-  auto run = [&](auto kernel, const auto &...args) {
-    if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess) return e;
-    kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.K, m.V, O, p.buf[sL], args...);
-    return cudaGetLastError();
-  };
-  if (fp8 && band)
-    e = run(fp8_kv_window_forward_wgmma<DCH, kBF16>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, *band, sp, hpt, *fp8);
-  else if (fp8)
-    e = run(fp8_kv_forward_wgmma<DCH, kBF16, kCausal>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, sp, hpt, *fp8);
-  else if (pk && band)
-    e = run(split_forward_paged_band_wgmma<DCH, kBF16>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, *band, sp, hpt);
-  else if (pk)
-    e = run(split_forward_paged_wgmma<DCH, kBF16, kCausal>, p.R, p.D, p.scale_log2, l_prec, p.group, *pk, sp, hpt);
-  else if (band)
-    e = run(split_forward_packed_band_wgmma<DCH, kBF16>, p.R, p.C, p.D, p.scale_log2, l_prec, p.group, *seq, *band, sp, hpt);
-  else
-    e = run(split_forward_packed_wgmma<DCH, kBF16, kCausal>, p.R, p.C, p.D, p.scale_log2, l_prec, p.group, *seq, sp, hpt);
-  if (e != cudaSuccess || plan.splits == 1) return e;
-  const uint32_t max_row = pk ? pk->max_row : seq->max_row;
-  const uint64_t threads = static_cast<uint64_t>(max_row) * (p.D / 4);
-  merge_sequence_splits<<<dim3(static_cast<uint32_t>((threads + 127) / 128), p.batch, plan.grid.z), 128, 0, stream>>>(
-      sp, O, p.buf[sL], l_prec, p.R, p.D, pk ? pk->row_offsets : seq->row_offsets);
   return cudaGetLastError();
 }
 
@@ -1767,6 +1698,22 @@ WgmmaPlan wgmma_plan_split(uint32_t D, uint32_t max_row, uint32_t key_bound, uin
   return p;
 }
 
+WgmmaPlan wgmma_forward_plan(uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
+                             uint32_t max_splits, const ForwardCall &call, uint32_t sm_count) {
+  if (!call.seq && !call.pk)
+    return wgmma_plan(MFA_FORWARD, D, R, C, batch, group, min_blocks, max_splits, false, sm_count, call.band);
+  const uint32_t max_row = call.pk ? call.pk->max_row : call.seq->max_row;
+  const uint32_t count = call.pk ? call.pk->count : call.seq->count;
+  if (call.split) {
+    const WgmmaPlan p = wgmma_plan_split(D, max_row, call.key_bound, count, batch, group, min_blocks, max_splits,
+                                         call.num_splits, sm_count, call.band);
+    if (p.splits > 1 || p.heads_per_tile > 1) return p;
+  }
+  // (a paged call's key axis does not enter the grid)
+  return wgmma_plan_sequences(MFA_FORWARD, D, max_row, call.pk ? 1 : call.seq->max_column, count, batch, group, false,
+                              sm_count);
+}
+
 static bool row_major_16bit(const AttentionParams &p) {
   for (int s = 0; s < kSlots; ++s)
     if (p.transposed[s]) return false;
@@ -1783,69 +1730,17 @@ static WgmmaPlan plan_for(int type, const AttentionParams &p, const Sequences *s
   return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, convert_dO, sm_count, band);
 }
 
-cudaError_t launch_wgmma_forward(const AttentionParams &p, const Sequences *seq, const Band *band, cudaStream_t stream) {
-  if (!row_major_16bit(p) || p.prec[sO] != FP32) {
-    set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
+cudaError_t launch_wgmma_forward(const AttentionParams &p, const ForwardCall &call, cudaStream_t stream) {
+  if (!row_major_16bit(p) || p.prec[sO] != FP32 || (call.fp8 && p.D % 16 != 0)) {
+    set_launch_detail(call.fp8 ? "descriptor is outside the FP8 K/V forward kernels' domain"
+                               : "descriptor is outside the wgmma forward kernel's domain");
     return cudaErrorInvalidValue;
   }
-  const WgmmaPlan plan = plan_for(MFA_FORWARD, p, seq, band, false);
+  const WgmmaPlan plan = wgmma_forward_plan(p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, call,
+                                            device_sm_count(current_device()));
   return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
-    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, seq, band,
+    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, call, plan,
                                                                                                       stream);
-  });
-}
-
-cudaError_t launch_wgmma_forward_paged(const AttentionParams &p, const PagedKV &pk, const Band *band,
-                                       cudaStream_t stream) {
-  if (!row_major_16bit(p) || p.prec[sO] != FP32) {
-    set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
-    return cudaErrorInvalidValue;
-  }
-  // (the plan of a packed call whose longest sequence has max_row queries: the key axis does not enter the grid)
-  const WgmmaPlan plan = wgmma_plan_sequences(MFA_FORWARD, p.D, pk.max_row, 1, pk.count, p.batch, p.group, false,
-                                              device_sm_count(current_device()));
-  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
-    return hop::launch_forward_paged<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, pk,
-                                                                                                            band, stream);
-  });
-}
-
-cudaError_t launch_wgmma_forward_split(const AttentionParams &p, const Sequences *seq, const PagedKV *pk,
-                                       const Band *band, uint32_t num_splits, uint32_t key_bound, cudaStream_t stream) {
-  const WgmmaPlan plan = wgmma_plan_split(p.D, pk ? pk->max_row : seq->max_row, key_bound, pk ? pk->count : seq->count,
-                                          p.batch, p.group, p.split_min_blocks, p.split_max, num_splits,
-                                          device_sm_count(current_device()), band);
-  if (plan.splits == 1 && plan.heads_per_tile == 1)
-    return pk ? launch_wgmma_forward_paged(p, *pk, band, stream) : launch_wgmma_forward(p, seq, band, stream);
-  if (!row_major_16bit(p) || p.prec[sO] != FP32) {
-    set_launch_detail("descriptor is outside the wgmma forward kernel's domain");
-    return cudaErrorInvalidValue;
-  }
-  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
-    return hop::launch_forward_split<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, plan, seq, pk,
-                                                                                                            band, stream);
-  });
-}
-
-cudaError_t launch_wgmma_forward_paged_fp8(const AttentionParams &p, const PagedKV &pk, const Band *band,
-                                           const Fp8KV &fp8, bool split, uint32_t num_splits, uint32_t key_bound,
-                                           cudaStream_t stream) {
-  bool transposed = false;
-  for (int s = 0; s < kSlots; ++s) transposed = transposed || p.transposed[s];
-  if ((p.prec[sQ] != FP16 && p.prec[sQ] != BF16) || p.prec[sO] != FP32 || transposed || p.D % 16 != 0 ||
-      p.D > kWgmmaMaxHead) {
-    set_launch_detail("descriptor is outside the FP8 K/V forward kernels' domain");
-    return cudaErrorInvalidValue;
-  }
-  WgmmaPlan plan = wgmma_plan_split(p.D, pk.max_row, key_bound, pk.count, p.batch, p.group, p.split_min_blocks,
-                                    p.split_max, split ? num_splits : 1, device_sm_count(current_device()), band);
-  if (!split) {  // one split, one head per tile: the grid of the unsplit paged call
-    plan.heads_per_tile = 1;
-    plan.grid = dim3((pk.max_row + plan.par - 1) / plan.par, p.batch, pk.count);
-  }
-  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
-    return hop::launch_forward_split<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(
-        p, plan, nullptr, &pk, band, stream, &fp8);
   });
 }
 

@@ -5,7 +5,8 @@
 
 Both trees compile the kernel sources in SOURCES through the library's Makefile, with the build's flags, into
 temporary directories; nothing in the repository is written.  A source the base does not have is compiled from the
-working tree alone and its functions are listed as new.  Functions are matched by mangled name.  The script
+working tree alone and its functions are listed as new.  Functions are matched by their demangled name without the
+parameter list (cu++filt), so that a kernel whose arguments moved into a struct is still compared with itself.  The script
 prints every function whose SASS is not byte-identical, with its instruction count before and after, and fails (exit
 status 1) when a function appears or disappears, or when anything ptxas -v reports differs from the base: a function's
 registers, barriers, shared and constant memory, stack frame, spills or diagnostics (counted by code), or the
@@ -22,6 +23,7 @@ CSRC = os.path.join("metal-flash-attention_b200", "csrc")
 SOURCES = ("kernels/wgmma_attention.cu", "kernels/simt_attention.cu", "kernels/paged_append.cu",
            "kernels/rotary_append.cu")
 CUOBJDUMP = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "cuobjdump")
+CUFILT = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "cu++filt")
 
 
 def compile_tree(tree, out):
@@ -38,8 +40,30 @@ def anonymous(text):
     return re.sub(r"_GLOBAL__N__[0-9a-f]+_", "_GLOBAL__N__", text)
 
 
+def without_parameters(demangled):
+    """a demangled function name without its trailing parameter list"""
+    if not demangled.endswith(")"):
+        return demangled
+    depth = 0
+    for i in range(len(demangled) - 1, -1, -1):
+        depth += {")": 1, "(": -1}.get(demangled[i], 0)
+        if depth == 0:
+            return demangled[:i]
+    return demangled
+
+
+def keys(names):
+    """{mangled name: the key a function is matched by}; fails if two functions of one file share a key"""
+    names = sorted(set(names))
+    out = subprocess.run([CUFILT], input="\n".join(names) + "\n", capture_output=True, text=True, check=True).stdout
+    key = {name: without_parameters(d) for name, d in zip(names, out.splitlines())}
+    if len(set(key.values())) != len(key):
+        sys.exit("sass_diff: two functions share a name without their parameter lists")
+    return key
+
+
 def sass(obj):
-    """{function: SASS text} of an object file"""
+    """{function key: SASS text} of an object file"""
     text = anonymous(subprocess.check_output([CUOBJDUMP, "-sass", obj], text=True))
     funcs, name = {}, None
     for line in text.splitlines():
@@ -49,7 +73,8 @@ def sass(obj):
             funcs[name] = []
         elif name is not None:
             funcs[name].append(line)
-    return {name: "\n".join(lines) for name, lines in funcs.items()}
+    key = keys(funcs)
+    return {key[name]: "\n".join(lines) for name, lines in funcs.items()}
 
 
 def instructions(text):
@@ -57,7 +82,7 @@ def instructions(text):
 
 
 def ptxas_report(log):
-    """{function: what ptxas -v reported for it} -- its resource line (registers, barriers, smem, cmem), its stack and
+    """{function key: what ptxas -v reported for it} -- its resource line (registers, barriers, smem, cmem), its stack and
     spill line, and how many diagnostics of each code it drew (without their PTX line numbers, which move with any
     source edit).  Key None holds the lines that belong to no function, such as the gmem total."""
     report, name = {None: {}}, None
@@ -78,7 +103,8 @@ def ptxas_report(log):
                 report[name]["stack and spills"] = text
             elif text and not text.startswith("Compile time"):
                 report[None][text] = report[None].get(text, 0) + 1
-    return report
+    key = keys(name for name in report if name is not None)
+    return {key.get(name): entry for name, entry in report.items()}
 
 
 def main():
