@@ -13,12 +13,16 @@
 //   backward dK/dV  loopBackwardKeyValue  AttentionKernel+Source.swift:244-293
 // Numerical conventions: log2-domain running max m, L = m + log2(l),
 // D stored pre-scaled by 1/sqrt(D), BF16 stores truncate, edge columns masked before softmax.
-// Causal (p.causal): row r sees column c iff c <= r + p.causal_offset; the loops skip the 64-blocks no row of the CTA
-// can see, the mask is applied with the edge mask, and a row that sees no column gets O = 0, L = +inf.
+// One body per kernel type (forward_body, backward_query_body, backward_key_value_body) serves every call form: the
+// call's layout (fixed-length, packed sequences, a paged K/V cache) and its mask (causal or none, or a sliding window)
+// are template parameters, and each __global__ entry point fixes both.
+// Causal (p.causal): row r sees column c iff c <= r + offset (C - R, or Cs - Rs of a sequence); the loops skip the
+// 64-blocks no row of the CTA can see, the mask is applied with the edge mask, and a row that sees no column gets
+// O = 0, L = +inf.
 // Grouped K/V (p.group query problems per K/V problem): query problem b reads K / V problem b / p.group, and a dK/dV
 // CTA sums over the rows of every query problem of its group.
-// Sliding window (Band, the simt_band_* kernels at the end): row r sees column c iff
-// r + delta - left <= c <= r + delta + right; the loops visit only the 64-blocks that meet the CTA's band.
+// Sliding window (Band, the simt_band_* kernels): row r sees column c iff r + offset - left <= c <= r + offset + right;
+// the loops visit only the 64-blocks that meet the CTA's band.
 //
 // Tiling: one CTA = 256 threads = a 64 x 64 block of the attention matrix; thread (tx, ty) owns
 // the 4 x 4 patch {rows ty+16i} x {cols tx+16j}.  Operands are staged through shared memory as
@@ -105,30 +109,37 @@ __device__ __forceinline__ void load_tile(float *dst, const Operand &op, uint32_
   }
 }
 
-// Paged K/V (simt_forward_kernel_paged): the keys of one sequence and K/V head in a pool [pages][P][heads][D], row-major;
-// key s is pool row paged_row(s) (the page id clamped into [0, pages)), rows at or past seq read as zero
+// Paged K/V (the paged forward): the keys of one sequence and K/V head in a pool [pages][P][kv_heads][D], row-major;
+// key s is pool row paged_row(s), and keys at or past seq read as zero.  Under a window (kBand) keys below `first`
+// read as zero too, without touching their page-table entries or pages (DESIGN "Paged page skipping").
+template <bool kBand>
 struct PagedOperand {
   const void *ptr;
   const int32_t *table;  // the sequence's page_table row
-  uint32_t seq;          // Cs
-  uint32_t D, heads, head;
-  uint32_t pages, page_shift;
+  PagedKV pk;            // pages, page_shift, kv_heads
+  uint32_t seq;          // Cs, or under a window the end of the keys the tile's band meets
+  uint32_t D, head;
   int prec;
 };
+template <>
+struct PagedOperand<true> : PagedOperand<false> {
+  uint32_t first;
+};
 
-template <int COLS, int LD>
-__device__ __forceinline__ void load_tile(float *dst, const PagedOperand &op, uint32_t s0, uint32_t d0, uint32_t dEnd,
-                                          int tid) {
+template <int COLS, int LD, bool kBand>
+__device__ __forceinline__ void load_tile(float *dst, const PagedOperand<kBand> &op, uint32_t s0, uint32_t d0,
+                                          uint32_t dEnd, int tid) {
   constexpr int kElems = kBlock * COLS;
 #pragma unroll 4
   for (int e = tid; e < kElems; e += kThreads) {
     const int s = e / COLS, d = e % COLS;
     const uint32_t gs = s0 + s, gd = d0 + d;
+    bool read = gs < op.seq && gd < dEnd;
+    if constexpr (kBand) read = read && gs >= op.first;
     float v = 0.f;
-    if (gs < op.seq && gd < dEnd) {
-      const int page = min(max(__ldg(op.table + (gs >> op.page_shift)), 0), static_cast<int>(op.pages) - 1);
-      const size_t row = (static_cast<size_t>(page) << op.page_shift) | (gs & ((1u << op.page_shift) - 1));
-      v = load_elem(op.ptr, (row * op.heads + op.head) * op.D + gd, op.prec);
+    if (read) {
+      const size_t row = paged_row(op.pk, op.table, gs);
+      v = load_elem(op.ptr, (row * op.pk.kv_heads + op.head) * op.D + gd, op.prec);
     }
     dst[s * LD + d] = v;
   }
@@ -217,18 +228,6 @@ __device__ __forceinline__ float row_sum16(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 8);
   return v;
 }
-
-// Causal: end of the columns the rows [r0, r0 + 64) can see (all C when not causal)
-__device__ __forceinline__ uint32_t visible_columns(const AttentionParams &p, uint32_t r0) {
-  if (!p.causal) return p.C;
-  const int last = static_cast<int>(min(r0 + kBlock, p.R)) - 1 + p.causal_offset;  // last column of the last row
-  return last < 0 ? 0u : min(p.C, static_cast<uint32_t>(last) + 1);
-}
-// masked: column c is past the edge, or past the diagonal of row r
-__device__ __forceinline__ bool masked(const AttentionParams &p, uint32_t r, uint32_t c) {
-  return c >= p.C || (p.causal && static_cast<int>(c) > static_cast<int>(r) + p.causal_offset);
-}
-
 __device__ __forceinline__ Operand make_operand(const AttentionParams &p, int slot, uint32_t seq, uint32_t b) {
   Operand op;
   size_t bytes = static_cast<size_t>(seq) * p.D * (p.prec[slot] == FP32 ? 4 : 2);
@@ -245,263 +244,33 @@ __device__ __forceinline__ char *stat_row(const AttentionParams &p, int slot, ui
   return static_cast<char *>(p.buf[slot]) + static_cast<size_t>(b) * p.R * (p.prec[slot] == FP32 ? 4 : 2);
 }
 
-// store a [64 x (NCH*64)] register accumulator block to a matrix operand (FP32/FP16/BF16, maybe transposed)
-template <int NCH>
-__device__ __forceinline__ void store_acc(const float (&acc)[NCH][4][4], const float (&rowScale)[4],
-                                          const AttentionParams &p, int slot, uint32_t seq, uint32_t b, uint32_t s0,
-                                          uint32_t dlo, uint32_t dhi, int tx, int ty) {
-  Operand op = make_operand(p, slot, seq, b);
-  void *dst = const_cast<void *>(op.ptr);
-#pragma unroll
-  for (int q = 0; q < NCH; ++q)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      uint32_t s = s0 + ty + 16 * i;
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        uint32_t d = dlo + q * kBlock + 4 * tx + jj;
-        if (s < seq && d < dhi) store_elem(dst, elem_index(op, s, d), op.prec, acc[q][i][jj] * rowScale[i]);
-      }
-    }
-}
-
 // ------------------------------------------------------------------------------------------------
-// forward: O = softmax(Q K^T / sqrt(D)) V,  L = log2(e) * logsumexp          (one CTA per 64 rows)
+// Call forms (Layout).  A CTA works on a span: the whole R x C problem (kFixed, with the causal offset C - R that
+// p.causal_offset holds), or sequence blockIdx.z of a packed (kPacked) or paged (kPaged) call, with its offset Cs - Rs.
+// Rows past a span's end read as zeros (Operand::seq).  A fixed span starts at row 0 and covers the whole operand, so
+// transposed fixed-length operands keep their leading dimension; packed operands are row-major (a transposed operand's
+// leading dimension is the whole buffer, which Operand does not carry; kernel.cpp rejects them).
 // ------------------------------------------------------------------------------------------------
-// (packed sequences: simt_forward_kernel_varlen, below, is this kernel's twin, and simt_forward_kernel_paged theirs)
-template <int NCH>
-__global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const AttentionParams p) {
-  extern __shared__ __align__(16) float smem[];
-  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
+enum class Layout { kFixed, kPacked, kPaged };
 
-  const Operand Q = make_operand(p, sQ, p.R, b), K = make_operand(p, sK, p.C, b / p.group),
-                V = make_operand(p, sV, p.C, b / p.group);
-
-  // m = -FLT_MAX, l = denorm_min  (AttentionKernel+Caching.swift:310-311)
-  float m[4], l[4];
-  float acc[NCH][4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    m[i] = -FLT_MAX;
-    l[i] = FLT_TRUE_MIN;
-  }
-#pragma unroll
-  for (int q = 0; q < NCH; ++q)
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] = 0.f;
-
-  const uint32_t cend = visible_columns(p, r0);
-  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
-    float s[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
-
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      // edge (and causal) mask (AttentionKernel+Softmax.swift:228-260), then online max / correction / sum (:267-324)
-      float mx = -FLT_MAX;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (masked(p, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
-        mx = fmaxf(mx, s[i][j]);
-      }
-      mx = row_max16(mx);
-      float m_new = fmaxf(m[i], mx * p.scale_log2);
-      float correction = exp2f(m[i] - m_new);
-      float sum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float pv = exp2f(fmaf(s[i][j], p.scale_log2, -m_new));
-        sum += pv;
-        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv;
-      }
-      sum = row_sum16(sum);
-      l[i] = fmaf(l[i], correction, sum);
-      m[i] = m_new;
-#pragma unroll
-      for (int q = 0; q < NCH; ++q)
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] *= correction;
-    }
-    // (the __syncthreads inside accumulate() orders the sP writes before its reads)
-    accumulate<NCH>(acc, sP, V, c0, 0, p.D, sX, tid, tx, ty);
-  }
-
-  // O *= 1/l on the last iteration (AttentionKernel+Source.swift:169-171); L = m + log2(l) (+Caching.swift:373-377)
-  // causal: a row that sees no column (r + offset < 0) gets O = 0 and L = +inf
-  float inv[4];
-  bool empty[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    empty[i] = p.causal && static_cast<int>(r0 + ty + 16 * i) + p.causal_offset < 0;
-    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
-  }
-  store_acc<NCH>(acc, inv, p, sO, p.R, b, r0, 0, p.D, tx, ty);
-  if (tx == 0 && p.buf[sL] != nullptr) {
-    char *Lbase = stat_row(p, sL, b);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      uint32_t r = r0 + ty + 16 * i;
-      if (r < p.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// backward dQ: D = rowsum(dO * O)/sqrt(D);  dQ = sum_c P (dP/sqrt(D) - D) K     (one CTA per 64 rows)
-// ------------------------------------------------------------------------------------------------
-// (packed sequences: simt_backward_query_kernel_varlen, below, is this kernel's twin)
-template <int NCH>
-__global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const AttentionParams p) {
-  extern __shared__ __align__(16) float smem[];
-  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
-
-  const Operand Q = make_operand(p, sQ, p.R, b), K = make_operand(p, sK, p.C, b / p.group),
-                V = make_operand(p, sV, p.C, b / p.group);
-  const Operand O = make_operand(p, sO, p.R, b), dO = make_operand(p, sdO, p.R, b);
-  const char *Lbase = stat_row(p, sL, b);
-  char *Dbase = stat_row(p, sD, b);
-
-  // computeD (AttentionKernel+Softmax.swift:32-221): D = (sum_d dO * O) * 1/sqrt(D), kept in FP32
-  // registers for this kernel and stored (possibly as BF16) for the dK/dV kernel.
-  float Lrow[4], Drow[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    uint32_t r = min(r0 + ty + 16 * i, p.R - 1);  // clamped like clampedParallelizationThreadOffset
-    float part = 0.f;
-    for (uint32_t d = tx; d < p.D; d += 16)
-      part = fmaf(load_elem(dO.ptr, elem_index(dO, r, d), dO.prec), load_elem(O.ptr, elem_index(O, r, d), O.prec), part);
-    Drow[i] = row_sum16(part) * p.scale;
-    Lrow[i] = load_elem(Lbase, r, p.prec[sL]);
-    if (tx == 0 && r0 + ty + 16 * i < p.R) store_elem(Dbase, r, p.prec[sD], Drow[i]);
-  }
-
-  float acc[NCH][4][4];
-#pragma unroll
-  for (int q = 0; q < NCH; ++q)
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] = 0.f;
-
-  const uint32_t cend = visible_columns(p, r0);
-  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
-    float s[4][4], dp[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);    // S  = Q K^T
-    gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);  // dP = dO V^T
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        // P = exp2(S * log2e/sqrt(D) - L);  dS = P * (dP/sqrt(D) - D)   (+Softmax.swift:419-427)
-        float pv = !masked(p, r0 + ty + 16 * i, c0 + tx + 16 * j) ? exp2f(fmaf(s[i][j], p.scale_log2, -Lrow[i])) : 0.f;
-        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv * fmaf(dp[i][j], p.scale, -Drow[i]);
-      }
-    accumulate<NCH>(acc, sP, K, c0, 0, p.D, sX, tid, tx, ty);  // dQ += dS K
-  }
-  const float one[4] = {1.f, 1.f, 1.f, 1.f};
-  store_acc<NCH>(acc, one, p, sdQ, p.R, b, r0, 0, p.D, tx, ty);
-}
-
-// ------------------------------------------------------------------------------------------------
-// backward dK/dV: dV = sum_r P^T dO;  dK = sum_r dS^T Q      (one CTA per 64 columns x D-slice)
-// Grouped K/V: blockIdx.y covers K/V heads, and the sums run over the rows of every query head of the group.
-// ------------------------------------------------------------------------------------------------
-// (packed sequences: simt_backward_key_value_kernel_varlen, below, is this kernel's twin)
-template <int NCH>
-__global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(const AttentionParams p,
-                                                                               uint32_t dSlices) {
-  extern __shared__ __align__(16) float smem[];
-  float *sA = smem, *sB = sA + kBlock * kLDA, *sPT = sB + kBlock * kLDA, *sX = sPT + kBlock * kLDP;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const uint32_t kvb = blockIdx.y / dSlices, slice = blockIdx.y % dSlices, c0 = blockIdx.x * kBlock;
-  const uint32_t dlo = slice * (NCH * kBlock);
-  const uint32_t dhi = min(p.D, dlo + NCH * kBlock);
-
-  const Operand K = make_operand(p, sK, p.C, kvb), V = make_operand(p, sV, p.C, kvb);
-
-  float accV[NCH][4][4], accK[NCH][4][4];
-#pragma unroll
-  for (int q = 0; q < NCH; ++q)
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) accV[q][i][jj] = accK[q][i][jj] = 0.f;
-
-  // causal: start at the 64-block holding the first row that sees column c0 (r >= c0 - offset)
-  const int first = static_cast<int>(c0) - p.causal_offset;
-  const uint32_t rstart = p.causal && first > 0 ? static_cast<uint32_t>(first) / kBlock * kBlock : 0;
-  for (uint32_t b = kvb * p.group; b < (kvb + 1) * p.group; ++b) {  // the query heads of the group
-    const Operand Q = make_operand(p, sQ, p.R, b), dO = make_operand(p, sdO, p.R, b);
-    const char *Lbase = stat_row(p, sL, b), *Dbase = stat_row(p, sD, b);
-    for (uint32_t r0 = rstart; r0 < p.R; r0 += kBlock) {
-      float s[4][4], dp[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-      gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);    // S[r][c]
-      gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);  // dP[r][c]
-
-      float pv[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint32_t r = r0 + ty + 16 * i;
-        uint32_t rc = min(r, p.R - 1);
-        // L and D are read back in their memory precision (+Softmax.swift:356-404, 453-468)
-        float Lr = load_elem(Lbase, rc, p.prec[sL]);
-        float Dr = load_elem(Dbase, rc, p.prec[sD]);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float e = (r < p.R && !(p.causal && static_cast<int>(c0 + tx + 16 * j) > static_cast<int>(r) + p.causal_offset))
-                        ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr))
-                        : 0.f;
-          pv[i][j] = e;
-          dp[i][j] = e * fmaf(dp[i][j], p.scale, -Dr);  // dS
-          sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = e;  // P^T
-        }
-      }
-      accumulate<NCH>(accV, sPT, dO, r0, dlo, dhi, sX, tid, tx, ty);  // dV += P^T dO
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = dp[i][j];  // dS^T
-      accumulate<NCH>(accK, sPT, Q, r0, dlo, dhi, sX, tid, tx, ty);  // dK += dS^T Q
-    }
-  }
-  const float one[4] = {1.f, 1.f, 1.f, 1.f};
-  store_acc<NCH>(accV, one, p, sdV, p.C, kvb, c0, dlo, dhi, tx, ty);
-  store_acc<NCH>(accK, one, p, sdK, p.C, kvb, c0, dlo, dhi, tx, ty);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Packed sequences (Sequences): the same three kernels on sequence blockIdx.z of every problem, with its span in place
-// of R, C and the causal offset.  Kernels of their own rather than a template flag on the ones above, which keeps those
-// instruction for instruction as they were.  Row-major operands only (a transposed operand's leading dimension is the
-// whole buffer, which Operand does not carry; kernel.cpp rejects them).  A change to a kernel above needs the same
-// change in its twin here.  Rows past a sequence's end read as zeros (Operand::seq).
-// ------------------------------------------------------------------------------------------------
 struct Span {
   SequenceSpan s;
-  int offset;  // causal: row r sees column c iff c <= r + offset (Cs - Rs)
+  int offset;  // row r's diagonal is column r + offset
 };
-__device__ __forceinline__ Span span_of(const Sequences &seq) {
+template <Layout kLayout>
+__device__ __forceinline__ Span span_of(const AttentionParams &p, const Sequences &seq, const PagedKV &pk) {
   Span sp;
-  sp.s = sequence_span(seq, blockIdx.z);
-  sp.offset = static_cast<int>(sp.s.C) - static_cast<int>(sp.s.R);
+  if constexpr (kLayout == Layout::kFixed) {
+    sp.s = SequenceSpan{0, p.R, 0, p.C};
+    sp.offset = p.causal_offset;
+  } else {
+    if constexpr (kLayout == Layout::kPacked) {
+      sp.s = sequence_span(seq, blockIdx.z);
+    } else {
+      sp.s = paged_span(pk, blockIdx.z);
+    }
+    sp.offset = static_cast<int>(sp.s.C) - static_cast<int>(sp.s.R);
+  }
   return sp;
 }
 // rows [first, first + len) of problem b of `slot`, whose buffer holds `rows` rows per problem
@@ -521,15 +290,7 @@ __device__ __forceinline__ Operand span_key(const AttentionParams &p, int slot, 
 __device__ __forceinline__ char *span_stats(const AttentionParams &p, int slot, uint32_t b, const Span &sp) {
   return stat_row(p, slot, b) + static_cast<size_t>(sp.s.q0) * (p.prec[slot] == FP32 ? 4 : 2);
 }
-__device__ __forceinline__ uint32_t span_visible_columns(const AttentionParams &p, const Span &sp, uint32_t r0) {
-  if (!p.causal) return sp.s.C;
-  const int last = static_cast<int>(min(r0 + kBlock, sp.s.R)) - 1 + sp.offset;
-  return last < 0 ? 0u : min(sp.s.C, static_cast<uint32_t>(last) + 1);
-}
-__device__ __forceinline__ bool span_masked(const AttentionParams &p, const Span &sp, uint32_t r, uint32_t c) {
-  return c >= sp.s.C || (p.causal && static_cast<int>(c) > static_cast<int>(r) + sp.offset);
-}
-// store_acc to the rows [0, op.seq) of `op`
+// store a [64 x (NCH*64)] register accumulator block, each row scaled, to the rows [0, op.seq) of `op`
 template <int NCH>
 __device__ __forceinline__ void span_store(const float (&acc)[NCH][4][4], const float (&rowScale)[4], const Operand &op,
                                            uint32_t s0, uint32_t dlo, uint32_t dhi, int tx, int ty) {
@@ -556,438 +317,200 @@ __device__ __forceinline__ void zero_acc(float (&acc)[NCH][4][4]) {
       for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] = 0.f;
 }
 
-template <int NCH>
-__global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel_varlen(const AttentionParams p, const Sequences seq) {
-  extern __shared__ __align__(16) float smem[];
-  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
-  const Span sp = span_of(seq);
-  if (r0 >= sp.s.R) return;  // a tile past the sequence's end
-  const Operand Q = span_query(p, sQ, b, sp), K = span_key(p, sK, b / p.group, sp), V = span_key(p, sV, b / p.group, sp);
-  float m[4], l[4], acc[NCH][4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    m[i] = -FLT_MAX;
-    l[i] = FLT_TRUE_MIN;
-  }
-  zero_acc(acc);
-  const uint32_t cend = span_visible_columns(p, sp, r0);
-  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
-    float s[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      float mx = -FLT_MAX;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (span_masked(p, sp, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
-        mx = fmaxf(mx, s[i][j]);
-      }
-      mx = row_max16(mx);
-      const float m_new = fmaxf(m[i], mx * p.scale_log2), correction = exp2f(m[i] - m_new);
-      float sum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float pv = exp2f(fmaf(s[i][j], p.scale_log2, -m_new));
-        sum += pv;
-        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv;
-      }
-      l[i] = fmaf(l[i], correction, row_sum16(sum));
-      m[i] = m_new;
-#pragma unroll
-      for (int q = 0; q < NCH; ++q)
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] *= correction;
-    }
-    accumulate<NCH>(acc, sP, V, c0, 0, p.D, sX, tid, tx, ty);
-  }
-  // a row that sees no key (causal, or a sequence without keys) gets O = 0 and L = +inf
-  float inv[4];
-  bool empty[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    empty[i] = sp.s.C == 0 || (p.causal && static_cast<int>(r0 + ty + 16 * i) + sp.offset < 0);
-    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
-  }
-  span_store<NCH>(acc, inv, span_query(p, sO, b, sp), r0, 0, p.D, tx, ty);
-  if (tx == 0 && p.buf[sL] != nullptr) {
-    char *Lbase = span_stats(p, sL, b, sp);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint32_t r = r0 + ty + 16 * i;
-      if (r < sp.s.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
-    }
-  }
-}
-
-// Paged K/V: simt_forward_kernel_varlen with K and V read from the sequence's pages of the pools (PagedOperand)
-template <int NCH>
-__global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel_paged(const AttentionParams p, const PagedKV pk) {
-  extern __shared__ __align__(16) float smem[];
-  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
-  Span sp;
-  sp.s = paged_span(pk, blockIdx.z);
-  sp.offset = static_cast<int>(sp.s.C) - static_cast<int>(sp.s.R);
-  if (r0 >= sp.s.R) return;  // a tile past the sequence's end
-  const Operand Q = span_query(p, sQ, b, sp);
-  const int32_t *table = pk.page_table + static_cast<size_t>(blockIdx.z) * pk.page_stride;
-  const PagedOperand K{p.buf[sK], table, sp.s.C, p.D, pk.kv_heads, b / p.group, pk.pages, pk.page_shift, p.prec[sK]},
-      V{p.buf[sV], table, sp.s.C, p.D, pk.kv_heads, b / p.group, pk.pages, pk.page_shift, p.prec[sV]};
-  float m[4], l[4], acc[NCH][4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    m[i] = -FLT_MAX;
-    l[i] = FLT_TRUE_MIN;
-  }
-  zero_acc(acc);
-  const uint32_t cend = span_visible_columns(p, sp, r0);
-  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
-    float s[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      float mx = -FLT_MAX;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (span_masked(p, sp, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
-        mx = fmaxf(mx, s[i][j]);
-      }
-      mx = row_max16(mx);
-      const float m_new = fmaxf(m[i], mx * p.scale_log2), correction = exp2f(m[i] - m_new);
-      float sum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float pv = exp2f(fmaf(s[i][j], p.scale_log2, -m_new));
-        sum += pv;
-        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv;
-      }
-      l[i] = fmaf(l[i], correction, row_sum16(sum));
-      m[i] = m_new;
-#pragma unroll
-      for (int q = 0; q < NCH; ++q)
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] *= correction;
-    }
-    accumulate<NCH>(acc, sP, V, c0, 0, p.D, sX, tid, tx, ty);
-  }
-  float inv[4];
-  bool empty[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    empty[i] = sp.s.C == 0 || (p.causal && static_cast<int>(r0 + ty + 16 * i) + sp.offset < 0);
-    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
-  }
-  span_store<NCH>(acc, inv, span_query(p, sO, b, sp), r0, 0, p.D, tx, ty);
-  if (tx == 0 && p.buf[sL] != nullptr) {
-    char *Lbase = span_stats(p, sL, b, sp);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint32_t r = r0 + ty + 16 * i;
-      if (r < sp.s.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
-    }
-  }
-}
-
-template <int NCH>
-__global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel_varlen(const AttentionParams p,
-                                                                                 const Sequences seq) {
-  extern __shared__ __align__(16) float smem[];
-  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
-  const Span sp = span_of(seq);
-  if (r0 >= sp.s.R) return;
-  const Operand Q = span_query(p, sQ, b, sp), K = span_key(p, sK, b / p.group, sp), V = span_key(p, sV, b / p.group, sp);
-  const Operand O = span_query(p, sO, b, sp), dO = span_query(p, sdO, b, sp);
-  const char *Lbase = span_stats(p, sL, b, sp);
-  char *Dbase = span_stats(p, sD, b, sp);
-  float Lrow[4], Drow[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const uint32_t r = min(r0 + ty + 16 * i, sp.s.R - 1);
-    float part = 0.f;
-    for (uint32_t d = tx; d < p.D; d += 16)
-      part = fmaf(load_elem(dO.ptr, elem_index(dO, r, d), dO.prec), load_elem(O.ptr, elem_index(O, r, d), O.prec), part);
-    Drow[i] = row_sum16(part) * p.scale;
-    Lrow[i] = load_elem(Lbase, r, p.prec[sL]);
-    if (tx == 0 && r0 + ty + 16 * i < sp.s.R) store_elem(Dbase, r, p.prec[sD], Drow[i]);
-  }
-  float acc[NCH][4][4];
-  zero_acc(acc);
-  const uint32_t cend = span_visible_columns(p, sp, r0);
-  for (uint32_t c0 = 0; c0 < cend; c0 += kBlock) {
-    float s[4][4], dp[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
-    gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float pv = !span_masked(p, sp, r0 + ty + 16 * i, c0 + tx + 16 * j)
-                             ? exp2f(fmaf(s[i][j], p.scale_log2, -Lrow[i]))
-                             : 0.f;
-        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv * fmaf(dp[i][j], p.scale, -Drow[i]);
-      }
-    accumulate<NCH>(acc, sP, K, c0, 0, p.D, sX, tid, tx, ty);
-  }
-  const float one[4] = {1.f, 1.f, 1.f, 1.f};
-  span_store<NCH>(acc, one, span_query(p, sdQ, b, sp), r0, 0, p.D, tx, ty);
-}
-
-template <int NCH>
-__global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel_varlen(const AttentionParams p,
-                                                                                      uint32_t dSlices,
-                                                                                      const Sequences seq) {
-  extern __shared__ __align__(16) float smem[];
-  float *sA = smem, *sB = sA + kBlock * kLDA, *sPT = sB + kBlock * kLDA, *sX = sPT + kBlock * kLDP;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const uint32_t kvb = blockIdx.y / dSlices, slice = blockIdx.y % dSlices, c0 = blockIdx.x * kBlock;
-  const uint32_t dlo = slice * (NCH * kBlock), dhi = min(p.D, dlo + NCH * kBlock);
-  const Span sp = span_of(seq);
-  if (c0 >= sp.s.C) return;  // (keys of a sequence without queries still store their zeros)
-  const Operand K = span_key(p, sK, kvb, sp), V = span_key(p, sV, kvb, sp);
-  float accV[NCH][4][4], accK[NCH][4][4];
-  zero_acc(accV);
-  zero_acc(accK);
-  const int first = static_cast<int>(c0) - sp.offset;
-  const uint32_t rstart = p.causal && first > 0 ? static_cast<uint32_t>(first) / kBlock * kBlock : 0;
-  for (uint32_t b = kvb * p.group; b < (kvb + 1) * p.group; ++b) {
-    const Operand Q = span_query(p, sQ, b, sp), dO = span_query(p, sdO, b, sp);
-    const char *Lbase = span_stats(p, sL, b, sp), *Dbase = span_stats(p, sD, b, sp);
-    for (uint32_t r0 = rstart; r0 < sp.s.R; r0 += kBlock) {
-      float s[4][4], dp[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-      gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
-      gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint32_t r = r0 + ty + 16 * i, rc = min(r, sp.s.R - 1);
-        const float Lr = load_elem(Lbase, rc, p.prec[sL]), Dr = load_elem(Dbase, rc, p.prec[sD]);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float e = r < sp.s.R && !span_masked(p, sp, r, c0 + tx + 16 * j)
-                              ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr))
-                              : 0.f;
-          dp[i][j] = e * fmaf(dp[i][j], p.scale, -Dr);  // dS
-          sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = e;  // P^T
-        }
-      }
-      accumulate<NCH>(accV, sPT, dO, r0, dlo, dhi, sX, tid, tx, ty);  // dV += P^T dO
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) sPT[(tx + 16 * j) * kLDP + ty + 16 * i] = dp[i][j];  // dS^T
-      accumulate<NCH>(accK, sPT, Q, r0, dlo, dhi, sX, tid, tx, ty);  // dK += dS^T Q
-    }
-  }
-  const float one[4] = {1.f, 1.f, 1.f, 1.f};
-  span_store<NCH>(accV, one, span_key(p, sdV, kvb, sp), c0, dlo, dhi, tx, ty);
-  span_store<NCH>(accK, one, span_key(p, sdK, kvb, sp), c0, dlo, dhi, tx, ty);
-}
-
 // ------------------------------------------------------------------------------------------------
-// Sliding window (Band): twins of the kernels above for the fixed-length (a span {0, R, 0, C}), packed and paged calls,
-// causal or not (the host passes a causal window as right = 0).  They visit only the 64-blocks that meet the band of
-// their rows (dK/dV: of their columns) and mask each element outside it.  Kernels of their own, with the band an
-// argument of its own, so that the kernels above and AttentionParams stay as they are.
+// Masks, a compile-time choice.  kBand = false: the edge, and with p.causal the causal mask (row r sees column c iff
+// c <= r + offset).  kBand = true: the edge and a sliding window (row r sees column c iff r + offset - left <= c <=
+// r + offset + right; the host passes a causal window as right = 0), in 64-bit arithmetic since a side may be as large
+// as INT32_MAX.  They stay apart so that the kernels without a window, the family's main path, do no 64-bit work.
 // ------------------------------------------------------------------------------------------------
-enum class Layout { kFixed, kPacked, kPaged };
-
-// The span a band kernel works on: the whole R x C problem, or sequence blockIdx.z
-template <Layout kLayout>
-__device__ __forceinline__ Span band_span(const AttentionParams &p, const Sequences &seq, const PagedKV &pk) {
-  Span sp;
-  if constexpr (kLayout == Layout::kFixed) {
-    sp.s = SequenceSpan{0, p.R, 0, p.C};
-  } else if constexpr (kLayout == Layout::kPacked) {
-    sp.s = sequence_span(seq, blockIdx.z);
+// The columns [*first, *end) of the 64-blocks that the rows [r0, min(r0 + 64, Rs)) see, *first rounded down to a block
+template <bool kBand>
+__device__ __forceinline__ void key_blocks(const AttentionParams &p, const Span &sp, const Band &band, uint32_t r0,
+                                           uint32_t *first, uint32_t *end) {
+  if constexpr (kBand) {
+    const int64_t lo = static_cast<int64_t>(r0) + sp.offset - band.left;
+    const int64_t hi = static_cast<int64_t>(min(r0 + kBlock, sp.s.R)) - 1 + sp.offset + band.right;
+    *first = lo <= 0 ? 0u : static_cast<uint32_t>(min(lo, static_cast<int64_t>(sp.s.C))) / kBlock * kBlock;
+    *end = hi < 0 ? 0u : static_cast<uint32_t>(min(hi + 1, static_cast<int64_t>(sp.s.C)));
   } else {
-    sp.s = paged_span(pk, blockIdx.z);
-  }
-  sp.offset = static_cast<int>(sp.s.C) - static_cast<int>(sp.s.R);
-  return sp;
-}
-// The columns [*first, *end) of the 64-blocks that the rows [r0, min(r0 + 64, Rs)) see: [r0 + delta - left,
-// last row + delta + right] within [0, Cs), *first rounded down to a block
-__device__ __forceinline__ void band_columns(const Span &sp, const Band &band, uint32_t r0, uint32_t *first,
-                                             uint32_t *end) {
-  const int64_t lo = static_cast<int64_t>(r0) + sp.offset - band.left;
-  const int64_t hi = static_cast<int64_t>(min(r0 + kBlock, sp.s.R)) - 1 + sp.offset + band.right;
-  *first = lo <= 0 ? 0u : static_cast<uint32_t>(min(lo, static_cast<int64_t>(sp.s.C))) / kBlock * kBlock;
-  *end = hi < 0 ? 0u : static_cast<uint32_t>(min(hi + 1, static_cast<int64_t>(sp.s.C)));
-}
-// The rows [*first, *end) of the 64-blocks that see the columns [c0, min(c0 + 64, Cs)): [c0 - delta - right,
-// last column - delta + left] within [0, Rs), *first rounded down to a block
-__device__ __forceinline__ void band_rows(const Span &sp, const Band &band, uint32_t c0, uint32_t *first,
-                                          uint32_t *end) {
-  const int64_t lo = static_cast<int64_t>(c0) - sp.offset - band.right;
-  const int64_t hi = static_cast<int64_t>(min(c0 + kBlock, sp.s.C)) - 1 - sp.offset + band.left;
-  *first = lo <= 0 ? 0u : static_cast<uint32_t>(min(lo, static_cast<int64_t>(sp.s.R))) / kBlock * kBlock;
-  *end = hi < 0 ? 0u : static_cast<uint32_t>(min(hi + 1, static_cast<int64_t>(sp.s.R)));
-}
-// masked: column c is past the edge, or outside row r's band (64-bit: a side may be as large as INT32_MAX)
-__device__ __forceinline__ bool band_masked(const Span &sp, const Band &band, uint32_t r, uint32_t c) {
-  const int64_t d = static_cast<int64_t>(c) - r - sp.offset;  // column - (row + delta)
-  return c >= sp.s.C || d > band.right || -d > band.left;
-}
-// row r sees no column: the sequence has no keys, or its band lies wholly before or past them
-__device__ __forceinline__ bool band_empty(const Span &sp, const Band &band, uint32_t r) {
-  const int64_t diag = static_cast<int64_t>(r) + sp.offset;
-  return sp.s.C == 0 || diag + band.right < 0 || diag - band.left >= static_cast<int64_t>(sp.s.C);
-}
-
-// Paged K/V under a window: PagedOperand whose keys below `first` (before the band of every row of the CTA) read as
-// zero without touching their page-table entries or pages; keys at or past `seq` (the band's end) likewise
-struct BandPagedOperand {
-  PagedOperand page;
-  uint32_t first;
-};
-template <int COLS, int LD>
-__device__ __forceinline__ void load_tile(float *dst, const BandPagedOperand &op, uint32_t s0, uint32_t d0,
-                                          uint32_t dEnd, int tid) {
-  constexpr int kElems = kBlock * COLS;
-  const PagedOperand &pg = op.page;
-#pragma unroll 4
-  for (int e = tid; e < kElems; e += kThreads) {
-    const int s = e / COLS, d = e % COLS;
-    const uint32_t gs = s0 + s, gd = d0 + d;
-    float v = 0.f;
-    if (gs >= op.first && gs < pg.seq && gd < dEnd) {
-      const int page = min(max(__ldg(pg.table + (gs >> pg.page_shift)), 0), static_cast<int>(pg.pages) - 1);
-      const size_t row = (static_cast<size_t>(page) << pg.page_shift) | (gs & ((1u << pg.page_shift) - 1));
-      v = load_elem(pg.ptr, (row * pg.heads + pg.head) * pg.D + gd, pg.prec);
-    }
-    dst[s * LD + d] = v;
-  }
-}
-
-// The forward under a window, over the columns [c_first, c_end) with K / V read through OperandKV
-template <int NCH, class OperandKV>
-__device__ __forceinline__ void band_forward_body(const AttentionParams &p, const Span &sp, const Band &band,
-                                                  uint32_t b, uint32_t r0, const OperandKV &K, const OperandKV &V,
-                                                  uint32_t c_first, uint32_t c_end, float *smem) {
-  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const Operand Q = span_query(p, sQ, b, sp);
-  float m[4], l[4], acc[NCH][4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    m[i] = -FLT_MAX;
-    l[i] = FLT_TRUE_MIN;
-  }
-  zero_acc(acc);
-  for (uint32_t c0 = c_first; c0 < c_end; c0 += kBlock) {
-    float s[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      float mx = -FLT_MAX;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (band_masked(sp, band, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
-        mx = fmaxf(mx, s[i][j]);
-      }
-      mx = row_max16(mx);
-      const float m_new = fmaxf(m[i], mx * p.scale_log2), correction = exp2f(m[i] - m_new);
-      float sum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float pv = exp2f(fmaf(s[i][j], p.scale_log2, -m_new));
-        sum += pv;
-        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv;
-      }
-      l[i] = fmaf(l[i], correction, row_sum16(sum));
-      m[i] = m_new;
-#pragma unroll
-      for (int q = 0; q < NCH; ++q)
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] *= correction;
-    }
-    accumulate<NCH>(acc, sP, V, c0, 0, p.D, sX, tid, tx, ty);
-  }
-  // a row that sees no key gets O = 0 and L = +inf
-  float inv[4];
-  bool empty[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    empty[i] = band_empty(sp, band, r0 + ty + 16 * i);
-    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
-  }
-  span_store<NCH>(acc, inv, span_query(p, sO, b, sp), r0, 0, p.D, tx, ty);
-  if (tx == 0 && p.buf[sL] != nullptr) {
-    char *Lbase = span_stats(p, sL, b, sp);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint32_t r = r0 + ty + 16 * i;
-      if (r < sp.s.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
+    *first = 0;
+    if (!p.causal) {
+      *end = sp.s.C;
+    } else {
+      const int last = static_cast<int>(min(r0 + kBlock, sp.s.R)) - 1 + sp.offset;  // last column of the last row
+      *end = last < 0 ? 0u : min(sp.s.C, static_cast<uint32_t>(last) + 1);
     }
   }
 }
+// The rows [*first, *end) of the 64-blocks that see the columns [c0, min(c0 + 64, Cs)), *first rounded down to a block
+template <bool kBand>
+__device__ __forceinline__ void query_blocks(const AttentionParams &p, const Span &sp, const Band &band, uint32_t c0,
+                                             uint32_t *first, uint32_t *end) {
+  if constexpr (kBand) {
+    const int64_t lo = static_cast<int64_t>(c0) - sp.offset - band.right;
+    const int64_t hi = static_cast<int64_t>(min(c0 + kBlock, sp.s.C)) - 1 - sp.offset + band.left;
+    *first = lo <= 0 ? 0u : static_cast<uint32_t>(min(lo, static_cast<int64_t>(sp.s.R))) / kBlock * kBlock;
+    *end = hi < 0 ? 0u : static_cast<uint32_t>(min(hi + 1, static_cast<int64_t>(sp.s.R)));
+  } else {
+    const int lo = static_cast<int>(c0) - sp.offset;  // the first row that sees column c0
+    *first = p.causal && lo > 0 ? static_cast<uint32_t>(lo) / kBlock * kBlock : 0;
+    *end = sp.s.R;
+  }
+}
+// column c is past the edge (tested with kEdge), or hidden from row r
+template <bool kBand, bool kEdge = true>
+__device__ __forceinline__ bool masked(const AttentionParams &p, const Span &sp, const Band &band, uint32_t r,
+                                       uint32_t c) {
+  if constexpr (kBand) {
+    const int64_t d = static_cast<int64_t>(c) - r - sp.offset;  // column - (row + offset)
+    return (kEdge && c >= sp.s.C) || d > band.right || -d > band.left;
+  } else {
+    return (kEdge && c >= sp.s.C) || (p.causal && static_cast<int>(c) > static_cast<int>(r) + sp.offset);
+  }
+}
+// row r sees no column: the span has no keys, or the row's diagonal (band) lies wholly before or past them
+template <bool kBand>
+__device__ __forceinline__ bool row_empty(const AttentionParams &p, const Span &sp, const Band &band, uint32_t r) {
+  if constexpr (kBand) {
+    const int64_t diag = static_cast<int64_t>(r) + sp.offset;
+    return sp.s.C == 0 || diag + band.right < 0 || diag - band.left >= static_cast<int64_t>(sp.s.C);
+  } else {
+    return sp.s.C == 0 || (p.causal && static_cast<int>(r) + sp.offset < 0);
+  }
+}
 
-template <int NCH, Layout kLayout>
-__global__ void __launch_bounds__(kThreads, 1) simt_band_forward_kernel(const AttentionParams p, const Sequences seq,
-                                                                        const PagedKV pk, const Band band) {
-  extern __shared__ __align__(16) float smem[];
-  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
-  const Span sp = band_span<kLayout>(p, seq, pk);
-  if (r0 >= sp.s.R) return;  // a tile past the sequence's end
-  uint32_t c_first, c_end;
-  band_columns(sp, band, r0, &c_first, &c_end);
+// K or V (`slot`) of K/V head kv for the forward tile of rows [r0, r0 + 64): the span's rows of the operand, or a paged
+// call's keys through its page table.  Under a window, a paged operand reads only the keys the tile's band can meet:
+// none before the band of its first row, nor any from the end of its key blocks on.
+template <Layout kLayout, bool kBand>
+__device__ __forceinline__ auto key_operand(const AttentionParams &p, int slot, uint32_t kv, const Span &sp,
+                                            const PagedKV &pk, const Band &band, uint32_t r0) {
   if constexpr (kLayout == Layout::kPaged) {
-    const int32_t *table = pk.page_table + static_cast<size_t>(blockIdx.z) * pk.page_stride;
-    // (keys before the band of the tile's first row, and from c_end on, are never read)
-    const uint32_t first = static_cast<uint32_t>(
-        max(static_cast<int64_t>(r0) + sp.offset - band.left, static_cast<int64_t>(0)));
-    const BandPagedOperand K{{p.buf[sK], table, c_end, p.D, pk.kv_heads, b / p.group, pk.pages, pk.page_shift,
-                              p.prec[sK]},
-                             first},
-        V{{p.buf[sV], table, c_end, p.D, pk.kv_heads, b / p.group, pk.pages, pk.page_shift, p.prec[sV]}, first};
-    band_forward_body<NCH>(p, sp, band, b, r0, K, V, c_first, c_end, smem);
+    PagedOperand<kBand> op;
+    op.ptr = p.buf[slot];
+    op.table = pk.page_table + static_cast<size_t>(blockIdx.z) * pk.page_stride;
+    op.pk = pk;
+    op.seq = sp.s.C;
+    op.D = p.D;
+    op.head = kv;
+    op.prec = p.prec[slot];
+    if constexpr (kBand) {
+      uint32_t c_first;
+      key_blocks<true>(p, sp, band, r0, &c_first, &op.seq);
+      op.first =
+          static_cast<uint32_t>(max(static_cast<int64_t>(r0) + sp.offset - band.left, static_cast<int64_t>(0)));
+    }
+    return op;
   } else {
-    band_forward_body<NCH>(p, sp, band, b, r0, span_key(p, sK, b / p.group, sp), span_key(p, sV, b / p.group, sp),
-                           c_first, c_end, smem);
+    return span_key(p, slot, kv, sp);
   }
 }
 
-template <int NCH, Layout kLayout>
-__global__ void __launch_bounds__(kThreads, 1) simt_band_backward_query_kernel(const AttentionParams p,
-                                                                               const Sequences seq, const Band band) {
+// ------------------------------------------------------------------------------------------------
+// forward: O = softmax(Q K^T / sqrt(D)) V,  L = log2(e) * logsumexp          (one CTA per 64 rows)
+// ------------------------------------------------------------------------------------------------
+template <int NCH, Layout kLayout, bool kBand>
+__device__ __forceinline__ void forward_body(const AttentionParams &p, const Sequences &seq, const PagedKV &pk,
+                                             const Band &band) {
   extern __shared__ __align__(16) float smem[];
   float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
-  const Span sp = band_span<kLayout>(p, seq, PagedKV{});
-  if (r0 >= sp.s.R) return;
+  const Span sp = span_of<kLayout>(p, seq, pk);
+  if (kLayout != Layout::kFixed && r0 >= sp.s.R) return;  // a tile past the sequence's end (a fixed grid has none)
+  const Operand Q = span_query(p, sQ, b, sp);
+  const auto K = key_operand<kLayout, kBand>(p, sK, b / p.group, sp, pk, band, r0),
+             V = key_operand<kLayout, kBand>(p, sV, b / p.group, sp, pk, band, r0);
+
+  // m = -FLT_MAX, l = denorm_min  (AttentionKernel+Caching.swift:310-311)
+  float m[4], l[4], acc[NCH][4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    m[i] = -FLT_MAX;
+    l[i] = FLT_TRUE_MIN;
+  }
+  zero_acc(acc);
+  uint32_t c_first, c_end;
+  key_blocks<kBand>(p, sp, band, r0, &c_first, &c_end);
+  for (uint32_t c0 = c_first; c0 < c_end; c0 += kBlock) {
+    float s[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
+    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      // mask (AttentionKernel+Softmax.swift:228-260), then online max / correction / sum (:267-324)
+      float mx = -FLT_MAX;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (masked<kBand>(p, sp, band, r0 + ty + 16 * i, c0 + tx + 16 * j)) s[i][j] = -INFINITY;
+        mx = fmaxf(mx, s[i][j]);
+      }
+      mx = row_max16(mx);
+      const float m_new = fmaxf(m[i], mx * p.scale_log2), correction = exp2f(m[i] - m_new);
+      float sum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float pv = exp2f(fmaf(s[i][j], p.scale_log2, -m_new));
+        sum += pv;
+        sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv;
+      }
+      l[i] = fmaf(l[i], correction, row_sum16(sum));
+      m[i] = m_new;
+#pragma unroll
+      for (int q = 0; q < NCH; ++q)
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) acc[q][i][jj] *= correction;
+    }
+    // (the __syncthreads inside accumulate() orders the sP writes before its reads)
+    accumulate<NCH>(acc, sP, V, c0, 0, p.D, sX, tid, tx, ty);
+  }
+
+  // O *= 1/l on the last iteration (AttentionKernel+Source.swift:169-171); L = m + log2(l) (+Caching.swift:373-377)
+  // a row that sees no column gets O = 0 and L = +inf
+  float inv[4];
+  bool empty[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    empty[i] = row_empty<kBand>(p, sp, band, r0 + ty + 16 * i);
+    inv[i] = empty[i] ? 0.f : 1.0f / l[i];
+  }
+  span_store<NCH>(acc, inv, span_query(p, sO, b, sp), r0, 0, p.D, tx, ty);
+  if (tx == 0 && p.buf[sL] != nullptr) {
+    char *Lbase = span_stats(p, sL, b, sp);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint32_t r = r0 + ty + 16 * i;
+      if (r < sp.s.R) store_elem(Lbase, r, p.prec[sL], empty[i] ? INFINITY : m[i] + log2f(l[i]));
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// backward dQ: D = rowsum(dO * O)/sqrt(D);  dQ = sum_c P (dP/sqrt(D) - D) K     (one CTA per 64 rows)
+// ------------------------------------------------------------------------------------------------
+template <int NCH, Layout kLayout, bool kBand>
+__device__ __forceinline__ void backward_query_body(const AttentionParams &p, const Sequences &seq, const Band &band) {
+  static_assert(kLayout != Layout::kPaged, "paged calls are forward only");
+  extern __shared__ __align__(16) float smem[];
+  float *sA = smem, *sB = sA + kBlock * kLDA, *sP = sB + kBlock * kLDA, *sX = sP + kBlock * kLDP;
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const uint32_t b = blockIdx.y, r0 = blockIdx.x * kBlock;
+  const Span sp = span_of<kLayout>(p, seq, PagedKV{});
+  if (kLayout != Layout::kFixed && r0 >= sp.s.R) return;  // a tile past the sequence's end (a fixed grid has none)
   const Operand Q = span_query(p, sQ, b, sp), K = span_key(p, sK, b / p.group, sp), V = span_key(p, sV, b / p.group, sp);
   const Operand O = span_query(p, sO, b, sp), dO = span_query(p, sdO, b, sp);
   const char *Lbase = span_stats(p, sL, b, sp);
   char *Dbase = span_stats(p, sD, b, sp);
+
+  // computeD (AttentionKernel+Softmax.swift:32-221): D = (sum_d dO * O) * 1/sqrt(D), kept in FP32
+  // registers for this kernel and stored (possibly as BF16) for the dK/dV kernel.
   float Lrow[4], Drow[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const uint32_t r = min(r0 + ty + 16 * i, sp.s.R - 1);
+    const uint32_t r = min(r0 + ty + 16 * i, sp.s.R - 1);  // clamped like clampedParallelizationThreadOffset
     float part = 0.f;
     for (uint32_t d = tx; d < p.D; d += 16)
       part = fmaf(load_elem(dO.ptr, elem_index(dO, r, d), dO.prec), load_elem(O.ptr, elem_index(O, r, d), O.prec), part);
@@ -995,52 +518,61 @@ __global__ void __launch_bounds__(kThreads, 1) simt_band_backward_query_kernel(c
     Lrow[i] = load_elem(Lbase, r, p.prec[sL]);
     if (tx == 0 && r0 + ty + 16 * i < sp.s.R) store_elem(Dbase, r, p.prec[sD], Drow[i]);
   }
+
   float acc[NCH][4][4];
   zero_acc(acc);
   uint32_t c_first, c_end;
-  band_columns(sp, band, r0, &c_first, &c_end);
+  key_blocks<kBand>(p, sp, band, r0, &c_first, &c_end);
   for (uint32_t c0 = c_first; c0 < c_end; c0 += kBlock) {
     float s[4][4], dp[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
       for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
-    gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);
+    gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);    // S  = Q K^T
+    gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);  // dP = dO V^T
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float pv = !band_masked(sp, band, r0 + ty + 16 * i, c0 + tx + 16 * j)
+        // P = exp2(S * log2e/sqrt(D) - L);  dS = P * (dP/sqrt(D) - D)   (+Softmax.swift:419-427)
+        const float pv = !masked<kBand>(p, sp, band, r0 + ty + 16 * i, c0 + tx + 16 * j)
                              ? exp2f(fmaf(s[i][j], p.scale_log2, -Lrow[i]))
                              : 0.f;
         sP[(ty + 16 * i) * kLDP + tx + 16 * j] = pv * fmaf(dp[i][j], p.scale, -Drow[i]);
       }
-    accumulate<NCH>(acc, sP, K, c0, 0, p.D, sX, tid, tx, ty);
+    accumulate<NCH>(acc, sP, K, c0, 0, p.D, sX, tid, tx, ty);  // dQ += dS K
   }
   const float one[4] = {1.f, 1.f, 1.f, 1.f};
   span_store<NCH>(acc, one, span_query(p, sdQ, b, sp), r0, 0, p.D, tx, ty);
 }
 
-template <int NCH, Layout kLayout>
-__global__ void __launch_bounds__(kThreads, 1) simt_band_backward_key_value_kernel(const AttentionParams p,
-                                                                                   uint32_t dSlices,
-                                                                                   const Sequences seq,
-                                                                                   const Band band) {
+// ------------------------------------------------------------------------------------------------
+// backward dK/dV: dV = sum_r P^T dO;  dK = sum_r dS^T Q      (one CTA per 64 columns x D-slice)
+// Grouped K/V: blockIdx.y covers K/V heads, and the sums run over the rows of every query head of the group.
+// ------------------------------------------------------------------------------------------------
+template <int NCH, Layout kLayout, bool kBand>
+__device__ __forceinline__ void backward_key_value_body(const AttentionParams &p, uint32_t dSlices,
+                                                        const Sequences &seq, const Band &band) {
+  static_assert(kLayout != Layout::kPaged, "paged calls are forward only");
   extern __shared__ __align__(16) float smem[];
   float *sA = smem, *sB = sA + kBlock * kLDA, *sPT = sB + kBlock * kLDA, *sX = sPT + kBlock * kLDP;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const uint32_t kvb = blockIdx.y / dSlices, slice = blockIdx.y % dSlices, c0 = blockIdx.x * kBlock;
   const uint32_t dlo = slice * (NCH * kBlock), dhi = min(p.D, dlo + NCH * kBlock);
-  const Span sp = band_span<kLayout>(p, seq, PagedKV{});
-  if (c0 >= sp.s.C) return;  // (columns that no row sees still store their zeros)
+  const Span sp = span_of<kLayout>(p, seq, PagedKV{});
+  // a tile past the sequence's end (a fixed grid has none); columns that no row sees still store their zeros
+  if (kLayout != Layout::kFixed && c0 >= sp.s.C) return;
   const Operand K = span_key(p, sK, kvb, sp), V = span_key(p, sV, kvb, sp);
   float accV[NCH][4][4], accK[NCH][4][4];
   zero_acc(accV);
   zero_acc(accK);
   uint32_t r_first, r_end;
-  band_rows(sp, band, c0, &r_first, &r_end);
-  for (uint32_t b = kvb * p.group; b < (kvb + 1) * p.group; ++b) {
+  query_blocks<kBand>(p, sp, band, c0, &r_first, &r_end);
+  // Columns past Cs need no mask here: their keys read as zero, and their dK / dV rows are never stored.  The fixed-length
+  // kernels leave them unmasked; the packed ones keep the test, without which ptxas spills the packed kernel at NCH = 4.
+  constexpr bool kColumnEdge = kLayout != Layout::kFixed;
+  for (uint32_t b = kvb * p.group; b < (kvb + 1) * p.group; ++b) {  // the query heads of the group
     const Operand Q = span_query(p, sQ, b, sp), dO = span_query(p, sdO, b, sp);
     const char *Lbase = span_stats(p, sL, b, sp), *Dbase = span_stats(p, sD, b, sp);
     for (uint32_t r0 = r_first; r0 < r_end; r0 += kBlock) {
@@ -1049,15 +581,16 @@ __global__ void __launch_bounds__(kThreads, 1) simt_band_backward_key_value_kern
       for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) s[i][j] = dp[i][j] = 0.f;
-      gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);
-      gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);
+      gemm_nt(s, Q, r0, K, c0, sA, sB, tid, tx, ty);    // S[r][c]
+      gemm_nt(dp, dO, r0, V, c0, sA, sB, tid, tx, ty);  // dP[r][c]
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const uint32_t r = r0 + ty + 16 * i, rc = min(r, sp.s.R - 1);
+        // L and D are read back in their memory precision (+Softmax.swift:356-404, 453-468)
         const float Lr = load_elem(Lbase, rc, p.prec[sL]), Dr = load_elem(Dbase, rc, p.prec[sD]);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const float e = r < sp.s.R && !band_masked(sp, band, r, c0 + tx + 16 * j)
+          const float e = r < sp.s.R && !masked<kBand, kColumnEdge>(p, sp, band, r, c0 + tx + 16 * j)
                               ? exp2f(fmaf(s[i][j], p.scale_log2, -Lr))
                               : 0.f;
           dp[i][j] = e * fmaf(dp[i][j], p.scale, -Dr);  // dS
@@ -1075,6 +608,62 @@ __global__ void __launch_bounds__(kThreads, 1) simt_band_backward_key_value_kern
   const float one[4] = {1.f, 1.f, 1.f, 1.f};
   span_store<NCH>(accV, one, span_key(p, sdV, kvb, sp), c0, dlo, dhi, tx, ty);
   span_store<NCH>(accK, one, span_key(p, sdK, kvb, sp), c0, dlo, dhi, tx, ty);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Entry points: fixed-length, packed (_varlen) and paged (forward only) calls without a window, and the same forms under
+// a window (simt_band_*, with Layout a template parameter).  Each is its body with the form fixed at compile time.
+// ------------------------------------------------------------------------------------------------
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel(const AttentionParams p) {
+  forward_body<NCH, Layout::kFixed, false>(p, Sequences{}, PagedKV{}, Band{});
+}
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel_varlen(const AttentionParams p, const Sequences seq) {
+  forward_body<NCH, Layout::kPacked, false>(p, seq, PagedKV{}, Band{});
+}
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_forward_kernel_paged(const AttentionParams p, const PagedKV pk) {
+  forward_body<NCH, Layout::kPaged, false>(p, Sequences{}, pk, Band{});
+}
+template <int NCH, Layout kLayout>
+__global__ void __launch_bounds__(kThreads, 1) simt_band_forward_kernel(const AttentionParams p, const Sequences seq,
+                                                                        const PagedKV pk, const Band band) {
+  forward_body<NCH, kLayout, true>(p, seq, pk, band);
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel(const AttentionParams p) {
+  backward_query_body<NCH, Layout::kFixed, false>(p, Sequences{}, Band{});
+}
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_backward_query_kernel_varlen(const AttentionParams p,
+                                                                                 const Sequences seq) {
+  backward_query_body<NCH, Layout::kPacked, false>(p, seq, Band{});
+}
+template <int NCH, Layout kLayout>
+__global__ void __launch_bounds__(kThreads, 1) simt_band_backward_query_kernel(const AttentionParams p,
+                                                                               const Sequences seq, const Band band) {
+  backward_query_body<NCH, kLayout, true>(p, seq, band);
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel(const AttentionParams p,
+                                                                               uint32_t dSlices) {
+  backward_key_value_body<NCH, Layout::kFixed, false>(p, dSlices, Sequences{}, Band{});
+}
+template <int NCH>
+__global__ void __launch_bounds__(kThreads, 1) simt_backward_key_value_kernel_varlen(const AttentionParams p,
+                                                                                      uint32_t dSlices,
+                                                                                      const Sequences seq) {
+  backward_key_value_body<NCH, Layout::kPacked, false>(p, dSlices, seq, Band{});
+}
+template <int NCH, Layout kLayout>
+__global__ void __launch_bounds__(kThreads, 1) simt_band_backward_key_value_kernel(const AttentionParams p,
+                                                                                   uint32_t dSlices,
+                                                                                   const Sequences seq,
+                                                                                   const Band band) {
+  backward_key_value_body<NCH, kLayout, true>(p, dSlices, seq, band);
 }
 
 inline int chunks_for(uint32_t D) { return (D + kBlock - 1) / kBlock; }
