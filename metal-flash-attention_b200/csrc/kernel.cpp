@@ -292,7 +292,7 @@ static int paged_of(const mfa_attention_kernel *k, const mfa_function_constants_
 // table's checks come first.  The key bound the plan cuts is the hint, or the table's bound (capped so that block counts
 // cannot overflow).
 constexpr uint32_t kMaxKeySplits = 16;
-static int split_of(const mfa_attention_kernel *k, const mfa_split_kv_t *s, ForwardCall *call) {
+static int split_of(const mfa_attention_kernel *k, const mfa_split_kv_t *s, AttentionCall *call) {
   if (!s) return fail(MFA_ERROR_INVALID_ARGUMENT, "Split-KV: NULL split.");
   if (k->type != MFA_FORWARD)
     return fail(MFA_ERROR_INVALID_ARGUMENT, "Split-KV: only the forward kernel splits its key range.");
@@ -320,11 +320,11 @@ static int fp8_of(const mfa_attention_kernel *k, const mfa_fp8_kv_t *f, Fp8KV *o
   return MFA_SUCCESS;
 }
 
-// The plan of a forward call on the tensor cores, per batch slice (a paged call is one slice), with the kernel's window:
+// The plan of a call on the tensor cores, per batch slice (a paged call is one slice), with the kernel's window:
 // f(first problem of the slice, plan)
 template <class F>
-static int forward_plans(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, ForwardCall call,
-                         F f) {
+static int wgmma_plans(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, AttentionCall call,
+                       F f) {
   const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
   uint32_t group = 1;
   const int status = kv_group_of(c, &group);
@@ -332,9 +332,11 @@ static int forward_plans(const mfa_attention_kernel_t *kernel, const mfa_functio
   Band band;
   call.band = band_of(kernel, c->row, call.pk ? call.pk->max_keys : c->column, &band);
   const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, sm_count = device_sm_count(current_device());
+  // (only the dK/dV plan reads it)
+  const bool convert_dO = d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q];
   return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t h0, uint32_t batch) -> int {
-    f(h0, wgmma_forward_plan(Dp, c->row, c->column, batch, group, d.split_min_blocks, d.split_max ? d.split_max : 1,
-                             call, sm_count));
+    f(h0, wgmma_plan(kernel->type, Dp, c->row, c->column, batch, group, d.split_min_blocks,
+                     d.split_max ? d.split_max : 1, convert_dO, call, sm_count));
     return MFA_SUCCESS;
   });
 }
@@ -347,9 +349,8 @@ static int encode_arguments(const mfa_attention_kernel_t *kernel, const mfa_func
   return MFA_SUCCESS;
 }
 
-// encode() of any kernel type in the form `call` describes (the backward kernels take call.seq only); the kernel's
-// window is added to the call here
-static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, ForwardCall call,
+// encode() of any kernel type in the form `call` describes; the kernel's window is added to the call here
+static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, AttentionCall call,
                   void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream);
 
 }  // namespace mfa
@@ -411,7 +412,7 @@ int mfa_attention_kernel_create(const mfa_attention_kernel_descriptor_t *kd, mfa
                   "descriptor.");
     }
     // (only the geometry fields are used: they depend on neither the problem size nor the device)
-    const WgmmaPlan plan = wgmma_plan(k->type, Dp, 1, 1, 1, 1, 0, 1, false, 1);
+    const WgmmaPlan plan = wgmma_plan(k->type, Dp, 1, 1, 1, 1, 0, 1, false, AttentionCall{}, 1);
     k->threads = plan.threads;
     k->smem_bytes = plan.smem_bytes;
     k->par = plan.par;
@@ -490,11 +491,11 @@ int mfa_attention_kernel_threadgroup_memory_allocation(const mfa_attention_kerne
 }
 
 namespace mfa {
-static int grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const ForwardCall &call,
-                     uint32_t *out) {
-  if (kernel->backend == MFA_BACKEND_TCGEN05 && kernel->type == MFA_FORWARD) {
-    *out = 0;  // the CTAs of one key range
-    return forward_plans(kernel, c, call, [&](uint32_t, const WgmmaPlan &plan) {
+static int grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                     const AttentionCall &call, uint32_t *out) {
+  if (kernel->backend == MFA_BACKEND_TCGEN05) {
+    *out = 0;  // the CTAs of one traversal range
+    return wgmma_plans(kernel, c, call, [&](uint32_t, const WgmmaPlan &plan) {
       *out += static_cast<uint32_t>(static_cast<uint64_t>(plan.grid.x) * plan.grid.y * plan.grid.z / plan.splits);
     });
   }
@@ -516,43 +517,31 @@ static int grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_co
 }
 
 static int launch_count(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
-                        const ForwardCall &call, uint32_t *out) {
-  const mfa_attention_kernel_descriptor_t &d = kernel->descriptor;
-  const uint32_t Dp = (d.head_dimension + 7u) / 8u * 8u, staged = __builtin_popcount(staged_operands(kernel));
+                        const AttentionCall &call, uint32_t *out) {
   *out = 0;
-  if (kernel->backend == MFA_BACKEND_TCGEN05 && kernel->type == MFA_FORWARD)
-    return forward_plans(kernel, c, call, [&](uint32_t, const WgmmaPlan &plan) { *out += staged + plan.launches; });
+  if (kernel->backend == MFA_BACKEND_TCGEN05) {
+    const uint32_t staged = __builtin_popcount(staged_operands(kernel));
+    return wgmma_plans(kernel, c, call, [&](uint32_t, const WgmmaPlan &plan) { *out += staged + plan.launches; });
+  }
   uint32_t group = 1;
   const int status = kv_group_of(c, &group);
   if (status != MFA_SUCCESS) return status;
-  const uint32_t sm_count = kernel->backend == MFA_BACKEND_TCGEN05 ? device_sm_count(current_device()) : 0;
-  const bool convert_dO = d.memory_precisions[MFA_dO] != d.memory_precisions[MFA_Q];
-  Band band;
-  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t, uint32_t batch) -> int {
-    if (kernel->backend != MFA_BACKEND_TCGEN05)
-      *out += 1;
-    else if (call.seq)
-      *out += staged + wgmma_plan_sequences(kernel->type, Dp, call.seq->max_row, call.seq->max_column, call.seq->count,
-                                            batch, group, convert_dO, sm_count)
-                           .launches;
-    else
-      *out += staged + wgmma_plan(kernel->type, Dp, c->row, c->column, batch, group, d.split_min_blocks, d.split_max,
-                                  convert_dO, sm_count, band_of(kernel, c->row, c->column, &band))
-                           .launches;
+  return for_each_batch_slice(c->batch_count ? c->batch_count : 1, group, [&](uint32_t, uint32_t) -> int {
+    *out += 1;
     return MFA_SUCCESS;
   });
 }
 
 // The plan of a split-KV call: the forward plan's on the tensor cores, one split on the SIMT family
-static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c, const ForwardCall &call,
-                      mfa_split_plan_t *out) {
+static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
+                      const AttentionCall &call, mfa_split_plan_t *out) {
   *out = mfa_split_plan_t{1, 1, 0, 0};
   if (kernel->backend != MFA_BACKEND_TCGEN05) {
     const int status = grid_size(kernel, c, call, &out->grid_size);
     return status != MFA_SUCCESS ? status : launch_count(kernel, c, call, &out->launch_count);
   }
   const uint32_t staged = __builtin_popcount(staged_operands(kernel));
-  return forward_plans(kernel, c, call, [&](uint32_t h0, const WgmmaPlan &plan) {
+  return wgmma_plans(kernel, c, call, [&](uint32_t h0, const WgmmaPlan &plan) {
     if (h0 == 0) {
       out->splits = plan.splits;
       out->heads_per_tile = plan.heads_per_tile;
@@ -566,14 +555,14 @@ static int split_plan(const mfa_attention_kernel_t *kernel, const mfa_function_c
 int mfa_attention_kernel_grid_size(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                    uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  return grid_size(kernel, c, ForwardCall{}, out);
+  return grid_size(kernel, c, AttentionCall{}, out);
 }
 
 int mfa_attention_kernel_grid_size_sequences(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                              const mfa_sequence_table_t *table, uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   Sequences seq;
-  ForwardCall call{&seq};
+  AttentionCall call{&seq};
   const int status = sequences_of(kernel, c, table, &seq);
   return status != MFA_SUCCESS ? status : grid_size(kernel, c, call, out);
 }
@@ -585,14 +574,14 @@ const char *mfa_attention_kernel_source_name(const mfa_attention_kernel_t *kerne
 int mfa_attention_kernel_launch_count(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                       uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  return launch_count(kernel, c, ForwardCall{}, out);
+  return launch_count(kernel, c, AttentionCall{}, out);
 }
 
 int mfa_attention_kernel_launch_count_sequences(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                                 const mfa_sequence_table_t *table, uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   Sequences seq;
-  ForwardCall call{&seq};
+  AttentionCall call{&seq};
   const int status = sequences_of(kernel, c, table, &seq);
   return status != MFA_SUCCESS ? status : launch_count(kernel, c, call, out);
 }
@@ -600,14 +589,14 @@ int mfa_attention_kernel_launch_count_sequences(const mfa_attention_kernel_t *ke
 int mfa_attention_kernel_encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants,
                                 void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   if (!kernel || !constants || !buffers) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
-  return encode(kernel, constants, ForwardCall{}, buffers, cuda_stream);
+  return encode(kernel, constants, AttentionCall{}, buffers, cuda_stream);
 }
 
 int mfa_attention_kernel_grid_size_paged(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *c,
                                          const mfa_paged_kv_t *table, uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   PagedKV pk;
-  ForwardCall call{nullptr, &pk};
+  AttentionCall call{nullptr, &pk};
   const int status = paged_of(kernel, c, table, &pk);
   return status != MFA_SUCCESS ? status : grid_size(kernel, c, call, out);
 }
@@ -616,7 +605,7 @@ int mfa_attention_kernel_launch_count_paged(const mfa_attention_kernel_t *kernel
                                             const mfa_paged_kv_t *table, uint32_t *out) {
   if (!kernel || !c || !out) return fail(MFA_ERROR_INVALID_ARGUMENT, "NULL argument.");
   PagedKV pk;
-  ForwardCall call{nullptr, &pk};
+  AttentionCall call{nullptr, &pk};
   const int status = paged_of(kernel, c, table, &pk);
   return status != MFA_SUCCESS ? status : launch_count(kernel, c, call, out);
 }
@@ -630,7 +619,7 @@ int mfa_attention_kernel_split_plan(const mfa_attention_kernel_t *kernel, const 
                                                 (sequences ? "both" : "neither") + " given).");
   Sequences seq;
   PagedKV pk;
-  ForwardCall call{sequences ? &seq : nullptr, paged ? &pk : nullptr};
+  AttentionCall call{sequences ? &seq : nullptr, paged ? &pk : nullptr};
   int status = sequences ? sequences_of(kernel, c, sequences, &seq) : paged_of(kernel, c, paged, &pk);
   if (status != MFA_SUCCESS || (status = split_of(kernel, split, &call)) != MFA_SUCCESS) return status;
   return split_plan(kernel, c, call, out);
@@ -640,7 +629,7 @@ int mfa_attention_kernel_encode_paged(const mfa_attention_kernel_t *kernel, cons
                                       const mfa_paged_kv_t *table, void *const buffers[MFA_BUFFER_COUNT],
                                       void *cuda_stream) {
   PagedKV pk;
-  ForwardCall call{nullptr, &pk};
+  AttentionCall call{nullptr, &pk};
   int status = encode_arguments(kernel, constants, buffers);
   if (status != MFA_SUCCESS || (status = paged_of(kernel, constants, table, &pk)) != MFA_SUCCESS) return status;
   return encode(kernel, constants, call, buffers, cuda_stream);
@@ -650,7 +639,7 @@ int mfa_attention_kernel_encode_sequences(const mfa_attention_kernel_t *kernel,
                                           const mfa_function_constants_t *constants, const mfa_sequence_table_t *table,
                                           void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   Sequences seq;
-  ForwardCall call{&seq};
+  AttentionCall call{&seq};
   int status = encode_arguments(kernel, constants, buffers);
   if (status != MFA_SUCCESS || (status = sequences_of(kernel, constants, table, &seq)) != MFA_SUCCESS) return status;
   return encode(kernel, constants, call, buffers, cuda_stream);
@@ -661,7 +650,7 @@ int mfa_attention_kernel_encode_paged_split(const mfa_attention_kernel_t *kernel
                                             const mfa_split_kv_t *split, void *const buffers[MFA_BUFFER_COUNT],
                                             void *cuda_stream) {
   PagedKV pk;
-  ForwardCall call{nullptr, &pk};
+  AttentionCall call{nullptr, &pk};
   int status = encode_arguments(kernel, constants, buffers);
   if (status != MFA_SUCCESS || (status = paged_of(kernel, constants, table, &pk)) != MFA_SUCCESS ||
       (status = split_of(kernel, split, &call)) != MFA_SUCCESS)
@@ -675,7 +664,7 @@ int mfa_attention_kernel_encode_paged_fp8(const mfa_attention_kernel_t *kernel,
                                           void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   PagedKV pk;
   Fp8KV scales;
-  ForwardCall call{nullptr, &pk, nullptr, &scales};
+  AttentionCall call{nullptr, &pk, nullptr, &scales};
   int status = encode_arguments(kernel, constants, buffers);
   if (status != MFA_SUCCESS || (status = paged_of(kernel, constants, table, &pk)) != MFA_SUCCESS ||
       (split && (status = split_of(kernel, split, &call)) != MFA_SUCCESS) ||
@@ -689,7 +678,7 @@ int mfa_attention_kernel_encode_sequences_split(const mfa_attention_kernel_t *ke
                                                 const mfa_sequence_table_t *table, const mfa_split_kv_t *split,
                                                 void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   Sequences seq;
-  ForwardCall call{&seq};
+  AttentionCall call{&seq};
   int status = encode_arguments(kernel, constants, buffers);
   if (status != MFA_SUCCESS || (status = sequences_of(kernel, constants, table, &seq)) != MFA_SUCCESS ||
       (status = split_of(kernel, split, &call)) != MFA_SUCCESS)
@@ -767,7 +756,7 @@ int mfa_paged_kv_append_rotary(const mfa_paged_kv_t *paged, const mfa_paged_kv_a
 }  // extern "C"
 
 namespace mfa {
-static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, ForwardCall call,
+static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_constants_t *constants, AttentionCall call,
                   void *const buffers[MFA_BUFFER_COUNT], void *cuda_stream) {
   int status = check_device();
   if (status != MFA_SUCCESS) return status;
@@ -829,19 +818,8 @@ static int encode(const mfa_attention_kernel_t *kernel, const mfa_function_const
       q.D = Dp;  // (q.scale / q.scale_log2 keep the true head dimension)
       if (e != cudaSuccess) return fail(MFA_ERROR_CUDA, std::string("operand staging failed: ") + cudaGetErrorString(e));
     }
-    if (kernel->backend == MFA_BACKEND_TCGEN05) {
-      switch (kernel->type) {
-        case MFA_FORWARD: e = launch_wgmma_forward(q, call, stream); break;
-        case MFA_BACKWARD_QUERY: e = launch_wgmma_backward_query(q, seq, call.band, stream); break;
-        default: e = launch_wgmma_backward_key_value(q, seq, call.band, stream); break;
-      }
-    } else {
-      switch (kernel->type) {
-        case MFA_FORWARD: e = launch_simt_forward(q, call, stream); break;
-        case MFA_BACKWARD_QUERY: e = launch_simt_backward_query(q, seq, call.band, stream); break;
-        default: e = launch_simt_backward_key_value(q, seq, call.band, stream); break;
-      }
-    }
+    e = kernel->backend == MFA_BACKEND_TCGEN05 ? launch_wgmma(kernel->type, q, call, stream)
+                                               : launch_simt(kernel->type, q, call, stream);
     if (e != cudaSuccess)
       return fail(MFA_ERROR_CUDA, std::string("launch of ") + kernel->source_name +
                                       (call.fp8 ? " (paged FP8 K/V)" : (call.pk ? " (paged K/V)" : "")) + " failed: " +

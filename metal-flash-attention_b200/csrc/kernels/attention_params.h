@@ -139,9 +139,10 @@ struct RotarySource {
 cudaError_t launch_rotary_kv_append(const PagedKV &pk, const AppendSource &src, const RotarySource &rot, void *k_pool,
                                     void *v_pool, const Fp8KV *fp8, cudaStream_t stream);
 
-// The form of a forward call: fixed-length problems, or packed sequences (seq) or a paged cache (pk); a window; FP8 pools
-// (paged); a split-KV request of a packed or paged call (num_splits 0: the plan's choice; key_bound: every Cs's bound)
-struct ForwardCall {
+// The form of a call: fixed-length problems, or packed sequences (seq) or a paged cache (pk); a window; FP8 pools
+// (paged); a split-KV request of a packed or paged call (num_splits 0: the plan's choice; key_bound: every Cs's bound).
+// The backward takes seq and band only: the host rejects a paged table, a split and FP8 for any kernel but the forward.
+struct AttentionCall {
   const Sequences *seq = nullptr;
   const PagedKV *pk = nullptr;
   const Band *band = nullptr;
@@ -151,24 +152,17 @@ struct ForwardCall {
 };
 
 // ---- SIMT FP32 family (any shape / layout / precision) -------------------------------------
-// The forward of call.seq, call.pk and call.band (a null one: absent), never split; FP8 K/V is not served here
-cudaError_t launch_simt_forward(const AttentionParams &p, const ForwardCall &call, cudaStream_t stream);
-// The backward: seq, packed sequences, or nullptr for problems of the full R x C shape; band, a window, or nullptr
-cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
-                                       cudaStream_t stream);
-cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
-                                           cudaStream_t stream);
+// Kernel `type` (mfa_kernel_type_t) in the form of call.seq, call.pk and call.band (a null one: absent), never split;
+// FP8 K/V is not served here
+cudaError_t launch_simt(int type, const AttentionParams &p, const AttentionCall &call, cudaStream_t stream);
 void simt_geometry(int type, uint32_t D, uint32_t *threads, uint32_t *smem_bytes, uint32_t *par, uint32_t *trav,
                    uint32_t *head);
 
 // ---- tensor-core family (wgmma_attention.cu; the backend keeps its historical name "tcgen05" in the ABI) --------
 // 16-bit row-major operands with D % 8 == 0 and D <= kWgmmaMaxHead; kernel.cpp stages every other layout into that form.
 constexpr uint32_t kWgmmaMaxHead = 256;
-cudaError_t launch_wgmma_forward(const AttentionParams &p, const ForwardCall &call, cudaStream_t stream);
-cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
-                                        cudaStream_t stream);
-cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
-                                            cudaStream_t stream);
+// Kernel `type` (mfa_kernel_type_t) in the form of `call`, on the grid of its wgmma_plan
+cudaError_t launch_wgmma(int type, const AttentionParams &p, const AttentionCall &call, cudaStream_t stream);
 // How the launcher of kernel `type` (mfa_kernel_type_t) runs one problem of padded head dimension D; every field is
 // derived from the kernels' compile-time configurations.  R, C and batch do not affect the geometry fields.
 struct WgmmaPlan {
@@ -180,29 +174,22 @@ struct WgmmaPlan {
   uint32_t launches;                   // kernels the launcher issues
   uint32_t heads_per_tile;             // split-KV packed / paged forward: query heads per tile (1 elsewhere)
 };
-// batch = query problems, group = query problems per K/V problem (only the dK/dV plan, whose CTAs own K/V tiles,
-// depends on it).  band: a sliding window (host-resolved, as launched), whose width in traversal blocks, not the whole
-// traversal axis, is what the split cuts
+// The plan of a call of kernel `type`, which its launcher and the host's counts follow.  batch = query problems,
+// group = query problems per K/V problem (only the dK/dV plan, whose CTAs own K/V tiles, and the split-KV forward
+// depend on it); min_blocks and max_splits: the parameter-table row's tuning columns; convert_dO: BF16 dO beside FP16
+// Q/K/V (only the dK/dV plan depends on it).
+// - Fixed-length problems: grid (tiles, heads, splits), the traversal axis split only when the SMs would otherwise
+//   idle.  call.band (host-resolved, as launched): only the band's width in traversal blocks is what the split cuts.
+// - Packed sequences or a paged cache, unsplit: never split, grid (tiles of the longest sequence, heads, count); the
+//   dO-conversion choice counts every CTA of that grid.
+// - A split-KV packed or paged forward (mfa_split_plan_t), unless it plans one split and one head per tile: grid (tiles
+//   of max_row x splits, batch / heads_per_tile, count).  call.key_bound bounds every sequence's keys; num_splits 0
+//   lets the tuning columns choose over ceil(key_bound / BN) blocks (a window's band width when narrower);
+//   heads_per_tile: the group (2..128) when max_row < 128, so that a tile holds 128 / group rows of each query head of
+//   a K/V head.
+// An empty call gives the geometry fields, which depend on neither the problem size nor the device.
 WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
-                     uint32_t max_splits, bool convert_dO, uint32_t sm_count, const Band *band = nullptr);
-// The plan of a packed call over `count` sequences of at most max_row x max_column: never split, grid (tiles of the
-// longest sequence, heads, count); the dO-conversion choice counts every CTA of that grid
-WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t max_column, uint32_t count,
-                               uint32_t batch, uint32_t group, bool convert_dO, uint32_t sm_count);
-// The plan of a split-KV packed or paged forward (mfa_split_plan_t): grid (tiles of max_row x splits, batch, count).
-// key_bound bounds every sequence's keys (the caller's hint, or the table's bound); num_splits 0 lets the parameter-table
-// row's tuning columns choose, as choose_splits does, over ceil(key_bound / BN) blocks (a window's band width when
-// narrower); n >= 1 is taken as given.  Every value is host-visible, so launcher, split_plan, grid size and launch
-// count agree.  heads_per_tile: the group (2..128) when max_row < 128, so that a tile holds m = 128 / group rows of
-// each query head of a K/V head instead of padding rows; grid (ceil(max_row / m) x splits, batch / heads_per_tile,
-// count).
-WgmmaPlan wgmma_plan_split(uint32_t D, uint32_t max_row, uint32_t key_bound, uint32_t count, uint32_t batch,
-                           uint32_t group, uint32_t min_blocks, uint32_t max_splits, uint32_t num_splits,
-                           uint32_t sm_count, const Band *band);
-// The plan of a forward call, which its launcher and the host's counts follow: wgmma_plan for fixed-length problems,
-// wgmma_plan_split for split calls unless it plans one split and one head per tile, else wgmma_plan_sequences.
-WgmmaPlan wgmma_forward_plan(uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
-                             uint32_t max_splits, const ForwardCall &call, uint32_t sm_count);
+                     uint32_t max_splits, bool convert_dO, const AttentionCall &call, uint32_t sm_count);
 
 // operand staging for the tensor-core family (pad_head.cu): a [batch][seq][D] (or, transposed, [batch][D][seq]) operand
 // is copied to row-major [batch][seq][Dp] with zero padding columns, and an FP32 output computed in that form is copied

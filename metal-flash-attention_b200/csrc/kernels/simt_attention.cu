@@ -37,6 +37,7 @@
 
 #include "attention_params.h"
 #include "device_state.h"
+#include "mfa_b200.h"
 
 namespace mfa {
 namespace simt {
@@ -700,7 +701,7 @@ static dim3 simt_grid(uint32_t rows, uint32_t y, const Sequences *seq) {
   return dim3((rows + simt::kBlock - 1) / simt::kBlock, y, seq ? seq->count : 1);
 }
 
-cudaError_t launch_simt_forward(const AttentionParams &p, const ForwardCall &call, cudaStream_t stream) {
+static cudaError_t launch_forward(const AttentionParams &p, const AttentionCall &call, cudaStream_t stream) {
   const Sequences *seq = call.seq;
   const PagedKV *pk = call.pk;
   const Band *band = call.band;
@@ -722,8 +723,8 @@ cudaError_t launch_simt_forward(const AttentionParams &p, const ForwardCall &cal
   });
 }
 
-cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
-                                       cudaStream_t stream) {
+static cudaError_t launch_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                        cudaStream_t stream) {
   const dim3 grid = simt_grid(seq ? seq->max_row : p.R, p.batch, seq);
   return simt::with_chunks<8>(simt::chunks_for(p.D), [&](auto nch) {
     constexpr int NCH = decltype(nch)::value;
@@ -738,8 +739,8 @@ cudaError_t launch_simt_backward_query(const AttentionParams &p, const Sequences
   });
 }
 
-cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
-                                           cudaStream_t stream) {
+static cudaError_t launch_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
+                                            cudaStream_t stream) {
   // two accumulators (dV, dK) per thread: keep at most 4 chunks (256 columns) of each in registers and
   // slice larger head dimensions over blockIdx.y (each slice recomputes S and dP).
   const int chunks = simt::chunks_for(p.D);
@@ -758,6 +759,14 @@ cudaError_t launch_simt_backward_key_value(const AttentionParams &p, const Seque
     if (seq) return simt::launch(simt::simt_backward_key_value_kernel_varlen<NCH>, grid, stream, p, dSlices, *seq);
     return simt::launch(simt::simt_backward_key_value_kernel<NCH>, grid, stream, p, dSlices);
   });
+}
+
+cudaError_t launch_simt(int type, const AttentionParams &p, const AttentionCall &call, cudaStream_t stream) {
+  switch (type) {
+    case MFA_FORWARD: return launch_forward(p, call, stream);
+    case MFA_BACKWARD_QUERY: return launch_backward_query(p, call.seq, call.band, stream);
+    default: return launch_backward_key_value(p, call.seq, call.band, stream);
+  }
 }
 
 // Launch geometry reported through AttentionKernel.threadgroupSize / threadgroupMemoryAllocation /

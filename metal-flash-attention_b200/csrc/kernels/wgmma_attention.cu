@@ -1014,7 +1014,7 @@ struct BwdArgs {
 template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal, bool kVarlen, bool kBand = false>
 __device__ __forceinline__ void backward_query_body(const CUtensorMap &mapQ, const CUtensorMap &mapdO,
                                                     const CUtensorMap &mapK, const CUtensorMap &mapV, const BwdArgs &a,
-                                                    const Sequences &seq, const Band &band = Band{}) {
+                                                    const Sequences &seq, const Band &band) {
   using Cfg = QCfg<DCH>;
   constexpr uint32_t NO = DCH * 64, BN = Cfg::BN;
   extern __shared__ uint8_t smem_raw[];
@@ -1152,27 +1152,26 @@ template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
 __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     attention_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
                                    const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
-                                   const BwdArgs a) {
-  backward_query_body<DCH, kBF16, kConvertDO, kCausal, false>(mapQ, mapdO, mapK, mapV, a, Sequences{});
+                                   const BwdArgs a, const Sequences seq, const Band band) {
+  backward_query_body<DCH, kBF16, kConvertDO, kCausal, false>(mapQ, mapdO, mapK, mapV, a, seq, band);
 }
 
 template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
 __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
-    packed_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ,
-                                          const __grid_constant__ CUtensorMap mapdO,
-                                          const __grid_constant__ CUtensorMap mapK,
-                                          const __grid_constant__ CUtensorMap mapV, const BwdArgs a,
-                                          const Sequences seq) {
-  backward_query_body<DCH, kBF16, kConvertDO, kCausal, true>(mapQ, mapdO, mapK, mapV, a, seq);
+    packed_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
+                                const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
+                                const BwdArgs a, const Sequences seq, const Band band) {
+  backward_query_body<DCH, kBF16, kConvertDO, kCausal, true>(mapQ, mapdO, mapK, mapV, a, seq, band);
 }
 
 template <uint32_t DCH, bool kBF16, bool kConvertDO>
 __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     band_backward_query_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
                               const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
-                              const BwdArgs a, const Band band) {
-  backward_query_body<DCH, kBF16, kConvertDO, true, false, true>(mapQ, mapdO, mapK, mapV, a, Sequences{}, band);
+                              const BwdArgs a, const Sequences seq, const Band band) {
+  backward_query_body<DCH, kBF16, kConvertDO, true, false, true>(mapQ, mapdO, mapK, mapV, a, seq, band);
 }
+
 template <uint32_t DCH, bool kBF16, bool kConvertDO>
 __global__ void __launch_bounds__(QCfg<DCH>::kThreads, 1)
     band_backward_query_packed_wgmma(const __grid_constant__ CUtensorMap mapQ,
@@ -1199,8 +1198,7 @@ struct KVCfg {
 template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal, bool kVarlen, bool kBand = false>
 __device__ __forceinline__ void backward_key_value_body(const CUtensorMap &mapQ, const CUtensorMap &mapdO,
                                                         const CUtensorMap &mapK, const CUtensorMap &mapV,
-                                                        const BwdArgs &a, const Sequences &seq,
-                                                        const Band &band = Band{}) {
+                                                        const BwdArgs &a, const Sequences &seq, const Band &band) {
   using Cfg = KVCfg<DCH>;
   constexpr uint32_t BM = Cfg::BM, NA = Cfg::kAcc;
   extern __shared__ uint8_t smem_raw[];
@@ -1342,34 +1340,33 @@ template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
     attention_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
                                        const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
-                                       const BwdArgs a) {
-  backward_key_value_body<DCH, kBF16, kConvertDO, kCausal, false>(mapQ, mapdO, mapK, mapV, a, Sequences{});
+                                       const BwdArgs a, const Sequences seq, const Band band) {
+  backward_key_value_body<DCH, kBF16, kConvertDO, kCausal, false>(mapQ, mapdO, mapK, mapV, a, seq, band);
 }
 
 template <uint32_t DCH, bool kBF16, bool kConvertDO, bool kCausal>
 __global__ void __launch_bounds__(2 * kWG, 1)
-    packed_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ,
-                                              const __grid_constant__ CUtensorMap mapdO,
-                                              const __grid_constant__ CUtensorMap mapK,
-                                              const __grid_constant__ CUtensorMap mapV, const BwdArgs a,
-                                              const Sequences seq) {
-  backward_key_value_body<DCH, kBF16, kConvertDO, kCausal, true>(mapQ, mapdO, mapK, mapV, a, seq);
+    packed_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
+                                    const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
+                                    const BwdArgs a, const Sequences seq, const Band band) {
+  backward_key_value_body<DCH, kBF16, kConvertDO, kCausal, true>(mapQ, mapdO, mapK, mapV, a, seq, band);
 }
 
 template <uint32_t DCH, bool kBF16, bool kConvertDO>
 __global__ void __launch_bounds__(2 * kWG, 1)
     band_backward_key_value_wgmma(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapdO,
                                   const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapV,
-                                  const BwdArgs a, const Band band) {
-  backward_key_value_body<DCH, kBF16, kConvertDO, true, false, true>(mapQ, mapdO, mapK, mapV, a, Sequences{}, band);
+                                  const BwdArgs a, const Sequences seq, const Band band) {
+  backward_key_value_body<DCH, kBF16, kConvertDO, true, false, true>(mapQ, mapdO, mapK, mapV, a, seq, band);
 }
+
 template <uint32_t DCH, bool kBF16, bool kConvertDO>
 __global__ void __launch_bounds__(2 * kWG, 1)
     band_backward_key_value_packed_wgmma(const __grid_constant__ CUtensorMap mapQ,
                                          const __grid_constant__ CUtensorMap mapdO,
                                          const __grid_constant__ CUtensorMap mapK,
-                                         const __grid_constant__ CUtensorMap mapV, const BwdArgs a,
-                                         const Sequences seq, const Band band) {
+                                         const __grid_constant__ CUtensorMap mapV, const BwdArgs a, const Sequences seq,
+                                         const Band band) {
   backward_key_value_body<DCH, kBF16, kConvertDO, true, true, true>(mapQ, mapdO, mapK, mapV, a, seq, band);
 }
 
@@ -1452,21 +1449,19 @@ static cudaError_t prepare(Kernel kernel, uint32_t smem) {
   return ensure_max_dynamic_smem(reinterpret_cast<const void *>(kernel), smem, current_device());
 }
 
-// The tensor maps of a kernel: Q and (with_dO) dO in boxes of Cfg::kQueryBoxRows rows, K and V in boxes of
-// Cfg::kKeyBoxRows.  Grouped K/V: K and V hold batch / group heads.
+// The tensor maps of a backward kernel: Q and dO in boxes of query_rows rows, K and V in boxes of key_rows.  Grouped
+// K/V: K and V hold batch / group heads.
 struct TensorMaps {
   CUtensorMap Q, dO, K, V;
 };
-template <class Cfg>
-static cudaError_t make_maps(const AttentionParams &p, bool with_dO, TensorMaps *m) {
+static cudaError_t make_maps(const AttentionParams &p, uint32_t query_rows, uint32_t key_rows, TensorMaps *m) {
   cudaError_t e;
-  if ((e = make_tensor_map_16bit(&m->Q, p.buf[sQ], p.R, p.D, p.batch, Cfg::kQueryBoxRows)) != cudaSuccess) return e;
-  if (with_dO &&
-      (e = make_tensor_map_16bit(&m->dO, p.buf[sdO], p.R, p.D, p.batch, Cfg::kQueryBoxRows)) != cudaSuccess)
+  if ((e = make_tensor_map_16bit(&m->Q, p.buf[sQ], p.R, p.D, p.batch, query_rows)) != cudaSuccess ||
+      (e = make_tensor_map_16bit(&m->dO, p.buf[sdO], p.R, p.D, p.batch, query_rows)) != cudaSuccess)
     return e;
   const uint32_t kv_heads = p.batch / p.group;
-  if ((e = make_tensor_map_16bit(&m->K, p.buf[sK], p.C, p.D, kv_heads, Cfg::kKeyBoxRows)) != cudaSuccess) return e;
-  return make_tensor_map_16bit(&m->V, p.buf[sV], p.C, p.D, kv_heads, Cfg::kKeyBoxRows);
+  if ((e = make_tensor_map_16bit(&m->K, p.buf[sK], p.C, p.D, kv_heads, key_rows)) != cudaSuccess) return e;
+  return make_tensor_map_16bit(&m->V, p.buf[sV], p.C, p.D, kv_heads, key_rows);
 }
 
 // The forward kernel of a call's form.  Only the forms compiled above are reachable: the split kernels serve packed and
@@ -1490,7 +1485,7 @@ static ForwardKernel forward_kernel(KVLayout layout, bool band, bool split, bool
 // one head per tile (FP8: always).  With more than one split the kernel writes partials [split][head][row] into the
 // workspace, and merge_splits (fixed) or merge_sequence_splits (packed, paged) merges them into O and L.
 template <uint32_t DCH, bool kBF16, bool kCausal>
-static cudaError_t launch_forward(const AttentionParams &p, const ForwardCall &call, const WgmmaPlan &plan,
+static cudaError_t launch_forward(const AttentionParams &p, const AttentionCall &call, const WgmmaPlan &plan,
                                   cudaStream_t stream) {
   using Cfg = FwdCfg<DCH>;
   constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
@@ -1542,8 +1537,27 @@ static cudaError_t launch_forward(const AttentionParams &p, const ForwardCall &c
   return cudaGetLastError();
 }
 
+// The backward kernel of kernel `type` (dQ or dK/dV) in a call's form
+using BackwardKernel = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+                                const BwdArgs, const Sequences, const Band);
+template <uint32_t DCH, bool kBF16, bool kConvert, bool kCausal>
+static BackwardKernel backward_kernel(int type, bool packed, bool band) {
+  if (type == MFA_BACKWARD_QUERY) {
+    if (band)
+      return packed ? band_backward_query_packed_wgmma<DCH, kBF16, kConvert>
+                    : band_backward_query_wgmma<DCH, kBF16, kConvert>;
+    return packed ? packed_backward_query_wgmma<DCH, kBF16, kConvert, kCausal>
+                  : attention_backward_query_wgmma<DCH, kBF16, kConvert, kCausal>;
+  }
+  if (band)
+    return packed ? band_backward_key_value_packed_wgmma<DCH, kBF16, kConvert>
+                  : band_backward_key_value_wgmma<DCH, kBF16, kConvert>;
+  return packed ? packed_backward_key_value_wgmma<DCH, kBF16, kConvert, kCausal>
+                : attention_backward_key_value_wgmma<DCH, kBF16, kConvert, kCausal>;
+}
+
 static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
-  BwdArgs a;
+  BwdArgs a{};
   a.O = static_cast<const float *>(p.buf[sO]);
   a.dO = p.buf[sdO];
   a.L = p.buf[sL];
@@ -1565,50 +1579,9 @@ static BwdArgs backward_args(const AttentionParams &p, const WgmmaPlan &plan) {
   return a;
 }
 
-// A backward kernel whose outputs are the BwdArgs fields out0 and, unless null, out1: FP32 tensors of `elems` elements
-// each.  Split: each split writes partial sums to the workspace, [split][output][elems], and sum_splits adds them into
-// the outputs.
-// Packed sequences (seq): `packed` runs instead, unsplit.  `extra` (a window's Band) follows the kernels' arguments.
-using OutputSlot = float *BwdArgs::*;
-template <class Cfg, class Kernel, class PackedKernel, class... Extra>
-static cudaError_t launch_backward(Kernel kernel, PackedKernel packed, const AttentionParams &p, const WgmmaPlan &plan,
-                                   const Sequences *seq, OutputSlot out0, OutputSlot out1, size_t elems,
-                                   cudaStream_t stream, const Extra &...extra) {
-  constexpr uint32_t kSmemBytes = Cfg::Smem::kSmemBytes;
-  const uint32_t outputs = out1 ? 2 : 1;
-  TensorMaps m;
-  cudaError_t e;
-  if (seq) {
-    if ((e = prepare(packed, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, true, &m)) != cudaSuccess) return e;
-    packed<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.dO, m.K, m.V, backward_args(p, plan), *seq,
-                                                             extra...);
-    return cudaGetLastError();
-  }
-  if ((e = prepare(kernel, kSmemBytes)) != cudaSuccess || (e = make_maps<Cfg>(p, true, &m)) != cudaSuccess) return e;
-  BwdArgs a = backward_args(p, plan);
-  float *const dst0 = a.*out0, *const dst1 = out1 ? a.*out1 : nullptr;
-  float *scratch = nullptr;
-  if (plan.splits > 1) {
-    void *ws = nullptr;
-    if ((e = workspace_for(current_device(), stream, plan.splits * outputs * elems * sizeof(float), &ws)) != cudaSuccess)
-      return e;
-    scratch = static_cast<float *>(ws);
-    a.split_stride = outputs * elems;
-    a.*out0 = scratch;
-    if (out1) a.*out1 = scratch + elems;
-  }
-  kernel<<<plan.grid, Cfg::kThreads, kSmemBytes, stream>>>(m.Q, m.dO, m.K, m.V, a, extra...);
-  if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
-  const size_t quads = elems / 4;  // D % 8 == 0
-  sum_splits<<<dim3(static_cast<uint32_t>((quads + 255) / 256), outputs), 256, 0, stream>>>(
-      reinterpret_cast<const float4 *>(scratch), reinterpret_cast<float4 *>(dst0), reinterpret_cast<float4 *>(dst1), quads,
-      a.split_stride / 4, plan.splits);
-  return cudaGetLastError();
-}
-
 // Calls f(DCH, kBF16, kConvertDO, kCausal), each as a std::integral_constant, for the kernel instantiation that serves p
 template <class F>
-static cudaError_t dispatch(const AttentionParams &p, bool convert_dO, F f) {
+static auto dispatch(const AttentionParams &p, bool convert_dO, F f) {
   return with_chunks(p.D, [&](auto dch) {
     auto types = [&](auto causal) {
       if (convert_dO) return f(dch, std::false_type(), std::true_type(), causal);
@@ -1621,8 +1594,10 @@ static cudaError_t dispatch(const AttentionParams &p, bool convert_dO, F f) {
 
 }  // namespace hop
 
-WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
-                     uint32_t max_splits, bool convert_dO, uint32_t sm_count, const Band *band) {
+// The plan of fixed-length problems
+static WgmmaPlan plan_fixed(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group,
+                            uint32_t min_blocks, uint32_t max_splits, bool convert_dO, uint32_t sm_count,
+                            const Band *band) {
   WgmmaPlan p{};
   p.heads_per_tile = 1;
   auto geometry = [&](auto cfg) {
@@ -1672,10 +1647,11 @@ WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batc
   return p;
 }
 
-WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t max_column, uint32_t count,
-                               uint32_t batch, uint32_t group, bool convert_dO, uint32_t sm_count) {
+// The plan of an unsplit call over `count` packed sequences of at most max_row x max_column
+static WgmmaPlan plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t max_column, uint32_t count,
+                                uint32_t batch, uint32_t group, bool convert_dO, uint32_t sm_count) {
   // min_blocks = 0: one traversal range per tile
-  WgmmaPlan p = wgmma_plan(type, D, max_row, max_column, batch, group, 0, 1, convert_dO, sm_count);
+  WgmmaPlan p = plan_fixed(type, D, max_row, max_column, batch, group, 0, 1, convert_dO, sm_count, nullptr);
   p.grid.z = count;
   p.convert_dO_first = type == MFA_BACKWARD_KEY_VALUE && convert_dO &&
                        static_cast<uint64_t>(p.grid.x) * p.grid.y * count > sm_count;
@@ -1683,11 +1659,13 @@ WgmmaPlan wgmma_plan_sequences(int type, uint32_t D, uint32_t max_row, uint32_t 
   return p;
 }
 
-WgmmaPlan wgmma_plan_split(uint32_t D, uint32_t max_row, uint32_t key_bound, uint32_t count, uint32_t batch,
-                           uint32_t group, uint32_t min_blocks, uint32_t max_splits, uint32_t num_splits,
-                           uint32_t sm_count, const Band *band) {
+// The plan of a split-KV packed or paged forward; every value is host-visible, so launcher, split_plan, grid size and
+// launch count agree
+static WgmmaPlan plan_split(uint32_t D, uint32_t max_row, uint32_t key_bound, uint32_t count, uint32_t batch,
+                            uint32_t group, uint32_t min_blocks, uint32_t max_splits, uint32_t num_splits,
+                            uint32_t sm_count, const Band *band) {
   // unsplit, blocks_per_split is the key-block bound of one tile (a window's band width when narrower)
-  WgmmaPlan p = wgmma_plan(MFA_FORWARD, D, max_row, key_bound, batch, 1, 0, 1, false, sm_count, band);
+  WgmmaPlan p = plan_fixed(MFA_FORWARD, D, max_row, key_bound, batch, 1, 0, 1, false, sm_count, band);
   // a group's query heads share a tile when an unpacked tile would be partly empty
   p.heads_per_tile = group >= 2 && group <= p.par && max_row < p.par ? group : 1;
   const uint32_t rows = p.par / p.heads_per_tile, tiles = (max_row + rows - 1) / rows;
@@ -1698,20 +1676,20 @@ WgmmaPlan wgmma_plan_split(uint32_t D, uint32_t max_row, uint32_t key_bound, uin
   return p;
 }
 
-WgmmaPlan wgmma_forward_plan(uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
-                             uint32_t max_splits, const ForwardCall &call, uint32_t sm_count) {
+WgmmaPlan wgmma_plan(int type, uint32_t D, uint32_t R, uint32_t C, uint32_t batch, uint32_t group, uint32_t min_blocks,
+                     uint32_t max_splits, bool convert_dO, const AttentionCall &call, uint32_t sm_count) {
   if (!call.seq && !call.pk)
-    return wgmma_plan(MFA_FORWARD, D, R, C, batch, group, min_blocks, max_splits, false, sm_count, call.band);
+    return plan_fixed(type, D, R, C, batch, group, min_blocks, max_splits, convert_dO, sm_count, call.band);
   const uint32_t max_row = call.pk ? call.pk->max_row : call.seq->max_row;
   const uint32_t count = call.pk ? call.pk->count : call.seq->count;
   if (call.split) {
-    const WgmmaPlan p = wgmma_plan_split(D, max_row, call.key_bound, count, batch, group, min_blocks, max_splits,
-                                         call.num_splits, sm_count, call.band);
+    const WgmmaPlan p = plan_split(D, max_row, call.key_bound, count, batch, group, min_blocks, max_splits,
+                                   call.num_splits, sm_count, call.band);
     if (p.splits > 1 || p.heads_per_tile > 1) return p;
   }
   // (a paged call's key axis does not enter the grid)
-  return wgmma_plan_sequences(MFA_FORWARD, D, max_row, call.pk ? 1 : call.seq->max_column, count, batch, group, false,
-                              sm_count);
+  return plan_sequences(type, D, max_row, call.pk ? 1 : call.seq->max_column, count, batch, group, convert_dO,
+                        sm_count);
 }
 
 static bool row_major_16bit(const AttentionParams &p) {
@@ -1719,29 +1697,6 @@ static bool row_major_16bit(const AttentionParams &p) {
     if (p.transposed[s]) return false;
   return (p.prec[sQ] == FP16 || p.prec[sQ] == BF16) && p.prec[sK] == p.prec[sQ] && p.prec[sV] == p.prec[sQ] &&
          p.D % 8 == 0 && p.D <= kWgmmaMaxHead;
-}
-
-static WgmmaPlan plan_for(int type, const AttentionParams &p, const Sequences *seq, const Band *band,
-                          bool convert_dO) {
-  const uint32_t sm_count = device_sm_count(current_device());
-  if (seq)
-    return wgmma_plan_sequences(type, p.D, seq->max_row, seq->max_column, seq->count, p.batch, p.group, convert_dO,
-                                sm_count);
-  return wgmma_plan(type, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, convert_dO, sm_count, band);
-}
-
-cudaError_t launch_wgmma_forward(const AttentionParams &p, const ForwardCall &call, cudaStream_t stream) {
-  if (!row_major_16bit(p) || p.prec[sO] != FP32 || (call.fp8 && p.D % 16 != 0)) {
-    set_launch_detail(call.fp8 ? "descriptor is outside the FP8 K/V forward kernels' domain"
-                               : "descriptor is outside the wgmma forward kernel's domain");
-    return cudaErrorInvalidValue;
-  }
-  const WgmmaPlan plan = wgmma_forward_plan(p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, call,
-                                            device_sm_count(current_device()));
-  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
-    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, call, plan,
-                                                                                                      stream);
-  });
 }
 
 static cudaError_t check_backward(const AttentionParams &p) {
@@ -1753,54 +1708,72 @@ static cudaError_t check_backward(const AttentionParams &p) {
   return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_wgmma_backward_query(const AttentionParams &p, const Sequences *seq, const Band *band,
-                                        cudaStream_t stream) {
+// A backward call of kernel `type` in the form `call` on the grid of its plan.  dK/dV with BF16 dO beside FP16 Q/K/V on
+// a grid of more than one wave: a pass of its own converts dO to FP16 first.  Split: each split writes partial sums of
+// the outputs (dQ; or dV and dK, per K/V head) to the workspace, [split][output][elems], and sum_splits adds them into
+// the outputs.
+static cudaError_t launch_backward(int type, const AttentionParams &p, const AttentionCall &call, cudaStream_t stream) {
   if (cudaError_t e = check_backward(p)) return e;
-  const bool convert = p.prec[sdO] != p.prec[sQ];
-  const WgmmaPlan plan = plan_for(MFA_BACKWARD_QUERY, p, seq, band, convert);
-  return hop::dispatch(p, convert, [&](auto dch, auto bf16, auto cvt, auto causal) {
-    constexpr uint32_t DCH = decltype(dch)::value;
-    constexpr bool kBF16 = decltype(bf16)::value, kConvert = decltype(cvt)::value, kCausal = decltype(causal)::value;
-    if (band)
-      return hop::launch_backward<hop::QCfg<DCH>>(hop::band_backward_query_wgmma<DCH, kBF16, kConvert>,
-                                                  hop::band_backward_query_packed_wgmma<DCH, kBF16, kConvert>, p, plan,
-                                                  seq, &hop::BwdArgs::dQ, nullptr,
-                                                  static_cast<size_t>(p.batch) * p.R * p.D, stream, *band);
-    return hop::launch_backward<hop::QCfg<DCH>>(hop::attention_backward_query_wgmma<DCH, kBF16, kConvert, kCausal>,
-                                                hop::packed_backward_query_wgmma<DCH, kBF16, kConvert, kCausal>,
-                                                p, plan, seq, &hop::BwdArgs::dQ, nullptr,
-                                                static_cast<size_t>(p.batch) * p.R * p.D, stream);
-  });
-}
-
-cudaError_t launch_wgmma_backward_key_value(const AttentionParams &p, const Sequences *seq, const Band *band,
-                                            cudaStream_t stream) {
-  if (cudaError_t e = check_backward(p)) return e;
-  const bool convert = p.prec[sdO] != p.prec[sQ];
-  const WgmmaPlan plan = plan_for(MFA_BACKWARD_KEY_VALUE, p, seq, band, convert);
+  const bool convert = p.prec[sdO] != p.prec[sQ], key_value = type == MFA_BACKWARD_KEY_VALUE;
+  const WgmmaPlan plan = wgmma_plan(type, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max, convert,
+                                    call, device_sm_count(current_device()));
   AttentionParams q = p;
+  cudaError_t e;
   if (plan.convert_dO_first) {
     const uint64_t elements = static_cast<uint64_t>(p.batch) * p.R * p.D;
     void *converted = nullptr;
-    cudaError_t e = workspace_for(current_device(), stream, elements * 2, &converted, /*slot=*/2);
-    if (e != cudaSuccess) return e;
-    if ((e = launch_bf16_to_f16(p.buf[sdO], converted, elements, stream)) != cudaSuccess) return e;
+    if ((e = workspace_for(current_device(), stream, elements * 2, &converted, /*slot=*/2)) != cudaSuccess ||
+        (e = launch_bf16_to_f16(p.buf[sdO], converted, elements, stream)) != cudaSuccess)
+      return e;
     q.buf[sdO] = converted;
     q.prec[sdO] = q.prec[sQ];
   }
-  return hop::dispatch(q, convert && !plan.convert_dO_first, [&](auto dch, auto bf16, auto cvt, auto causal) {
-    constexpr uint32_t DCH = decltype(dch)::value;
-    constexpr bool kBF16 = decltype(bf16)::value, kConvert = decltype(cvt)::value, kCausal = decltype(causal)::value;
-    if (band)
-      return hop::launch_backward<hop::KVCfg<DCH>>(
-          hop::band_backward_key_value_wgmma<DCH, kBF16, kConvert>,
-          hop::band_backward_key_value_packed_wgmma<DCH, kBF16, kConvert>, q, plan, seq, &hop::BwdArgs::dV,
-          &hop::BwdArgs::dK, static_cast<size_t>(q.batch / q.group) * q.C * q.D, stream, *band);
-    return hop::launch_backward<hop::KVCfg<DCH>>(
-        hop::attention_backward_key_value_wgmma<DCH, kBF16, kConvert, kCausal>,
-        hop::packed_backward_key_value_wgmma<DCH, kBF16, kConvert, kCausal>, q, plan, seq, &hop::BwdArgs::dV,
-        &hop::BwdArgs::dK, static_cast<size_t>(q.batch / q.group) * q.C * q.D,  // per K/V head
-        stream);
+  const hop::BackwardKernel kernel =
+      hop::dispatch(q, convert && !plan.convert_dO_first, [&](auto dch, auto bf16, auto cvt, auto causal) {
+        return hop::backward_kernel<decltype(dch)::value, decltype(bf16)::value, decltype(cvt)::value,
+                                    decltype(causal)::value>(type, call.seq, call.band);
+      });
+  hop::TensorMaps m;
+  if ((e = hop::prepare(kernel, plan.smem_bytes)) != cudaSuccess ||
+      (e = hop::make_maps(q, key_value ? plan.trav : plan.par, key_value ? plan.par : plan.trav, &m)) != cudaSuccess)
+    return e;
+  hop::BwdArgs a = hop::backward_args(q, plan);
+  const uint32_t outputs = key_value ? 2 : 1;
+  const size_t elems = key_value ? static_cast<size_t>(q.batch / q.group) * q.C * q.D
+                                 : static_cast<size_t>(q.batch) * q.R * q.D;
+  float *const out0 = key_value ? a.dV : a.dQ, *const out1 = key_value ? a.dK : nullptr;
+  float *part = nullptr;
+  if (plan.splits > 1) {
+    void *ws = nullptr;
+    const size_t bytes = plan.splits * outputs * elems * sizeof(float);
+    if ((e = workspace_for(current_device(), stream, bytes, &ws)) != cudaSuccess) return e;
+    part = static_cast<float *>(ws);
+    a.split_stride = outputs * elems;
+    (key_value ? a.dV : a.dQ) = part;
+    if (key_value) a.dK = part + elems;
+  }
+  kernel<<<plan.grid, plan.threads, plan.smem_bytes, stream>>>(m.Q, m.dO, m.K, m.V, a, call.seq ? *call.seq : Sequences{},
+                                                               call.band ? *call.band : Band{});
+  if ((e = cudaGetLastError()) != cudaSuccess || plan.splits == 1) return e;
+  const size_t quads = elems / 4;  // D % 8 == 0
+  hop::sum_splits<<<dim3(static_cast<uint32_t>((quads + 255) / 256), outputs), 256, 0, stream>>>(
+      reinterpret_cast<const float4 *>(part), reinterpret_cast<float4 *>(out0), reinterpret_cast<float4 *>(out1), quads,
+      a.split_stride / 4, plan.splits);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_wgmma(int type, const AttentionParams &p, const AttentionCall &call, cudaStream_t stream) {
+  if (type != MFA_FORWARD) return launch_backward(type, p, call, stream);
+  if (!row_major_16bit(p) || p.prec[sO] != FP32 || (call.fp8 && p.D % 16 != 0)) {
+    set_launch_detail(call.fp8 ? "descriptor is outside the FP8 K/V forward kernels' domain"
+                               : "descriptor is outside the wgmma forward kernel's domain");
+    return cudaErrorInvalidValue;
+  }
+  const WgmmaPlan plan = wgmma_plan(MFA_FORWARD, p.D, p.R, p.C, p.batch, p.group, p.split_min_blocks, p.split_max,
+                                    false, call, device_sm_count(current_device()));
+  return hop::dispatch(p, false, [&](auto dch, auto bf16, auto, auto causal) {
+    return hop::launch_forward<decltype(dch)::value, decltype(bf16)::value, decltype(causal)::value>(p, call, plan,
+                                                                                                      stream);
   });
 }
 

@@ -146,25 +146,26 @@ def run_case(mfa, torch, seed, timed, form, D, mode, causal, G, lowMid, transpos
         return paged.results()
 
 
-def dump(out_dir, timed, names):
+def dump(out_dir, timed, names, cases=CASES, run=run_case, functions=lambda case: instantiations(*case[:2], case[7]),
+         backend="simtFP32"):
+    """Runs `cases` through `run`, each of whose kernels must be on `backend`; functions(case): its entry functions"""
     import torch
     import mfa_b200 as mfa
     os.makedirs(out_dir, exist_ok=True)
     info = {"library": mfa.library_path(), "version": mfa.version(), "timed": timed, "cases": {}}
-    for i, (name, case) in enumerate(CASES.items()):
+    for i, (name, case) in enumerate(cases.items()):
         if names and name not in names:
             continue
         record = {}
         with recorded(mfa, torch, record, timed):
-            out = run_case(mfa, torch, 3000 + i, timed, *case)
-        bad = {kind: r["backend"] for kind, r in record.items() if r["backend"] != mfa.Backend.simtFP32.name}
+            out = run(mfa, torch, 3000 + i, timed, *case)
+        bad = {kind: r["backend"] for kind, r in record.items() if r["backend"] != backend}
         assert not bad and len(record) == (1 if case[0] == "paged" else 3), (name, record)
         if not timed:
             for key, array in out.items():
                 np.save(os.path.join(out_dir, f"{name}_{key}.npy"), array)
         digests = {key: hashlib.sha256(array.tobytes()).hexdigest() for key, array in out.items()}
-        info["cases"][name] = {"instantiations": instantiations(case[0], case[1], case[7]), "kernels": record,
-                               "outputs": digests}
+        info["cases"][name] = {"instantiations": functions(case), "kernels": record, "outputs": digests}
         print(name, json.dumps(record), flush=True)
     with open(os.path.join(out_dir, "shapes.json"), "w") as f:
         json.dump(info, f, indent=1)
@@ -209,18 +210,20 @@ def compare(a, b):
     return ok
 
 
-def main():
+def main(**cases):
+    """The command line; `cases`: dump's cases, run, functions and backend (default: the SIMT cases)"""
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", help="directory to write the arrays (with --time: the timings) to")
     ap.add_argument("--time", action="store_true", help="time each kernel type at a user's sizes; save digests only")
-    ap.add_argument("--case", action="append", choices=list(CASES), help="run only this case (repeatable)")
+    ap.add_argument("--case", action="append", choices=list(cases.get("cases", CASES)),
+                    help="run only this case (repeatable)")
     ap.add_argument("--compare", nargs=2, metavar=("DIR_A", "DIR_B"), help="compare the cases DIR_A holds")
     args = ap.parse_args()
     if args.compare:
         sys.exit(0 if compare(*args.compare) else 1)
     if not args.out:
         ap.error("--out or --compare is required")
-    dump(args.out, args.time, args.case)
+    dump(args.out, args.time, args.case, **cases)
 
 
 if __name__ == "__main__":

@@ -6,7 +6,8 @@
 Both trees compile the kernel sources in SOURCES through the library's Makefile, with the build's flags, into
 temporary directories; nothing in the repository is written.  A source the base does not have is compiled from the
 working tree alone and its functions are listed as new.  Functions are matched by their demangled name without the
-parameter list (cu++filt), so that a kernel whose arguments moved into a struct is still compared with itself.  The script
+parameter list (cu++filt), so that a kernel whose arguments moved into a struct is still compared with itself, and their
+SASS with runs of spaces collapsed, since cuobjdump pads every line to the widest instruction of the file.  The script
 prints every function whose SASS is not byte-identical, with its instruction count before and after, and fails (exit
 status 1) when a function appears or disappears, or when anything ptxas -v reports differs from the base: a function's
 registers, barriers, shared and constant memory, stack frame, spills or diagnostics (counted by code), or the
@@ -63,7 +64,7 @@ def keys(names):
 
 
 def sass(obj):
-    """{function key: SASS text} of an object file"""
+    """{function key: SASS text} of an object file, runs of spaces collapsed"""
     text = anonymous(subprocess.check_output([CUOBJDUMP, "-sass", obj], text=True))
     funcs, name = {}, None
     for line in text.splitlines():
@@ -72,7 +73,7 @@ def sass(obj):
             name = m.group(1)
             funcs[name] = []
         elif name is not None:
-            funcs[name].append(line)
+            funcs[name].append(re.sub(" +", " ", line))  # (cuobjdump pads to the widest line of the whole file)
     key = keys(funcs)
     return {key[name]: "\n".join(lines) for name, lines in funcs.items()}
 

@@ -43,9 +43,12 @@ def test_ptxas_serializes_no_wgmma():
 
 def test_tensor_core_kernels_have_no_spills_and_no_stack_frame():
     report, _ = _ptxas_report()
-    kernels = {name: r for name, r in report.items() if re.search(r"attention_\w+_wgmma", name)}
-    # forward, dQ and dK/dV: 3 head-dimension chunk counts x their type / mask / dO-conversion instantiations
-    assert len(kernels) == 48, sorted(kernels)
+    # every entry function (mangled "<name>_wgmmaI<template arguments>"): the forward's call forms, and the dQ and dK/dV
+    # kernels, of which several sit within a few registers of the limit
+    kernels = {name: r for name, r in report.items() if re.search(r"_wgmmaI", name)}
+    # 3 head-dimension chunk counts x each form's type / mask / dO-conversion instantiations
+    assert len(kernels) == 216, sorted(kernels)
+    assert len([name for name in kernels if "backward" in name]) == 108, sorted(kernels)
     bad = {name: r for name, r in kernels.items() if r != (0, 0, 0)}
     assert not bad, "stack frame / spill stores / spill loads (bytes): " + repr(bad)
 

@@ -249,10 +249,13 @@ def test_launch_count_is_what_encode_launches(R, C, D, batch, transposes, bf16, 
     kernel.encode(c, ptrs)                 # first encode: workspaces and shared-memory opt-ins
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        # the trace can miss the first kernel of the window: a torch kernel goes first, and only the library's count
+        bufs[Op.L].add_(0.0)
+        torch.cuda.synchronize()
         kernel.encode(c, ptrs)
         torch.cuda.synchronize()
     launched = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-                and not e.name.startswith(("Memcpy", "Memset"))]
+                and "mfa::" in e.name]
     assert len(launched) == kernel.launchCount(c), launched
 
 
