@@ -229,9 +229,24 @@ LAUNCH_COUNT_CASES = [  # (R, C, D, batch, transposes, bf16, kernel type)
 @pytest.mark.gpu
 @pytest.mark.parametrize("R,C,D,batch,transposes,bf16,t", LAUNCH_COUNT_CASES)
 def test_launch_count_is_what_encode_launches(R, C, D, batch, transposes, bf16, t):
-    """launchCount against the CUDA kernels a torch.profiler trace of one encode() records."""
+    """launchCount against the CUDA kernels a torch.profiler trace of one encode() records, in a process of its own
+    (as the split and packed suites trace theirs): a trace in the pytest process recorded no kernel at all once GPU
+    work of other processes had run between an earlier profiler session of the session and it."""
+    import json
+    args = (R, C, D, batch, tuple(transposes), bf16, int(t))
+    code = f"import json, sys; sys.path.insert(0, {ROOT!r}); from tests.test_host_api import _trace_launches; " \
+           f"print(json.dumps(_trace_launches(*{args!r})))"
+    proc = subprocess.run([sys.executable, "-c", code], cwd=ROOT, capture_output=True, text=True, timeout=600)
+    assert proc.returncode == 0, proc.stderr[-4000:]
+    launched, count = json.loads(proc.stdout.strip().splitlines()[-1])
+    assert len(launched) == count, launched
+
+
+def _trace_launches(R, C, D, batch, transposes, bf16, t):
+    """(the library's kernels a torch.profiler trace of one encode records, launchCount)"""
     import torch
     from torch.profiler import ProfilerActivity, profile
+    t = KT(t)
     d = make(R, C, D, lowIn=True, transposes=transposes, bf16=bf16)
     d.batchCount = batch
     c = mfa.FunctionConstantValues()
@@ -256,7 +271,7 @@ def test_launch_count_is_what_encode_launches(R, C, D, batch, transposes, bf16, 
         torch.cuda.synchronize()
     launched = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
                 and "mfa::" in e.name]
-    assert len(launched) == kernel.launchCount(c), launched
+    return launched, kernel.launchCount(c)
 
 
 def test_invalid_precision_pairs_are_rejected():
